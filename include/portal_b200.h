@@ -101,7 +101,8 @@ PE_API int pe_scene_uniform_block(pe_ctx* ctx, int width, int height, const void
  * "min_blocks", "hoist_planes" (0/1, default 1: per-plane normal algebra evaluated once per upload on the
  * host), "lazy_planes" (0/1, default 1: a plane test stops as soon as its result is certain to be
  * rejected, same pixels), "with_probe" (0/1, default 0: also generate the camera-teleportation probe kernel; pe_probe_ray
- * switches it on by itself), "adaptive" (0/1, default 1: an int uniform or a matrix structure that differed between
+ * switches it on by itself), "with_refine" (0/1, default 0: also generate pe_refine_kernel; pe_render_adaptive switches it
+ * on by itself), "adaptive" (0/1, default 1: an int uniform or a matrix structure that differed between
  * renders more than 4 times stops being a specialisation constant, which bounds recompilation when an animation
  * drives it), "uniforms_in_smem" (0 = constant bank (default), 1 = every block copies the uniform block into
  * shared memory with a cooperative loop, 2 = with one TMA bulk copy + mbarrier; same pixels, measured in DESIGN.md section 3),
@@ -172,6 +173,23 @@ PE_API int pe_host_unregister(pe_ctx* ctx, void* p);
 /* Page-locked host memory for the readback calls. */
 PE_API int pe_host_malloc(pe_ctx* ctx, size_t bytes, void** out);
 PE_API int pe_host_free(pe_ctx* ctx, void* p);
+/* Adaptive anti-aliasing (opt-in; no counterpart in the reference): trace all `_aa_count` samples only where a one-sample
+ * frame has an edge.  With N = `_aa_count`, a = `_aa_start` and T = `threshold`:
+ *   1. F1 = the frame rendered with the single sample a, written to `out_device`: bit-identical to pe_render / pe_render_rgba8
+ *      with `_aa_count` = 1 (the override is restored afterwards and is not a uniform change for re-specialisation).
+ *   2. Mask: Q(p) = the unorm8 r, g, b of F1 at pixel p (an RGBA8 frame's bytes; a float frame quantised exactly as
+ *      pe_quantize_rgba8 does).  p is refined iff, for some channel, max - min of Q over p's 3x3 neighbourhood (clipped to
+ *      the frame) is > T.  T < 0 refines every pixel, T >= 255 none.
+ *   3. Every refined pixel is overwritten with exactly what pe_render with `_aa_count` = N writes there (samples a .. a+N-1,
+ *      summed in that order, sqrt(sum / N)); the others keep their F1 value.
+ * So  adaptive(T) == where(mask_T(F1), F_N, F1)  bit for bit; T < 0 gives F_N, T = 255 gives F1, N = 1 gives pe_render.
+ * `rgba8` selects the output format of `out_device` (0: float RGBA, 16 B/pixel; 1: RGBA8).  `refined_count_device`
+ * (optional, device uint32) receives the number of refined pixels.  Enqueues three kernel launches on `stream` (NULL: the
+ * context's stream) and returns without synchronising.  Only whole-frame targets ({w, h, h, 0, 1, 1, layout}) are accepted;
+ * n_strips == 0 renders nothing and succeeds.  The pixel list lives in context scratch slots 123 and 124 (pe_scratch_buffer).
+ * The first call for a scene compiles a second program (the render program plus pe_refine_kernel, option "with_refine"). */
+PE_API int pe_render_adaptive(pe_ctx* ctx, const pe_target* target, int threshold, int rgba8, void* out_device,
+                              void* refined_count_device, void* stream);
 /* Camera-teleportation probe (replaces teleport_external_ray, src/main.rs:1361-1409 +
  * src/frag.glsl:166-257, 527-547): follow the segment a -> b through the scene's portals (at most
  * 10, `teleport_light_u` forced on) and return where its end point lands -- directly, instead of

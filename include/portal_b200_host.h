@@ -178,6 +178,11 @@ PE_API int ph_player_render_frame(ph_player* pl, pe_ctx* ctx, const ph_frame_par
 PE_API int ph_player_render_motion_blur_frame(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index,
                                               int frame_count, int motion_blur_frames, double duration_seconds,
                                               uint8_t* out_host_rgba8);
+/* Adaptive anti-aliasing for the player's frames (off by default): when on, ph_player_render_frame and every sub-frame of
+ * ph_player_render_motion_blur_frame (before the unchanged gamma-2 average) are rendered by pe_render_adaptive with
+ * `threshold` -- one sample everywhere, all aa_count samples where the one-sample frame has an edge.  ph_player_render_frame
+ * then stages the frame in the context's scratch slot 0.  The scene-level ph_render_* functions are not affected. */
+PE_API int ph_player_set_adaptive_aa(ph_player* pl, int on, int threshold);
 
 /* ---- image files either side of the path ------------------------------------------------------------------------
  * Textures reach the reference as PNG files (Texture2D::from_file_with_format, src/main.rs:1066-1085) and frames leave it as

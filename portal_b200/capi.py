@@ -88,6 +88,7 @@ def lib() -> C.CDLL:
         "pe_host_unregister": (i32, [vp, vp]),
         "pe_host_malloc": (i32, [vp, C.c_size_t, C.POINTER(vp)]),
         "pe_host_free": (i32, [vp, vp]),
+        "pe_render_adaptive": (i32, [vp, C.POINTER(PeTarget), i32, i32, vp, vp, vp]),
         "pe_probe_ray": (i32, [vp, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_int32),
                                C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
         "pe_autotune": (i32, [vp, C.POINTER(PeTarget), i32, cp, C.c_size_t]),
@@ -172,6 +173,7 @@ def lib() -> C.CDLL:
         "ph_scene_camera_name": (i32, [vp, i32, C.POINTER(cp)]),
         "ph_player_render_frame": (i32, [vp, vp, C.POINTER(PhFrameParams), vp, i32]),
         "ph_player_render_motion_blur_frame": (i32, [vp, vp, C.POINTER(PhFrameParams), i32, i32, i32, C.c_double, vp]),
+        "ph_player_set_adaptive_aa": (i32, [vp, i32, i32]),
     })
     for name, (res, args) in sig.items():
         fn = getattr(L, name)

@@ -325,9 +325,9 @@ PE_FI unsigned unorm8(float v) {
     return (unsigned)__float2int_rn(v * 255.0f);
 }
 
-PE_FI void store_pixel(const PeLaunch& L, int px, int lrow, int grow, vec3 sum, int bounces) {
-    // frag.glsl:526, :551: sqrt(result / aa_count), alpha 1
-    vec3 c = sqrt(sum / float(_aa_count));
+PE_FI void store_pixel(const PeLaunch& L, int px, int lrow, int grow, vec3 sum, int bounces, int divisor) {
+    // frag.glsl:526, :551: sqrt(result / aa_count), alpha 1; `divisor` is the number of samples in `sum`
+    vec3 c = sqrt(sum / float(divisor));
     size_t idx = size_t(L.out_full_frame ? grow : lrow) * size_t(L.width) + size_t(px);
     if (L.out_rgba8) {
         // GL float -> unorm8: clamp to [0,1] (NaN -> 0), scale by 255, round to nearest even;
@@ -462,7 +462,10 @@ extern "C" __global__ void pe_probe_kernel(const PeProbe P) {
 #define PE_BLOCK_W (PE_TILE_W < 16 ? 16 : PE_TILE_W)                                   /* pixels across a block */
 #define PE_BLOCK_ROWS ((PE_BLOCK_THREADS / 32) / (PE_BLOCK_W / PE_TILE_W) * (32 / PE_TILE_W)) /* rows of a block */
 
-#if !PE_PERSISTENT
+#ifndef PE_WITH_REFINE
+#define PE_WITH_REFINE 0
+#endif
+#if !PE_PERSISTENT || PE_WITH_REFINE
 namespace pe {
 // One view of one AA sample: get_color2 (frag.glsl:408-464).
 PE_FI vec3 trace_view(int px, int grow, int a, int eye, int& worst) {
@@ -479,19 +482,10 @@ PE_FI vec3 trace_view(int px, int grow, int a, int eye, int& worst) {
     worst = pe::max(worst, s.bounce);
     return c;
 }
-}  // namespace pe
-// ------------------------------------------------------------------------------------------
-// One thread per pixel.  Block = W warps = a PE_BLOCK_W x PE_BLOCK_ROWS pixel tile (8x4 warp tiles: two abreast).
-extern "C" __global__ void __launch_bounds__(PE_BLOCK_THREADS, PE_MIN_BLOCKS) pe_render_kernel(const PeLaunch L) {
-    using namespace pe;
-    PE_STAGE_UNIFORMS();
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int warps_x = PE_BLOCK_W / PE_TILE_W;
-    const int px = blockIdx.x * PE_BLOCK_W + (warp % warps_x) * PE_TILE_W + (lane % PE_TILE_W);
-    const int lrow = blockIdx.y * PE_BLOCK_ROWS + (warp / warps_x) * (32 / PE_TILE_W) + (lane / PE_TILE_W);
-    int grow;
-    if (px >= L.width || !local_to_global_row(L, lrow, grow)) return;
 
+// Every AA sample of one pixel, summed in sample order, and its store: the body of the one-thread-per-pixel render kernel
+// and of the refine kernel, so a refined pixel is exactly the pixel a render with the same `_aa_count` writes.
+PE_FI void render_pixel(const PeLaunch& L, int px, int lrow, int grow) {
     vec3 sum = vec3(0.0f);
     int worst = 0;
     for (int a = _aa_start; a < _aa_count + _aa_start; a++) {  // frag.glsl:522-525
@@ -503,7 +497,59 @@ extern "C" __global__ void __launch_bounds__(PE_BLOCK_THREADS, PE_MIN_BLOCKS) pe
             sum += trace_view(px, grow, a, 0, worst);
         }
     }
-    store_pixel(L, px, lrow, grow, sum, worst);
+    store_pixel(L, px, lrow, grow, sum, worst, _aa_count);
+}
+}  // namespace pe
+#endif
+
+#if PE_WITH_REFINE
+// Adaptive anti-aliasing, second pass (pe_render_adaptive): re-render the pixels of a list with all `_aa_count` samples.
+// The list (packed (y << 16) | x, whole-frame coordinates) and its length come from pe_k_refine_list (pe_kernels.cu).
+struct PeRefine {
+    PeLaunch L;              // whole-frame target: local row == global row
+    const unsigned* list;
+    unsigned* count;         // [0] list length, [1] refill cursor (zeroed by the host before the list is built)
+};
+namespace pe {
+// List entry i: all samples of its pixel, stored over the one-sample value
+PE_FI void refine_entry(const PeRefine& R, unsigned i) {
+    const unsigned p = R.list[i];
+    const int px = int(p & 0xffffu), y = int(p >> 16);
+    render_pixel(R.L, px, y, y);
+}
+}  // namespace pe
+// Warp refill from an atomic cursor, as in the persistent scheduler: a warp takes the next 32 list entries when all of its
+// lanes are done, so warps that drew short rays keep taking work while others finish long portal chains.  Against a
+// grid-stride loop over the same grid (H100, 4K, aa 4): 17 % faster on mobius_monoportal, whose edge pixels run the Newton
+// solver for very different times; within +-0.05 ms on the other config scenes (BASELINE.md section 5).
+extern "C" __global__ void __launch_bounds__(PE_BLOCK_THREADS, PE_MIN_BLOCKS) pe_refine_kernel(const PeRefine R) {
+    using namespace pe;
+    PE_STAGE_UNIFORMS();
+    const unsigned n = R.count[0];
+    const int lane = threadIdx.x & 31;
+    while (true) {
+        unsigned base = 0;
+        if (lane == 0) base = atomicAdd(R.count + 1, 32u);
+        base = __shfl_sync(0xffffffffu, base, 0);
+        if (base >= n) return;
+        if (base + unsigned(lane) < n) refine_entry(R, base + unsigned(lane));
+    }
+}
+#endif
+
+#if !PE_PERSISTENT
+// ------------------------------------------------------------------------------------------
+// One thread per pixel.  Block = W warps = a PE_BLOCK_W x PE_BLOCK_ROWS pixel tile (8x4 warp tiles: two abreast).
+extern "C" __global__ void __launch_bounds__(PE_BLOCK_THREADS, PE_MIN_BLOCKS) pe_render_kernel(const PeLaunch L) {
+    using namespace pe;
+    PE_STAGE_UNIFORMS();
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int warps_x = PE_BLOCK_W / PE_TILE_W;
+    const int px = blockIdx.x * PE_BLOCK_W + (warp % warps_x) * PE_TILE_W + (lane % PE_TILE_W);
+    const int lrow = blockIdx.y * PE_BLOCK_ROWS + (warp / warps_x) * (32 / PE_TILE_W) + (lane / PE_TILE_W);
+    int grow;
+    if (px >= L.width || !local_to_global_row(L, lrow, grow)) return;
+    render_pixel(L, px, lrow, grow);
 }
 #else
 // ------------------------------------------------------------------------------------------
@@ -603,7 +649,7 @@ extern "C" __global__ void __launch_bounds__(PE_BLOCK_THREADS, PE_MIN_BLOCKS) pe
                     eye = first_eye;
                     skip = !primary_ray(px, grow, a, eye, s);   // next AA sample of the same pixel (may fall outside a 360 / VR180 image)
                 } else {
-                    store_pixel(L, px, lrow, grow, sum, worst);
+                    store_pixel(L, px, lrow, grow, sum, worst, _aa_count);
                     alive = false;
                 }
             }

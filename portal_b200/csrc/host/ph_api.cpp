@@ -28,6 +28,8 @@ struct ph_player {
     std::string err;
     ph_update_hook hook = nullptr;      // the caller's per-update work (video frames): SceneRenderer::update's tail, main.rs:1536-1542
     void* hook_user = nullptr;
+    bool adaptive_aa = false;           // ph_player_set_adaptive_aa: frames go through pe_render_adaptive
+    int adaptive_threshold = 8;
     explicit ph_player(ph_scene* sc) : s(sc), player(sc->scene) {}
 };
 
@@ -565,8 +567,24 @@ int ph_player_render_frame(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p,
     if (upload_renderer_uniforms_cam(pl->s, ctx, p, c.get_matrix(), c.teleport_matrix, c.in_subspace)) return pfail(pl, pl->s->err);
     if (upload_stereo_uniforms(pl, ctx)) return 1;
     pe_target t = {p->width, p->height, p->height, 0, 1, 1, 1};
-    int rc = rgba8 ? pe_render_host_rgba8(ctx, &t, (uint8_t*)out_host) : pe_render_host(ctx, &t, (float*)out_host);
+    int rc;
+    if (pl->adaptive_aa) {
+        // the frame lands in scratch slot 0 (reused by every frame) and is read back from there
+        const size_t bytes = size_t(p->width) * size_t(p->height) * (rgba8 ? 4 : 16);
+        void* dev = nullptr;
+        rc = pe_scratch_buffer(ctx, 0, bytes, &dev) || pe_render_adaptive(ctx, &t, pl->adaptive_threshold, rgba8, dev, nullptr, nullptr) ||
+             pe_memcpy_d2h(ctx, out_host, dev, bytes, nullptr);
+    } else {
+        rc = rgba8 ? pe_render_host_rgba8(ctx, &t, (uint8_t*)out_host) : pe_render_host(ctx, &t, (float*)out_host);
+    }
     if (rc) return pfail(pl, std::string("render failed: ") + pe_last_error(ctx));
+    return 0;
+}
+
+int ph_player_set_adaptive_aa(ph_player* pl, int on, int threshold) {
+    if (!pl) return 1;
+    pl->adaptive_aa = on != 0;
+    pl->adaptive_threshold = threshold;
     return 0;
 }
 
@@ -595,7 +613,8 @@ int ph_player_render_motion_blur_frame(ph_player* pl, pe_ctx* ctx, const ph_fram
             rc = 1;
         } else if (upload_stereo_uniforms(pl, ctx)) {
             rc = 1;
-        } else if (pe_render_rgba8(ctx, &t, sub[size_t(j)], nullptr)) {
+        } else if (pl->adaptive_aa ? pe_render_adaptive(ctx, &t, pl->adaptive_threshold, 1, sub[size_t(j)], nullptr, nullptr)
+                                   : pe_render_rgba8(ctx, &t, sub[size_t(j)], nullptr)) {
             pl->err = std::string("render failed: ") + pe_last_error(ctx);
             rc = 1;
         }

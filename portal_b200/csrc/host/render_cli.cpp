@@ -4,12 +4,16 @@
 //   portal_b200_render render-frame <scene.ron> [--width W] [--height H] [--render-depth D] [--aa-count N]
 //                      [--time T] [--stage NAME] [--animation NAME] [--camera NAME] [--device K]
 //                      [--texture name=file.png | name=file.rgba:WxH ...] [--assets DIR] [--output out.png|.ppm|.rgba]
+//                      [--adaptive-aa T]
 //   portal_b200_render render <scene.ron> [--animations a,b,... | --starts-with PREFIX] [--fps N] [--motion-blur-frames M] [--width W]
 //                      [--height H] [--render-depth D] [--aa-count N] [--stereo-image] [--no-skip-existing] [--out-dir DIR] [--max-frames K]
-//                      [--frame-format ppm|png|rgba] [--assets DIR]
+//                      [--frame-format ppm|png|rgba] [--assets DIR] [--adaptive-aa T]
 //                      (`portal render`, main.rs:2808-2873 -> render_named_animations :1876-1930 ->
 //                       render_animation :1757-1830; frames are written as DIR/<animation>/frame_<i>.<format>, the
 //                       ffmpeg step is out of scope)
+//
+// --adaptive-aa T (not in the reference; off by default): every frame / sub-frame is traced with one sample, and with all
+// --aa-count samples only where that frame has an edge (a 3x3 unorm8 range above T, pe_render_adaptive).
 //
 // Output: the RGBA8 frame the reference hands to export_png (main.rs:2939-2943) as a PNG when the name ends in .png
 // (ph_png_encode_rgba8), as raw RGBA8 for .rgba, else as a binary PPM (P6, alpha dropped).  Textures: every texture of the
@@ -145,16 +149,17 @@ int main(int argc, char** argv) {
     const bool anim_cmd = argc >= 3 && std::strcmp(argv[1], "render") == 0;
     if (!frame_cmd && !anim_cmd) {
         std::fprintf(stderr, "usage: %s render-frame <scene.ron> [--width W] [--height H] [--render-depth D] [--aa-count N] [--time T] "
-                             "[--stage NAME] [--animation NAME] [--camera NAME] [--device K] [--texture name=file.png|name=file.rgba:WxH] [--assets DIR] [--output out.png|.ppm|.rgba]\n"
+                             "[--stage NAME] [--animation NAME] [--camera NAME] [--device K] [--texture name=file.png|name=file.rgba:WxH] [--assets DIR] [--output out.png|.ppm|.rgba] [--adaptive-aa T]\n"
                              "       %s render <scene.ron> [a,b | --animations a,b | --starts-with PREFIX] [--fps N] [--motion-blur-frames M] [--width W] [--height H] "
-                             "[--render-depth D] [--aa-count N] [--stereo-image] [--no-skip-existing] [--out-dir DIR] [--max-frames K]\n", argv[0], argv[0]);
+                             "[--render-depth D] [--aa-count N] [--stereo-image] [--no-skip-existing] [--out-dir DIR] [--max-frames K] [--adaptive-aa T]\n", argv[0], argv[0]);
         return 2;
     }
     std::string scene_path = argv[2], output = "frame.ppm", out_dir = "video";
     // defaults of RenderFrameCliOptions (main.rs:2744-2754) / RenderCliOptions (main.rs:2764-2803)
     int width = frame_cmd ? 1920 : 3840, height = frame_cmd ? 1080 : 2160, depth = frame_cmd ? 100 : 150, aa = frame_cmd ? 1 : 4, device = 0;
     int fps = 60, motion_blur = 1, max_frames = -1;
-    bool stereo = false, skip_existing = true;
+    bool stereo = false, skip_existing = true, adaptive = false;
+    int adaptive_threshold = 0;
     double time = 0.0;
     std::vector<std::string> textures;
     std::string stage, animation, camera, animations, starts_with, assets, frame_ext = ".ppm";
@@ -184,6 +189,14 @@ int main(int argc, char** argv) {
         else if (a == "--texture") textures.push_back(next());
         else if (a == "--assets") assets = next();
         else if (a == "--frame-format") frame_ext = std::string(".") + next();          // render: ppm (default) | png | rgba
+        else if (a == "--adaptive-aa" || a == "--adaptive_aa") {
+            const char* v = next();
+            char* end = nullptr;
+            const long t = std::strtol(v, &end, 10);
+            if (!*v || *end) { std::fprintf(stderr, "--adaptive-aa needs an integer threshold, got `%s`\n", v); return 2; }
+            adaptive = true;
+            adaptive_threshold = int(std::max(-1L, std::min(t, 255L)));
+        }
         else { std::fprintf(stderr, "unknown option %s\n", a.c_str()); return 2; }
     }
     bool ok = false;
@@ -195,6 +208,7 @@ int main(int argc, char** argv) {
     pe_ctx* ctx = pe_create(device);
     if (!ctx) { std::fprintf(stderr, "pe_create: %s\n", pe_last_error(nullptr)); return 1; }
     ph_player* player = ph_player_new(scene);
+    if (adaptive) ph_player_set_adaptive_aa(player, 1, adaptive_threshold);
     if (frame_cmd) {  // main.rs:2900-2926
         if (!stage.empty() && ph_player_init_stage(player, stage.c_str())) {
             std::fprintf(stderr, "Scene `%s` has no stage named `%s`\n", scene_path.c_str(), stage.c_str());

@@ -53,6 +53,8 @@ struct Variant {
     CUmodule_t module = nullptr;
     CUfunction_t kernel = nullptr;
     CUfunction_t probe = nullptr;
+    CUfunction_t refine = nullptr;   // pe_refine_kernel (programs generated with_refine)
+    int refine_blocks_per_sm = 1;
     CUdeviceptr_t const_ptr = 0;
     size_t const_size = 0;
     int regs = 0;
@@ -327,6 +329,7 @@ std::vector<int> variant_key(pe_ctx* c, const std::vector<int>& ints, const std:
     if (c->opts.specialize_matrices)
         for (auto& zo : masks) { key.push_back(int(zo.first)); key.push_back(int(zo.second)); }
     key.push_back(c->opts.with_probe ? 1 : 0);
+    key.push_back(c->opts.with_refine ? 1 : 0);
     key.push_back(c->opts.uniforms_in_smem);
     key.push_back(c->opts.tile_w);
     key.push_back(c->opts.canon_rays ? 1 : 0);
@@ -523,6 +526,13 @@ bool select_variant(pe_ctx* c) {
         if (c->opts.with_probe) {
             r = d->cuModuleGetFunction(&v->probe, v->module, "pe_probe_kernel");
             if (r != 0) { c->err = "cuModuleGetFunction(pe_probe_kernel): " + driver_error(d, r); return false; }
+        }
+        if (c->opts.with_refine) {
+            r = d->cuModuleGetFunction(&v->refine, v->module, "pe_refine_kernel");
+            if (r != 0) { c->err = "cuModuleGetFunction(pe_refine_kernel): " + driver_error(d, r); return false; }
+            int nb = 1;
+            if (d->cuOccupancyMaxActiveBlocksPerMultiprocessor(&nb, v->refine, c->opts.block_threads, 0) == 0 && nb > 0)
+                v->refine_blocks_per_sm = nb;
         }
         d->cuFuncGetAttribute(&v->regs, 4 /*CU_FUNC_ATTRIBUTE_NUM_REGS*/, v->kernel);
         int nb = 1;
@@ -802,6 +812,7 @@ int pe_set_option(pe_ctx* c, const char* key, int value) {
     else if (k == "hoist_planes") c->opts.hoist_planes = value != 0;
     else if (k == "lazy_planes") c->opts.lazy_planes = value != 0;
     else if (k == "with_probe") c->opts.with_probe = value != 0;   // pe_probe_ray turns it on by itself; exposed for inspection
+    else if (k == "with_refine") c->opts.with_refine = value != 0; // pe_render_adaptive turns it on by itself; likewise
     else if (k == "adaptive") c->adapt = value != 0;
     else if (k == "canon_rays") c->opts.canon_rays = value != 0;
     else if (k == "w_aware") c->opts.w_aware = value != 0;
@@ -1093,6 +1104,77 @@ int pe_probe_ray(pe_ctx* c, const float a[3], const float b[3], float pos_out[3]
     if (have_result) *have_result = host[3] != 0.0f;
     if (encounter_object) *encounter_object = host[4] != 0.0f;
     if (change_subspace) *change_subspace = host[5] != 0.0f;
+    return 0;
+}
+
+// Adaptive anti-aliasing: a one-sample frame, the list of its edge pixels, and every listed pixel rendered again with all
+// `_aa_count` samples by the program's pe_refine_kernel (the render kernel's own per-pixel code).
+int pe_render_adaptive(pe_ctx* c, const pe_target* t, int threshold, int rgba8, void* out_device, void* refined_count_device,
+                       void* stream) {
+    if (!c) return 1;
+    if (!out_device) return c->fail("pe_render_adaptive: out_device is null");
+    if (!check_target(c, t) || !bind_device(c)) return 1;
+    if (t->n_strips == 0) return 0;   // nothing of this frame belongs to the caller
+    if (t->strip_first != 0 || t->n_strips != 1 || t->strip_rows < t->height)
+        return c->fail("pe_render_adaptive: only whole-frame targets ({w, h, h, 0, 1, 1, layout}) are supported -- the 3x3 edge "
+                       "window of a pixel crosses strip boundaries");
+    ensure_layout(c);
+    const int aa_slot = c->layout.int_slot["_aa_count"];
+    const int n_aa = *islot(c, aa_slot);
+    CUstream_t s = stream ? (CUstream_t)stream : (CUstream_t)c->stream;
+
+    // (1) the one-sample frame, straight into the caller's buffer: exactly pe_render(_rgba8) with `_aa_count` = 1.  The
+    // override is not a scene change for the specialisation tracker (as `teleport_light_u` in pe_probe_ray).
+    *islot(c, aa_slot) = 1;
+    const bool had_adapt = c->adapt;
+    c->adapt = false;
+    int rc = render_impl(c, t, out_device, nullptr, s, rgba8 != 0);
+    c->adapt = had_adapt;
+    *islot(c, aa_slot) = n_aa;
+    if (rc) return 1;
+
+    // (2) the list of pixels to refine: count + refill cursor in scratch slot 124, packed pixel indices in slot 123
+    const size_t n_px = size_t(t->width) * size_t(t->height);
+    void *list = nullptr, *counter = nullptr;
+    if (pe_scratch_buffer(c, 123, n_px * 4, &list) || pe_scratch_buffer(c, 124, 16, &counter)) return 1;
+    if (!cuda_ok(c, cudaMemsetAsync(counter, 0, 16, (cudaStream_t)s), "pe_render_adaptive: counter reset")) return 1;
+    if (!cuda_ok(c, (cudaError_t)launch_refine_list(out_device, rgba8 != 0, t->width, t->height, threshold, (unsigned*)list,
+                                                    (unsigned*)counter, (cudaStream_t)s), "pe_render_adaptive: refine list"))
+        return 1;
+    c->launches++;
+    if (refined_count_device &&
+        !cuda_ok(c, cudaMemcpyAsync(refined_count_device, counter, 4, cudaMemcpyDeviceToDevice, (cudaStream_t)s), "refined count copy"))
+        return 1;
+
+    // (3) the refine pass: the same program with pe_refine_kernel, `_aa_count` = N
+    const bool had_refine = c->opts.with_refine;
+    c->opts.with_refine = true;
+    const bool ok = select_variant(c);
+    c->opts.with_refine = had_refine;
+    if (!ok) return 1;
+    update_derived(c);
+    Variant* v = c->current;
+    if (!upload_uniform_block(c, v->const_ptr, s)) return 1;
+    struct { PeLaunchHost L; const void* list; void* count; } R;
+    std::memset(&R, 0, sizeof R);
+    R.L.out = out_device;
+    R.L.width = t->width;
+    R.L.height = t->height;
+    R.L.strip_rows = t->strip_rows;
+    R.L.strip_step = t->strip_step;
+    R.L.n_strips = 1;
+    R.L.out_full_frame = 1;
+    R.L.tiles_x = (t->width + 7) / 8;
+    R.L.tiles_y = (t->height + 3) / 4;
+    R.L.out_rgba8 = rgba8 ? 1 : 0;
+    R.L.strip_shift = -1;
+    R.list = list;
+    R.count = counter;
+    void* args[] = {&R};
+    const unsigned gx = unsigned(c->sm_count * v->refine_blocks_per_sm);
+    CUresult_t r = c->drv->cuLaunchKernel(v->refine, gx, 1, 1, unsigned(c->opts.block_threads), 1, 1, 0, s, args, nullptr);
+    if (r != 0) return c->fail("cuLaunchKernel(pe_refine_kernel): " + driver_error(c->drv, r));
+    c->launches++;
     return 0;
 }
 

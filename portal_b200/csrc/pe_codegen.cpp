@@ -540,6 +540,8 @@ GenResult generate_program(const SceneDesc& scene, const ConstLayout& L, const G
     hd << "#define PE_BLOCK_THREADS " << opts.block_threads << "\n";
     hd << "#define PE_MIN_BLOCKS " << opts.min_blocks << "\n";
     hd << "#define PE_WITH_PROBE " << (opts.with_probe ? 1 : 0) << "\n";
+    // emitted only when on, so every other program's source -- and its entry in the on-disk cubin cache -- stays as it was
+    if (opts.with_refine) hd << "#define PE_WITH_REFINE 1\n";
     hd << "#define PE_TILE_W " << opts.tile_w << "\n";
     hd << "#define PE_CANON_RAYS " << (opts.canon_rays ? 1 : 0) << "\n";
     hd << "#define PE_W_AWARE " << ((opts.w_aware && opts.canon_rays) ? 1 : 0) << "\n";

@@ -95,6 +95,7 @@ struct GenOptions {
     bool hoist_planes = true;  // per-plane normal work evaluated on the host (see PlaneRec)
     bool lazy_planes = true;   // with hoist_planes: plane tests stop as soon as nearer() is certain to reject them
     bool with_probe = false;  // also emit pe_probe_kernel (camera-teleportation probe)
+    bool with_refine = false;  // also emit pe_refine_kernel (second pass of adaptive anti-aliasing, pe_render_adaptive)
     // Uniform block staged in shared memory: every block copies the constant block to a __shared__ image in its prologue
     // and the program reads uniforms from there (LDS operands) instead of the constant bank (LDCU / UR operands).  What
     // north_star sketches; off by default, see DESIGN.md sections 3 and 10.

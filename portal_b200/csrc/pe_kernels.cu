@@ -201,10 +201,57 @@ __global__ void __launch_bounds__(256) pe_k_count_diff(const uint4* __restrict__
     if ((threadIdx.x & 31) == 0 && mine) atomicAdd(count, mine);
 }
 
+// Adaptive anti-aliasing edge mask (pe_render_adaptive).  Q = the unorm8 r, g, b of the one-sample frame (RGBA8 bytes, or
+// the float frame quantised as pe_k_quantize_rgba8 does); a pixel is refined when, for some channel, max - min of Q over its
+// 3x3 neighbourhood clipped to the frame exceeds `threshold`.  One warp per 8x4 tile: the tile's refined pixels are balloted,
+// lane 0 reserves their list slots with one atomicAdd, and they are written in tile order (lane order), so the refine pass's
+// warps start on neighbouring pixels.  The order of tiles in the list depends on scheduling; the set does not.
+template <bool RGBA8>
+__global__ void __launch_bounds__(256) pe_k_refine_list(const void* __restrict__ frame, int width, int height, int tiles_x,
+                                                        unsigned n_tiles, int threshold, unsigned* __restrict__ list,
+                                                        unsigned* __restrict__ count) {
+    const unsigned tile = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (tile >= n_tiles) return;                                  // warp-uniform
+    const unsigned lane = threadIdx.x & 31u;
+    const int x = int(tile % unsigned(tiles_x)) * 8 + int(lane & 7u), y = int(tile / unsigned(tiles_x)) * 4 + int(lane >> 3);
+    bool refine = false;
+    if (x < width && y < height) {
+        unsigned lo[3] = {255u, 255u, 255u}, hi[3] = {0u, 0u, 0u};
+        for (int yy = max(y - 1, 0); yy <= min(y + 1, height - 1); yy++)
+            for (int xx = max(x - 1, 0); xx <= min(x + 1, width - 1); xx++) {
+                const size_t i = size_t(yy) * size_t(width) + size_t(xx);
+                const unsigned q = RGBA8 ? reinterpret_cast<const unsigned*>(frame)[i] : pack8(reinterpret_cast<const float4*>(frame)[i]);
+#pragma unroll
+                for (int ch = 0; ch < 3; ch++) {
+                    const unsigned v = (q >> (8 * ch)) & 0xffu;
+                    lo[ch] = min(lo[ch], v);
+                    hi[ch] = max(hi[ch], v);
+                }
+            }
+        const int range = int(max(hi[0] - lo[0], max(hi[1] - lo[1], hi[2] - lo[2])));
+        refine = range > threshold;
+    }
+    const unsigned m = __ballot_sync(0xffffffffu, refine);
+    if (m == 0u) return;
+    unsigned base = 0;
+    if (lane == 0) base = atomicAdd(count, unsigned(__popc(m)));
+    base = __shfl_sync(0xffffffffu, base, 0);
+    if (refine) list[base + unsigned(__popc(m & ((1u << lane) - 1u)))] = (unsigned(y) << 16) | unsigned(x);
+}
 
 }  // namespace
 
 namespace pe_host {
+
+int launch_refine_list(const void* frame, bool rgba8, int width, int height, int threshold, unsigned* list, unsigned* count,
+                       cudaStream_t s) {
+    const int tiles_x = (width + 7) / 8;
+    const unsigned n_tiles = unsigned(tiles_x) * unsigned((height + 3) / 4);
+    const unsigned blocks = (n_tiles + 7u) / 8u;                  // 8 warps = 8 tiles per block
+    if (rgba8) pe_k_refine_list<true><<<blocks, 256, 0, s>>>(frame, width, height, tiles_x, n_tiles, threshold, list, count);
+    else pe_k_refine_list<false><<<blocks, 256, 0, s>>>(frame, width, height, tiles_x, n_tiles, threshold, list, count);
+    return (int)cudaGetLastError();
+}
 
 int launch_quantize_rgba8(const void* in, void* out, size_t n, int sms, cudaStream_t s) {
     if (aligned16(out)) pe_k_quantize_rgba8<<<grid_for((n + 3) / 4, sms), 256, 0, s>>>((const float4*)in, (uchar4*)out, n);

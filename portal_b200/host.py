@@ -208,6 +208,11 @@ class HostPlayer:
     def set_anaglyph(self, draw_anaglyph: bool, colorful: bool = False, p: float = 0.29, q: float = 0.06):
         self._check(self._lib.ph_player_set_anaglyph(self._p, int(draw_anaglyph), int(colorful), float(p), float(q)))
 
+    def set_adaptive_aa(self, on: bool, threshold: int = 8):
+        """Adaptive anti-aliasing for render_frame and every motion-blur sub-frame (pe_render_adaptive): one sample
+        everywhere, all aa_count samples where the one-sample frame's 3x3 unorm8 range exceeds `threshold`."""
+        self._check(self._lib.ph_player_set_adaptive_aa(self._p, int(on), int(threshold)))
+
     def camera_state(self) -> dict:
         cam, inv, orbit, times = (C.c_double * 16)(), (C.c_double * 16)(), (C.c_double * 6)(), (C.c_double * 2)()
         sub, scale, n = C.c_int32(), C.c_double(), C.c_int64()

@@ -332,6 +332,32 @@ class SceneRenderer:
         self.set_uniforms()
         self._check(self._lib.pe_render_rgba8(self._ctx, C.byref(target), out_ptr, stream or None))
 
+    def draw_texture_adaptive(self, target: PeTarget, out_ptr: int, threshold: int, rgba8: bool = False, refined_ptr: int = 0,
+                              stream: int = 0):
+        """Adaptive anti-aliasing into device memory (async, pe_render_adaptive): the one-sample frame, then all aa_count
+        samples on the pixels whose 3x3 unorm8 range in it exceeds `threshold`.  `refined_ptr` (optional, device uint32)
+        receives the number of refined pixels.  Whole-frame targets only."""
+        self.set_uniforms()
+        self._check(self._lib.pe_render_adaptive(self._ctx, C.byref(target), int(threshold), int(rgba8), out_ptr, refined_ptr or None,
+                                                 stream or None))
+
+    def render_host_adaptive(self, width: int, height: int, threshold: int, rgba8: bool = False) -> tuple[np.ndarray, int]:
+        """One adaptive frame on the host (float RGBA, or RGBA8) and the number of refined pixels."""
+        n = width * height
+        bpp = 4 if rgba8 else 16
+        frame = np.empty((height, width, 4), dtype=np.uint8 if rgba8 else np.float32)
+        count = np.zeros(1, dtype=np.uint32)
+        dev = C.c_void_p()
+        self._check(self._lib.pe_device_malloc(self._ctx, n * bpp + 16, C.byref(dev)))
+        try:
+            cnt_dev = dev.value + n * bpp
+            self.draw_texture_adaptive(self.full_target(width, height), dev.value, threshold, rgba8, cnt_dev)
+            self._check(self._lib.pe_memcpy_d2h(self._ctx, frame.ctypes.data, dev.value, n * bpp, None))
+            self._check(self._lib.pe_memcpy_d2h(self._ctx, count.ctypes.data, cnt_dev, 4, None))
+        finally:
+            self._lib.pe_device_free(self._ctx, dev)
+        return frame, int(count[0])
+
     def submit_host_rgba8(self, width: int, height: int, host_ptr: int) -> int:
         """Queue one frame (render + D2H into pinned `host_ptr`) and return its ticket; at most
         PE_PIPELINE_DEPTH frames are in flight, frame i's copy overlaps frame i+1's kernel."""
