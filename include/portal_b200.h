@@ -186,7 +186,7 @@ PE_API int pe_host_free(pe_ctx* ctx, void* p);
  * `rgba8` selects the output format of `out_device` (0: float RGBA, 16 B/pixel; 1: RGBA8).  `refined_count_device`
  * (optional, device uint32) receives the number of refined pixels.  Enqueues three kernel launches on `stream` (NULL: the
  * context's stream) and returns without synchronising.  Only whole-frame targets ({w, h, h, 0, 1, 1, layout}) are accepted;
- * n_strips == 0 renders nothing and succeeds.  The pixel list lives in context scratch slots 123 and 124 (pe_scratch_buffer).
+ * n_strips == 0 renders nothing and succeeds.
  * The first call for a scene compiles a second program (the render program plus pe_refine_kernel, option "with_refine"). */
 PE_API int pe_render_adaptive(pe_ctx* ctx, const pe_target* target, int threshold, int rgba8, void* out_device,
                               void* refined_count_device, void* stream);
@@ -218,7 +218,8 @@ PE_API int pe_device_free(pe_ctx* ctx, void* device_ptr);
 PE_API int pe_memcpy_d2h(pe_ctx* ctx, void* host_dst, const void* device_src, size_t bytes, void* stream);
 /* Context-owned device scratch, slot 0..127: allocated on first use, grown (never shrunk) when a larger size is asked
  * for, freed by pe_destroy.  For per-frame intermediates of a frame loop (motion-blur sub-frames): no cudaMalloc /
- * cudaFree -- each a device-wide synchronisation -- inside the loop. */
+ * cudaFree -- each a device-wide synchronisation -- inside the loop.  Every slot is the caller's: the library keeps its
+ * own intermediates elsewhere. */
 PE_API int pe_scratch_buffer(pe_ctx* ctx, int slot, size_t bytes, void** device_ptr_out);
 /* Stream-ordered cross-GPU signalling without a collective: pe_signal_u32 publishes `value` to up to 8
  * flag words (device pointers, local or peer-mapped) after everything earlier in the stream -- remote

@@ -1,31 +1,17 @@
-// portal_b200 C ABI (include/portal_b200.h): context, scene builder, NVRTC specialisation cache,
-// constant-block uploader and launcher of the sm_90a ray-loop kernel.
+// portal_b200 C ABI (include/portal_b200.h): context, scene builder, constant-block uploader and launcher of the sm_90a
+// ray-loop kernel.  The scene program's variants (NVRTC, cubin cache, specialisation) are managed by pe_program.cpp.
 //
 // Mirrors, call for call, what the reference's SceneRenderer does with its macroquad Material
 // (/root/reference/src/main.rs:934-1064 new, :1266-1359 set_uniforms, :1411-1428 draw_texture,
 // /root/reference/src/gui/scene.rs:545-658 Scene::set_uniforms, :1112-1176 get_new_material).
 // There is NO CPU rendering path in this library: without a CUDA device pe_render* fail.
-#include <cuda_runtime.h>
-#include <dlfcn.h>
-#include <nvrtc.h>
-#include <sys/stat.h>
-#include <unistd.h>
-
 #include <cmath>
 #include <cstdio>
-#include <cstdlib>
 #include <cstring>
-#include <fstream>
-#include <map>
-#include <memory>
 #include <mutex>
 #include <string>
-#include <type_traits>
-#include <vector>
 
-#include "../../include/portal_b200.h"
-#include "pe_codegen.h"
-#include "pe_driver.h"
+#include "pe_context.h"
 #include "pe_internal.h"
 #include "pe_kernels.h"
 
@@ -47,125 +33,29 @@ struct PeLaunchHost {  // must match `PeLaunch` in device/pe_kernel.cuh
 };
 static_assert(sizeof(PeLaunchHost) == 72, "PeLaunch layout");
 
-struct Variant {
-    std::string source;
-    std::vector<char> cubin;
-    CUmodule_t module = nullptr;
-    CUfunction_t kernel = nullptr;
-    CUfunction_t probe = nullptr;
-    CUfunction_t refine = nullptr;   // pe_refine_kernel (programs generated with_refine)
-    int refine_blocks_per_sm = 1;
-    CUdeviceptr_t const_ptr = 0;
-    size_t const_size = 0;
-    int regs = 0;
-    int blocks_per_sm = 1;
-    // A second load of the same cubin: its own copy of the uniform block.  Two frames of one context can then be in flight at
-    // once (on two streams) -- frame f + 1's uniforms are uploaded while frame f's kernel still reads its own.
-    CUmodule_t module2 = nullptr;
-    CUfunction_t kernel2 = nullptr;
-    CUdeviceptr_t const_ptr2 = 0;
-};
-
-struct Texture {
-    void* dev = nullptr;
-    int w = 0, h = 0;
-};
-
 std::string g_create_error;
 std::mutex g_create_mutex;
-
-uint64_t fnv1a(const std::string& s, uint64_t h) {
-    for (unsigned char c : s) {
-        h ^= c;
-        h *= 1099511628211ull;
-    }
-    return h;
-}
-
-std::string lib_dir() {
-    Dl_info info;
-    if (dladdr((void*)&fnv1a, &info) && info.dli_fname) {
-        std::string p = info.dli_fname;
-        size_t s = p.rfind('/');
-        return s == std::string::npos ? "." : p.substr(0, s);
-    }
-    return ".";
-}
-
-std::string cache_dir() {
-    const char* e = std::getenv("PORTAL_B200_CACHE_DIR");
-    std::string d = e && *e ? e : lib_dir() + "/_cache";
-    mkdir(d.c_str(), 0755);
-    return d;
-}
-
-}  // namespace
-
-struct pe_ctx {
-    int device = -1;
-    bool has_gpu = false;
-    int sm_count = 132;
-    std::string err;
-
-    SceneDesc scene;
-    ConstLayout layout;
-    bool layout_valid = false;
-    GenOptions opts;
-    bool lineinfo = true;
-
-    std::vector<uint8_t> cblock;  // host image of the constant block
-    std::map<std::string, std::vector<float>> pending_mat;
-    std::map<std::string, float> pending_f;
-    std::map<std::string, int> pending_i;
-
-    std::map<std::vector<int>, std::unique_ptr<Variant>> variants;  // key: specialised ints + matrix structure masks
-    Variant* current = nullptr;
-    std::map<std::string, Texture> textures;
-
-    cudaStream_t stream = nullptr;
-    unsigned int* queue_dev = nullptr;
-    void* scratch_dev = nullptr;  // pe_render_host* staging
-    size_t scratch_bytes = 0;
-    void* scratch8_dev = nullptr;
-    // pe_submit_host_rgba8 pipeline
-    struct Slot { void* dev = nullptr; size_t bytes = 0; cudaEvent_t rendered = nullptr, copied = nullptr; uint64_t ticket = 0; };
-    Slot slots[PE_PIPELINE_DEPTH];
-    // adaptive de-specialisation: a slot whose value differed between renders more than kMaxRespecialisations times is read
-    // from the constant block from then on (bounds NVRTC compiles when an animation drives an int or a matrix structure)
-    std::vector<int> last_ints, int_changes;
-    std::vector<std::pair<unsigned, unsigned>> last_masks;
-    std::vector<int> mat_changes;
-    bool adapt = true;
-    cudaStream_t copy_stream = nullptr;
-    uint64_t next_ticket = 0;
-    size_t scratch8_bytes = 0;
-    uint64_t launches = 0;
-    const DriverApi* drv = nullptr;
-    // Uniform uploads go through a ring of PINNED staging images: cuMemcpyHtoDAsync from pageable memory first synchronises the
-    // stream (CUDA's documented behaviour), which made every frame's upload wait for the previous frame's kernel -- the host
-    // could never run ahead, and the frame pipelines (pe_submit_host_*, two frames in flight) were serialised by it.
-    static constexpr int kStage = 16;
-    uint8_t* ustage = nullptr;
-    size_t ustage_stride = 0;
-    cudaEvent_t ustage_done[kStage] = {nullptr};
-    bool ustage_used[kStage] = {false};
-    int ustage_next = 0;
-    struct Scratch { void* dev = nullptr; size_t bytes = 0; };
-    std::map<int, Scratch> user_scratch;   // pe_scratch_buffer
-
-    int fail(const std::string& m, int code = 1) {
-        err = m;
-        return code;
-    }
-};
-
-namespace {
 
 bool cuda_ok(pe_ctx* c, cudaError_t e, const char* what) {
     if (e == cudaSuccess) return true;
     c->err = std::string(what) + ": " + cudaGetErrorString(e);
     return false;
 }
+
+cudaStream_t stream_of(pe_ctx* c, void* stream) { return stream ? (cudaStream_t)stream : c->stream; }
+
+// Gives `*target` a value for the guard's lifetime and restores the old one on every return path.  A null target (a
+// uniform the scene does not declare) is left alone.
+template <class T>
+struct ScopedOverride {
+    T* target;
+    T saved;
+    ScopedOverride(T* p, const T& value) : target(p), saved(p ? *p : T()) { if (p) *p = value; }
+    explicit ScopedOverride(T* p) : target(p), saved(*p) {}   // saves only: the caller changes *p itself
+    ~ScopedOverride() { if (target) *target = saved; }
+    ScopedOverride(const ScopedOverride&) = delete;
+    ScopedOverride& operator=(const ScopedOverride&) = delete;
+};
 
 void set_renderer_defaults(pe_ctx* c);
 
@@ -190,9 +80,21 @@ float pinned_tanf(float x) {
     return (q & 1) ? -c / s : s / c;
 }
 
-void ensure_layout(pe_ctx* c) {
+float* fslot(pe_ctx* c, int slot) { return reinterpret_cast<float*>(c->cblock.data() + c->layout.off_float) + slot; }
+int* islot(pe_ctx* c, int slot) { return reinterpret_cast<int*>(c->cblock.data() + c->layout.off_int) + slot; }
+
+}  // namespace
+
+void pe_host::ensure_layout(pe_ctx* c) {
     if (c->layout_valid) return;
     c->layout = make_layout(c->scene);
+    const ConstLayout& L = c->layout;
+    c->slot_resolution_x = L.float_slot.at("_resolution_x");
+    c->slot_resolution_y = L.float_slot.at("_resolution_y");
+    c->slot_tan_half_view = L.float_slot.at("_tan_half_view");
+    c->slot_aa_count = L.int_slot.at("_aa_count");
+    c->slot_aa_start = L.int_slot.at("_aa_start");
+    c->slot_ray_tracing_depth = L.int_slot.at("_ray_tracing_depth");
     c->cblock.assign(c->layout.size, 0);
     c->layout_valid = true;
     set_renderer_defaults(c);
@@ -208,8 +110,7 @@ void ensure_layout(pe_ctx* c) {
     c->pending_i.clear();
 }
 
-float* fslot(pe_ctx* c, int slot) { return reinterpret_cast<float*>(c->cblock.data() + c->layout.off_float) + slot; }
-int* islot(pe_ctx* c, int slot) { return reinterpret_cast<int*>(c->cblock.data() + c->layout.off_int) + slot; }
+namespace {
 
 void set_renderer_defaults(pe_ctx* c) {
     // SceneRenderer::new (/root/reference/src/main.rs:1021-1047) and RotateAroundCam::new (:94-130)
@@ -281,268 +182,6 @@ void update_derived(pe_ctx* c) {
     }
 }
 
-std::vector<int> current_ints(pe_ctx* c) {
-    const int n = c->layout.n_int + kNumRendererInts;
-    std::vector<int> v(n);
-    std::memcpy(v.data(), c->cblock.data() + c->layout.off_int, size_t(n) * 4);
-    return v;
-}
-
-// Structure of every scene matrix in the block: which entries are exactly 0 / exactly 1 (bits 0..15 of the two masks) and
-// whether all 16 are finite (bit 16 of the second).  Three more records follow for `_camera`, `_camera_left_eye`,
-// `_camera_right_eye`: of those only "the bottom row is exactly 0 0 0 1" and the finite flag are recorded -- a camera moves
-// every frame, whether it is affine does not change.
-std::vector<std::pair<unsigned, unsigned>> matrix_masks(pe_ctx* c) {
-    std::vector<std::pair<unsigned, unsigned>> out(size_t(c->layout.n_mat) + 3);
-    const float* m = reinterpret_cast<const float*>(c->cblock.data() + c->layout.off_mat);
-    auto masks_of = [&](int slot, bool bottom_row_only) {
-        unsigned z = 0, o = 0;
-        bool finite = true;
-        for (int e = 0; e < 16; e++) {
-            const float v = m[16 * slot + e];
-            if (!std::isfinite(v)) finite = false;
-            if (v == 0.0f) z |= 1u << e;
-            else if (v == 1.0f) o |= 1u << e;
-        }
-        if (bottom_row_only) {
-            const bool affine = (z & 0x0888u) == 0x0888u && (o & 0x8000u);
-            z = affine ? 0x0888u : 0u;
-            o = affine ? 0x8000u : 0u;
-            if (!affine) finite = false;           // nothing to gain: keep one variant for every non-affine camera
-        }
-        return std::pair<unsigned, unsigned>{z, o | (finite ? 1u << 16 : 0u)};
-    };
-    for (int k = 0; k < c->layout.n_mat; k++) out[size_t(k)] = masks_of(k, false);
-    const int cams[3] = {c->layout.camera_slot, c->layout.camera_slot + 2, c->layout.camera_slot + 3};
-    for (int q = 0; q < 3; q++) out[size_t(c->layout.n_mat + q)] = masks_of(cams[q], true);
-    return out;
-}
-
-std::vector<int> variant_key(pe_ctx* c, const std::vector<int>& ints, const std::vector<std::pair<unsigned, unsigned>>& masks) {
-    std::vector<int> key;
-    if (c->opts.specialize_ints) {
-        key = ints;
-        // dynamic renderer ints do not take part in specialisation
-        key[c->layout.int_slot["_ray_tracing_depth"]] = 0;
-        key[c->layout.int_slot["_aa_start"]] = 0;
-    }
-    if (c->opts.specialize_matrices)
-        for (auto& zo : masks) { key.push_back(int(zo.first)); key.push_back(int(zo.second)); }
-    key.push_back(c->opts.with_probe ? 1 : 0);
-    key.push_back(c->opts.with_refine ? 1 : 0);
-    key.push_back(c->opts.uniforms_in_smem);
-    key.push_back(c->opts.tile_w);
-    key.push_back(c->opts.canon_rays ? 1 : 0);
-    key.push_back(c->opts.w_aware ? 1 : 0);
-    key.push_back(c->opts.block_threads);
-    key.push_back(c->opts.min_blocks);
-    key.push_back(c->opts.persistent ? 1 : 0);
-    for (char d : c->opts.dynamic_ints) key.push_back(d);
-    for (char d : c->opts.dynamic_mats) key.push_back(d);
-    return key;
-}
-
-// The JIT compiler is loaded PRIVATELY by path (the toolkit this library was built with, PE_NVRTC_PATH) instead of being a
-// link-time dependency: a process that imported torch first already holds torch's own libnvrtc.so.12 (another release),
-// and a DT_NEEDED entry would silently bind to that one -- the programs build() compiled into the disk cache would then
-// never be used on the GPU box, and the SASS inspected in the build container would not be the SASS that runs.
-struct NvrtcApi {
-    nvrtcResult (*Version)(int*, int*) = nullptr;
-    nvrtcResult (*CreateProgram)(nvrtcProgram*, const char*, const char*, int, const char* const*, const char* const*) = nullptr;
-    nvrtcResult (*CompileProgram)(nvrtcProgram, int, const char* const*) = nullptr;
-    nvrtcResult (*GetProgramLogSize)(nvrtcProgram, size_t*) = nullptr;
-    nvrtcResult (*GetProgramLog)(nvrtcProgram, char*) = nullptr;
-    nvrtcResult (*GetCUBINSize)(nvrtcProgram, size_t*) = nullptr;
-    nvrtcResult (*GetCUBIN)(nvrtcProgram, char*) = nullptr;
-    nvrtcResult (*DestroyProgram)(nvrtcProgram*) = nullptr;
-    const char* (*GetErrorString)(nvrtcResult) = nullptr;
-    std::string why;
-    bool ok = false;
-};
-const NvrtcApi& nvrtc_api() {
-    static NvrtcApi api;
-    static std::once_flag once;
-    std::call_once(once, [] {
-        void* h = nullptr;
-        const char* env = std::getenv("PORTAL_B200_NVRTC");
-        const char* candidates[] = {env && *env ? env : nullptr,
-#ifdef PE_NVRTC_PATH
-                                    PE_NVRTC_PATH,
-#endif
-                                    "/usr/local/cuda/lib64/libnvrtc.so.12", "libnvrtc.so.12", "libnvrtc.so"};
-        for (const char* cnd : candidates) {
-            if (!cnd) continue;
-            h = dlopen(cnd, RTLD_NOW | RTLD_LOCAL);
-            if (h) break;
-        }
-        if (!h) { api.why = std::string("cannot load NVRTC: ") + dlerror(); return; }
-        auto bind = [&](const char* name, auto& fn) {
-            fn = reinterpret_cast<std::remove_reference_t<decltype(fn)>>(dlsym(h, name));
-            if (!fn && api.why.empty()) api.why = std::string("NVRTC: missing symbol ") + name;
-            return fn != nullptr;
-        };
-        api.ok = bind("nvrtcVersion", api.Version) & bind("nvrtcCreateProgram", api.CreateProgram) &
-                 bind("nvrtcCompileProgram", api.CompileProgram) & bind("nvrtcGetProgramLogSize", api.GetProgramLogSize) &
-                 bind("nvrtcGetProgramLog", api.GetProgramLog) & bind("nvrtcGetCUBINSize", api.GetCUBINSize) &
-                 bind("nvrtcGetCUBIN", api.GetCUBIN) & bind("nvrtcDestroyProgram", api.DestroyProgram) &
-                 bind("nvrtcGetErrorString", api.GetErrorString);
-    });
-    return api;
-}
-
-// NVRTC: source -> sm_90a cubin (disk-cached by content hash).
-bool compile_cubin(pe_ctx* c, const std::string& source, std::vector<char>& cubin, bool force_recompile = false) {
-    std::vector<std::string> o = {"--gpu-architecture=sm_90a", "--std=c++20", "-default-device", "--fmad=false",
-                                  "--prec-div=true", "--prec-sqrt=true", "--ftz=false"};
-    if (c->lineinfo) o.push_back("-lineinfo");
-    const NvrtcApi& N = nvrtc_api();
-    if (!N.ok) { c->err = N.why; return false; }
-    int major = 0, minor = 0;
-    N.Version(&major, &minor);
-    std::string tag = "nvrtc" + std::to_string(major) + "." + std::to_string(minor);
-    for (auto& s : o) tag += s;
-    uint64_t h1 = fnv1a(tag, fnv1a(source, 1469598103934665603ull));
-    uint64_t h2 = fnv1a(source, fnv1a(tag, 0x9e3779b97f4a7c15ull));
-    char name[64];
-    std::snprintf(name, sizeof name, "/%016llx%016llx.cubin", (unsigned long long)h1, (unsigned long long)h2);
-    const std::string path = cache_dir() + name;
-    {
-        std::ifstream f(path, std::ios::binary);
-        if (f) {
-            cubin.assign(std::istreambuf_iterator<char>(f), std::istreambuf_iterator<char>());
-            // a truncated copy (interrupted transfer to the GPU box) must not be trusted: ELF magic + section table inside the file
-            bool ok = cubin.size() > 64 && std::memcmp(cubin.data(), "\x7f" "ELF", 4) == 0;
-            if (ok) {
-                uint64_t shoff = 0;
-                uint16_t shentsize = 0, shnum = 0;
-                std::memcpy(&shoff, cubin.data() + 0x28, 8);
-                std::memcpy(&shentsize, cubin.data() + 0x3a, 2);
-                std::memcpy(&shnum, cubin.data() + 0x3c, 2);
-                ok = shoff + uint64_t(shentsize) * shnum <= cubin.size();
-            }
-            if (ok && !force_recompile) return true;
-            cubin.clear();
-            std::remove(path.c_str());
-        }
-    }
-    nvrtcProgram prog;
-    if (N.CreateProgram(&prog, source.c_str(), "scene_program.cu", 0, nullptr, nullptr) != NVRTC_SUCCESS) {
-        c->err = "nvrtcCreateProgram failed";
-        return false;
-    }
-    std::vector<const char*> opts;
-    for (auto& s : o) opts.push_back(s.c_str());
-    nvrtcResult r = N.CompileProgram(prog, int(opts.size()), opts.data());
-    size_t ls = 0;
-    N.GetProgramLogSize(prog, &ls);
-    std::string log(ls, '\0');
-    if (ls) N.GetProgramLog(prog, &log[0]);
-    if (r != NVRTC_SUCCESS) {
-        // Diagnostics already carry "<scene element>(local line)" thanks to the #line directives
-        // the generator puts around every user snippet.
-        c->err = std::string("scene program failed to compile (") + N.GetErrorString(r) + "):\n" + log;
-        N.DestroyProgram(&prog);
-        return false;
-    }
-    size_t cs = 0;
-    N.GetCUBINSize(prog, &cs);
-    cubin.resize(cs);
-    N.GetCUBIN(prog, cubin.data());
-    N.DestroyProgram(&prog);
-    {
-        std::string tmp = path + ".tmp" + std::to_string((long long)getpid());
-        std::ofstream f(tmp, std::ios::binary);
-        if (f) {
-            f.write(cubin.data(), std::streamsize(cubin.size()));
-            f.close();
-            std::rename(tmp.c_str(), path.c_str());
-        }
-    }
-    return true;
-}
-
-const int kMaxRespecialisations = 4;
-
-// Make the variant for the current integer uniforms current (generate / compile / load as needed).
-bool select_variant(pe_ctx* c) {
-    ensure_layout(c);
-    std::vector<int> ints = current_ints(c);
-    std::vector<std::pair<unsigned, unsigned>> masks = matrix_masks(c);
-    if (c->adapt) {
-        c->opts.dynamic_ints.resize(ints.size(), 0);
-        c->opts.dynamic_mats.resize(masks.size(), 0);
-        c->int_changes.resize(ints.size(), 0);
-        c->mat_changes.resize(masks.size(), 0);
-        if (c->last_ints.size() == ints.size())
-            for (size_t k = 0; k < ints.size(); k++)
-                if (ints[k] != c->last_ints[k] && ++c->int_changes[k] > kMaxRespecialisations) c->opts.dynamic_ints[k] = 1;
-        if (c->last_masks.size() == masks.size())
-            for (size_t k = 0; k < masks.size(); k++)
-                if (masks[k] != c->last_masks[k] && ++c->mat_changes[k] > kMaxRespecialisations) c->opts.dynamic_mats[k] = 1;
-        c->last_ints = ints;
-        c->last_masks = masks;
-    }
-    for (size_t k = 0; k < ints.size() && k < c->opts.dynamic_ints.size(); k++)
-        if (c->opts.dynamic_ints[k]) ints[k] = 0;                       // not part of the key, not baked in
-    for (size_t k = 0; k < masks.size() && k < c->opts.dynamic_mats.size(); k++)
-        if (c->opts.dynamic_mats[k]) masks[k] = {0u, 0u};               // general matrix: full FFMA chain
-    std::vector<int> key = variant_key(c, ints, masks);
-    auto it = c->variants.find(key);
-    if (it == c->variants.end()) {
-        if (c->variants.size() >= 64) {  // bound the cache: drop everything but the current variant
-            for (auto v = c->variants.begin(); v != c->variants.end();) {
-                if (v->second.get() == c->current) { ++v; continue; }
-                if (v->second->module && c->has_gpu) { cudaDeviceSynchronize(); c->drv->cuModuleUnload(v->second->module); }
-                if (v->second->module2 && c->has_gpu) c->drv->cuModuleUnload(v->second->module2);
-                v = c->variants.erase(v);
-            }
-        }
-        GenResult g = generate_program(c->scene, c->layout, c->opts, ints, masks);
-        if (!g.error.empty()) {
-            c->err = g.error;
-            return false;
-        }
-        auto v = std::make_unique<Variant>();
-        v->source = std::move(g.source);
-        if (!compile_cubin(c, v->source, v->cubin)) return false;
-        it = c->variants.emplace(key, std::move(v)).first;
-    }
-    Variant* v = it->second.get();
-    if (c->has_gpu && !v->module) {
-        const DriverApi* d = c->drv;
-        CUresult_t r = d->cuModuleLoadData(&v->module, v->cubin.data());
-        if (r != 0) {
-            // a cached cubin the driver rejects (corrupt file, other driver generation): evict it and compile once more
-            if (!compile_cubin(c, v->source, v->cubin, true)) return false;
-            r = d->cuModuleLoadData(&v->module, v->cubin.data());
-        }
-        if (r != 0) { c->err = "cuModuleLoadData: " + driver_error(d, r); return false; }
-        r = d->cuModuleGetFunction(&v->kernel, v->module, "pe_render_kernel");
-        if (r != 0) { c->err = "cuModuleGetFunction(pe_render_kernel): " + driver_error(d, r); return false; }
-        const char* block_symbol = c->opts.uniforms_in_smem ? "PE_C_UPLOAD" : "PE_C";
-        r = d->cuModuleGetGlobal(&v->const_ptr, &v->const_size, v->module, block_symbol);
-        if (r != 0) { c->err = std::string("cuModuleGetGlobal(") + block_symbol + "): " + driver_error(d, r); return false; }
-        if (v->const_size != c->layout.size) { c->err = "constant block size mismatch between host and device"; return false; }
-        if (c->opts.with_probe) {
-            r = d->cuModuleGetFunction(&v->probe, v->module, "pe_probe_kernel");
-            if (r != 0) { c->err = "cuModuleGetFunction(pe_probe_kernel): " + driver_error(d, r); return false; }
-        }
-        if (c->opts.with_refine) {
-            r = d->cuModuleGetFunction(&v->refine, v->module, "pe_refine_kernel");
-            if (r != 0) { c->err = "cuModuleGetFunction(pe_refine_kernel): " + driver_error(d, r); return false; }
-            int nb = 1;
-            if (d->cuOccupancyMaxActiveBlocksPerMultiprocessor(&nb, v->refine, c->opts.block_threads, 0) == 0 && nb > 0)
-                v->refine_blocks_per_sm = nb;
-        }
-        d->cuFuncGetAttribute(&v->regs, 4 /*CU_FUNC_ATTRIBUTE_NUM_REGS*/, v->kernel);
-        int nb = 1;
-        if (d->cuOccupancyMaxActiveBlocksPerMultiprocessor(&nb, v->kernel, c->opts.block_threads, 0) == 0 && nb > 0)
-            v->blocks_per_sm = nb;
-    }
-    c->current = v;
-    return true;
-}
-
 bool bind_device(pe_ctx* c) {
     if (!c->has_gpu) {
         c->err = "this context has no CUDA device (compile-only); portal_b200 has no CPU rendering path";
@@ -572,10 +211,6 @@ bool check_target(pe_ctx* c, const pe_target* t) {
 }  // namespace
 
 int pe_internal_device(pe_ctx* c) { return (c && c->has_gpu) ? c->device : -1; }
-int pe_internal_render_impl(pe_ctx* c, const pe_target* t, void* out_device, void* stream, int rgba8, int instance);
-int pe_internal_render(pe_ctx* c, const pe_target* t, void* out_device, void* stream, int rgba8, int instance) {
-    return pe_internal_render_impl(c, t, out_device, stream, rgba8, instance);
-}
 
 extern "C" {
 
@@ -608,8 +243,7 @@ pe_ctx* pe_create(int device) {
                 return nullptr;
             }
         }
-        if (cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess ||
-            cudaMalloc(&c->queue_dev, 256) != cudaSuccess) {
+        if (cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess || c->queue.ensure(256) != cudaSuccess) {
             g_create_error = "cannot create stream / queue counter";
             if (c->stream) cudaStreamDestroy(c->stream);
             return nullptr;
@@ -622,31 +256,18 @@ pe_ctx* pe_create(int device) {
 
 void pe_destroy(pe_ctx* c) {
     if (!c) return;
+    unload_variants(c, nullptr);   // waits for the device
     if (c->has_gpu) {
-        cudaSetDevice(c->device);
-        cudaDeviceSynchronize();
-        for (auto& kv : c->variants) {
-            if (kv.second->module) c->drv->cuModuleUnload(kv.second->module);
-            if (kv.second->module2) c->drv->cuModuleUnload(kv.second->module2);
-        }
-        for (auto& kv : c->textures)
-            if (kv.second.dev) cudaFree(kv.second.dev);
-        if (c->scratch_dev) cudaFree(c->scratch_dev);
-        if (c->scratch8_dev) cudaFree(c->scratch8_dev);
         for (auto& sl : c->slots) {
-            if (sl.dev) cudaFree(sl.dev);
             if (sl.rendered) cudaEventDestroy(sl.rendered);
             if (sl.copied) cudaEventDestroy(sl.copied);
         }
-        for (auto& kv : c->user_scratch)
-            if (kv.second.dev) cudaFree(kv.second.dev);
         if (c->ustage) cudaFreeHost(c->ustage);
         for (auto& e : c->ustage_done) if (e) cudaEventDestroy(e);
         if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
-        if (c->queue_dev) cudaFree(c->queue_dev);
         if (c->stream) cudaStreamDestroy(c->stream);
     }
-    delete c;
+    delete c;   // the device buffers free themselves
 }
 
 const char* pe_last_error(pe_ctx* c) { return c ? c->err.c_str() : g_create_error.c_str(); }
@@ -654,16 +275,7 @@ const char* pe_last_error(pe_ctx* c) { return c ? c->err.c_str() : g_create_erro
 // ------------------------------------------------------------------------------ scene builder
 int pe_scene_begin(pe_ctx* c) {
     if (!c) return 1;
-    if (c->has_gpu) {
-        cudaSetDevice(c->device);
-        cudaDeviceSynchronize();
-        for (auto& kv : c->variants) {
-            if (kv.second->module) c->drv->cuModuleUnload(kv.second->module);
-            if (kv.second->module2) c->drv->cuModuleUnload(kv.second->module2);
-        }
-    }
-    c->variants.clear();
-    c->current = nullptr;
+    unload_variants(c, nullptr);
     c->scene = SceneDesc();
     c->layout_valid = false;
     c->last_ints.clear();
@@ -824,17 +436,7 @@ int pe_set_option(pe_ctx* c, const char* key, int value) {
         c->opts.tile_w = value;
     }
     else return c->fail("unknown option `" + k + "`");
-    // options change the generated program
-    if (c->has_gpu) {
-        cudaSetDevice(c->device);
-        cudaDeviceSynchronize();
-        for (auto& kv : c->variants) {
-            if (kv.second->module) c->drv->cuModuleUnload(kv.second->module);
-            if (kv.second->module2) c->drv->cuModuleUnload(kv.second->module2);
-        }
-    }
-    c->variants.clear();
-    c->current = nullptr;
+    unload_variants(c, nullptr);   // options change the generated program
     return 0;
 }
 
@@ -858,8 +460,8 @@ int pe_scene_uniform_block(pe_ctx* c, int width, int height, const void** data, 
     if (!c || !data || !size) return 1;
     if (width <= 0 || height <= 0) return c->fail("pe_scene_uniform_block: bad frame size");
     ensure_layout(c);
-    *fslot(c, c->layout.float_slot["_resolution_x"]) = float(width);
-    *fslot(c, c->layout.float_slot["_resolution_y"]) = float(height);
+    *fslot(c, c->slot_resolution_x) = float(width);
+    *fslot(c, c->slot_resolution_y) = float(height);
     if (!select_variant(c)) return 1;
     update_derived(c);
     *data = c->cblock.data();
@@ -904,7 +506,7 @@ int pe_set_uniform_f32(pe_ctx* c, const char* name, float v) {
     *fslot(c, it->second) = v;
     if (n == "_view_angle") {
         // frag.glsl:450 `tan(_view_angle / 2.)` -- a uniform expression, evaluated once here in fp32 (pinned tan)
-        *fslot(c, c->layout.float_slot["_tan_half_view"]) = pinned_tanf(v / 2.0f);
+        *fslot(c, c->slot_tan_half_view) = pinned_tanf(v / 2.0f);
     }
     return 0;
 }
@@ -927,15 +529,12 @@ int pe_set_texture(pe_ctx* c, const char* name, const uint8_t* rgba8, int w, int
     auto it = c->layout.tex_slot.find(name);
     if (it == c->layout.tex_slot.end()) return c->fail(std::string("unknown texture `") + name + "`", 2);
     if (!bind_device(c)) return 1;
-    Texture& t = c->textures[name];
+    DeviceBuffer& t = c->textures[name];
     size_t bytes = size_t(w) * size_t(h) * 4;
     cudaStreamSynchronize(c->stream);
-    if (t.dev) cudaFree(t.dev);
-    t.dev = nullptr;
-    if (!cuda_ok(c, cudaMalloc(&t.dev, bytes), "cudaMalloc(texture)")) return 1;
+    t.release();
+    if (!cuda_ok(c, t.ensure(bytes), "cudaMalloc(texture)")) return 1;
     if (!cuda_ok(c, cudaMemcpy(t.dev, rgba8, bytes, cudaMemcpyHostToDevice), "cudaMemcpy(texture)")) return 1;
-    t.w = w;
-    t.h = h;
     uint8_t* rec = c->cblock.data() + c->layout.off_tex + size_t(it->second) * 16;
     std::memcpy(rec, &t.dev, 8);
     std::memcpy(rec + 8, &w, 4);
@@ -950,8 +549,12 @@ size_t pe_target_pixels(const pe_target* t) {
     return size_t(t->n_strips) * size_t(t->strip_rows) * size_t(t->width);
 }
 
+}  // extern "C"
+
+namespace {
+
 // Enqueue the upload of the host image of the uniform block to `dst` on stream `s`, from pinned staging memory.
-static bool upload_uniform_block(pe_ctx* c, CUdeviceptr_t dst, CUstream_t s) {
+bool upload_uniform_block(pe_ctx* c, CUdeviceptr_t dst, CUstream_t s) {
     const size_t n = c->cblock.size();
     const size_t stride = (n + 255) & ~size_t(255);
     if (!c->ustage || c->ustage_stride < stride) {
@@ -975,40 +578,15 @@ static bool upload_uniform_block(pe_ctx* c, CUdeviceptr_t dst, CUstream_t s) {
     return true;
 }
 
-static int render_impl(pe_ctx* c, const pe_target* t, void* out_device, void* bounces_device, void* stream, bool rgba8, int instance = 0) {
-    if (!c) return 1;
-    if (!out_device) return c->fail("pe_render: out_device is null");
-    if (!check_target(c, t) || !bind_device(c)) return 1;
-    if (t->n_strips == 0) return 0;   // nothing of this frame belongs to the caller
-    ensure_layout(c);
-    *fslot(c, c->layout.float_slot["_resolution_x"]) = float(t->width);
-    *fslot(c, c->layout.float_slot["_resolution_y"]) = float(t->height);
-    if (!select_variant(c)) return 1;
-    update_derived(c);
-    Variant* v = c->current;
-    const DriverApi* d = c->drv;
-    CUstream_t s = stream ? (CUstream_t)stream : (CUstream_t)c->stream;
-
-    CUfunction_t kernel = v->kernel;
-    CUdeviceptr_t const_ptr = v->const_ptr;
-    CUresult_t r = 0;
-    if (instance == 1) {
-        if (!v->module2) {
-            size_t sz = 0;
-            r = d->cuModuleLoadData(&v->module2, v->cubin.data());
-            if (r == 0) r = d->cuModuleGetFunction(&v->kernel2, v->module2, "pe_render_kernel");
-            if (r == 0) r = d->cuModuleGetGlobal(&v->const_ptr2, &sz, v->module2, c->opts.uniforms_in_smem ? "PE_C_UPLOAD" : "PE_C");
-            if (r != 0) return c->fail("second program instance: " + driver_error(d, r));
-        }
-        kernel = v->kernel2;
-        const_ptr = v->const_ptr2;
-    }
-    if (!upload_uniform_block(c, const_ptr, s)) return 1;
-
+// The render kernel's launch record for a render of `t` into `out`.  pe_refine_kernel takes the same record for its
+// whole-frame target: it reads only out, width, out_rgba8, bounces and the store index, and with local row == global row
+// the store index does not depend on the layout flag.  tiles_x / tiles_y count the persistent scheduler's 8x4-pixel tiles,
+// a fixed size in device/pe_kernel.cuh.
+PeLaunchHost launch_record(pe_ctx* c, const pe_target* t, void* out, void* bounces, bool rgba8) {
     PeLaunchHost L;
     std::memset(&L, 0, sizeof L);
-    L.out = out_device;
-    L.bounces = bounces_device;
+    L.out = out;
+    L.bounces = bounces;
     L.width = t->width;
     L.height = t->height;
     L.strip_rows = t->strip_rows;
@@ -1016,39 +594,67 @@ static int render_impl(pe_ctx* c, const pe_target* t, void* out_device, void* bo
     L.strip_step = t->strip_step;
     L.n_strips = t->n_strips;
     L.out_full_frame = t->full_frame_layout ? 1 : 0;
-    const int local_rows = t->n_strips * t->strip_rows;
     L.tiles_x = (t->width + 7) / 8;
-    L.tiles_y = (local_rows + 3) / 4;
+    L.tiles_y = (t->n_strips * t->strip_rows + 3) / 4;
     L.out_rgba8 = rgba8 ? 1 : 0;
-    L.queue = c->queue_dev;
+    L.queue = c->queue.dev;
     L.strip_shift = -1;
     if ((t->strip_rows & (t->strip_rows - 1)) == 0)
         for (int sh = 0; sh < 31; sh++)
             if ((1 << sh) == t->strip_rows) L.strip_shift = sh;
+    return L;
+}
+
+// Grid of the one-thread-per-pixel render kernel over the target's local rows: must match PE_BLOCK_W / PE_BLOCK_ROWS in
+// device/pe_kernel.cuh
+void render_grid(const GenOptions& o, const pe_target* t, unsigned& gx, unsigned& gy) {
+    const int tile_w = o.tile_w, block_w = tile_w < 16 ? 16 : tile_w;
+    const int rows_per_block = (o.block_threads / 32) / (block_w / tile_w) * (32 / tile_w);
+    gx = unsigned((t->width + block_w - 1) / block_w);
+    gy = unsigned((t->n_strips * t->strip_rows + rows_per_block - 1) / rows_per_block);
+}
+
+// pe_render / pe_render_rgba8 through program instance 0 or 1.  `counted`: see select_variant.
+int render_impl(pe_ctx* c, const pe_target* t, void* out_device, void* bounces_device, void* stream, bool rgba8, int instance = 0,
+                bool counted = true) {
+    if (!c) return 1;
+    if (!out_device) return c->fail("pe_render: out_device is null");
+    if (!check_target(c, t) || !bind_device(c)) return 1;
+    if (t->n_strips == 0) return 0;   // nothing of this frame belongs to the caller
+    ensure_layout(c);
+    *fslot(c, c->slot_resolution_x) = float(t->width);
+    *fslot(c, c->slot_resolution_y) = float(t->height);
+    if (!select_variant(c, false, false, counted)) return 1;
+    update_derived(c);
+    Variant* v = c->current;
+    if (!load_instance(c, *v, instance)) return 1;
+    const DriverApi* d = c->drv;
+    const CUstream_t s = (CUstream_t)stream_of(c, stream);
+    if (!upload_uniform_block(c, v->inst[instance].const_ptr, s)) return 1;
+
+    PeLaunchHost L = launch_record(c, t, out_device, bounces_device, rgba8);
     void* args[] = {&L};
     unsigned gx, gy;
     if (c->opts.persistent) {
-        r = d->cuMemsetD32Async((CUdeviceptr_t)c->queue_dev, 0, 1, s);
+        CUresult_t r = d->cuMemsetD32Async((CUdeviceptr_t)c->queue.dev, 0, 1, s);
         if (r != 0) return c->fail("queue reset: " + driver_error(d, r));
         gx = unsigned(c->sm_count * v->blocks_per_sm);
         gy = 1;
     } else {
-        // must match PE_BLOCK_W / PE_BLOCK_ROWS in device/pe_kernel.cuh
-        const int tile_w = c->opts.tile_w, block_w = tile_w < 16 ? 16 : tile_w;
-        const int rows_per_block = (c->opts.block_threads / 32) / (block_w / tile_w) * (32 / tile_w);
-        gx = unsigned((t->width + block_w - 1) / block_w);
-        gy = unsigned((local_rows + rows_per_block - 1) / rows_per_block);
+        render_grid(c->opts, t, gx, gy);
     }
-    r = d->cuLaunchKernel(kernel, gx, gy, 1, unsigned(c->opts.block_threads), 1, 1, 0, s, args, nullptr);
+    CUresult_t r = d->cuLaunchKernel(v->inst[instance].kernel, gx, gy, 1, unsigned(c->opts.block_threads), 1, 1, 0, s, args, nullptr);
     if (r != 0) return c->fail("cuLaunchKernel(pe_render_kernel): " + driver_error(d, r));
     c->launches++;
     return 0;
 }
 
-}  // extern "C"
-int pe_internal_render_impl(pe_ctx* c, const pe_target* t, void* out_device, void* stream, int rgba8, int instance) {
+}  // namespace
+
+int pe_internal_render(pe_ctx* c, const pe_target* t, void* out_device, void* stream, int rgba8, int instance) {
     return render_impl(c, t, out_device, nullptr, stream, rgba8 != 0, instance);
 }
+
 extern "C" {
 
 int pe_render(pe_ctx* c, const pe_target* t, void* out_device, void* bounces_device, void* stream) {
@@ -1059,47 +665,30 @@ int pe_render_rgba8(pe_ctx* c, const pe_target* t, void* out_device_rgba8, void*
     return render_impl(c, t, out_device_rgba8, nullptr, stream, true);
 }
 
-static bool ensure_scratch(pe_ctx* c, void** p, size_t* have, size_t need);
-
 int pe_probe_ray(pe_ctx* c, const float a[3], const float b[3], float pos_out[3], int32_t* have_result,
                  int32_t* encounter_object, int32_t* change_subspace) {
     if (!c) return 1;
     if (!a || !b || !pos_out) return c->fail("pe_probe_ray: null argument");
     if (!bind_device(c)) return 1;
     ensure_layout(c);
-    // main.rs:1367: the probe always runs with `teleport_light_u` = 1 (if the scene has that uniform)
+    // main.rs:1367: the probe always runs with `teleport_light_u` = 1 (if the scene has that uniform); that is not a scene
+    // change for the specialisation tracker
     auto tl = c->layout.int_slot.find("teleport_light_u");
-    int saved = 0;
-    if (tl != c->layout.int_slot.end()) { saved = *islot(c, tl->second); *islot(c, tl->second) = 1; }
-    const bool had_probe = c->opts.with_probe, had_adapt = c->adapt;
-    c->opts.with_probe = true;
-    c->adapt = false;                 // the probe's own `teleport_light_u` = 1 is not a scene change
-    bool ok = select_variant(c);
-    c->adapt = had_adapt;
-    if (ok) update_derived(c);
-    struct { float ax, ay, az, bx, by, bz; void* out; } P;
+    ScopedOverride<int> teleport(tl != c->layout.int_slot.end() ? islot(c, tl->second) : nullptr, 1);
+    if (!select_variant(c, /*need_probe=*/true, false, /*counted=*/false)) return 1;
+    update_derived(c);
+    if (!cuda_ok(c, c->staging8.ensure(64), "cudaMalloc(staging)")) return 1;
+    Variant* v = c->current;
+    const CUstream_t s = (CUstream_t)c->stream;
+    struct { float ax, ay, az, bx, by, bz; void* out; } P = {a[0], a[1], a[2], b[0], b[1], b[2], c->staging8.dev};
+    void* args[] = {&P};
+    if (!upload_uniform_block(c, v->inst[0].const_ptr, s)) return 1;
+    CUresult_t r = c->drv->cuLaunchKernel(v->probe, 1, 1, 1, 32, 1, 1, 0, s, args, nullptr);
+    if (r != 0) return c->fail("pe_probe_kernel: " + driver_error(c->drv, r));
+    c->launches++;
     float host[6] = {0, 0, 0, 0, 0, 0};
-    if (ok) {
-        if (!ensure_scratch(c, &c->scratch8_dev, &c->scratch8_bytes, 64)) ok = false;
-    }
-    if (ok) {
-        Variant* v = c->current;
-        const DriverApi* d = c->drv;
-        CUstream_t s = (CUstream_t)c->stream;
-        P = {a[0], a[1], a[2], b[0], b[1], b[2], c->scratch8_dev};
-        void* args[] = {&P};
-        CUresult_t r = upload_uniform_block(c, v->const_ptr, s) ? 0 : 999;
-        if (r == 0) r = d->cuLaunchKernel(v->probe, 1, 1, 1, 32, 1, 1, 0, s, args, nullptr);
-        if (r != 0) { c->err = "pe_probe_kernel: " + driver_error(d, r); ok = false; }
-        else {
-            c->launches++;
-            ok = cuda_ok(c, cudaMemcpyAsync(host, c->scratch8_dev, sizeof host, cudaMemcpyDeviceToHost, c->stream), "probe readback") &&
-                 cuda_ok(c, cudaStreamSynchronize(c->stream), "pe_probe_ray");
-        }
-    }
-    c->opts.with_probe = had_probe;
-    if (tl != c->layout.int_slot.end()) *islot(c, tl->second) = saved;
-    if (!ok) return 1;
+    if (!cuda_ok(c, cudaMemcpyAsync(host, c->staging8.dev, sizeof host, cudaMemcpyDeviceToHost, c->stream), "probe readback") ||
+        !cuda_ok(c, cudaStreamSynchronize(c->stream), "pe_probe_ray")) return 1;
     for (int k = 0; k < 3; k++) pos_out[k] = host[k];
     if (have_result) *have_result = host[3] != 0.0f;
     if (encounter_object) *encounter_object = host[4] != 0.0f;
@@ -1119,73 +708,41 @@ int pe_render_adaptive(pe_ctx* c, const pe_target* t, int threshold, int rgba8, 
         return c->fail("pe_render_adaptive: only whole-frame targets ({w, h, h, 0, 1, 1, layout}) are supported -- the 3x3 edge "
                        "window of a pixel crosses strip boundaries");
     ensure_layout(c);
-    const int aa_slot = c->layout.int_slot["_aa_count"];
-    const int n_aa = *islot(c, aa_slot);
-    CUstream_t s = stream ? (CUstream_t)stream : (CUstream_t)c->stream;
+    const cudaStream_t s = stream_of(c, stream);
+    {
+        // (1) the one-sample frame, straight into the caller's buffer: exactly pe_render(_rgba8) with `_aa_count` = 1.  The
+        // override is not a scene change for the specialisation tracker (as `teleport_light_u` in pe_probe_ray).
+        ScopedOverride<int> one_sample(islot(c, c->slot_aa_count), 1);
+        if (render_impl(c, t, out_device, nullptr, s, rgba8 != 0, 0, /*counted=*/false)) return 1;
+    }
 
-    // (1) the one-sample frame, straight into the caller's buffer: exactly pe_render(_rgba8) with `_aa_count` = 1.  The
-    // override is not a scene change for the specialisation tracker (as `teleport_light_u` in pe_probe_ray).
-    *islot(c, aa_slot) = 1;
-    const bool had_adapt = c->adapt;
-    c->adapt = false;
-    int rc = render_impl(c, t, out_device, nullptr, s, rgba8 != 0);
-    c->adapt = had_adapt;
-    *islot(c, aa_slot) = n_aa;
-    if (rc) return 1;
-
-    // (2) the list of pixels to refine: count + refill cursor in scratch slot 124, packed pixel indices in slot 123
+    // (2) the list of pixels to refine: packed pixel indices, and their count + refill cursor
     const size_t n_px = size_t(t->width) * size_t(t->height);
-    void *list = nullptr, *counter = nullptr;
-    if (pe_scratch_buffer(c, 123, n_px * 4, &list) || pe_scratch_buffer(c, 124, 16, &counter)) return 1;
-    if (!cuda_ok(c, cudaMemsetAsync(counter, 0, 16, (cudaStream_t)s), "pe_render_adaptive: counter reset")) return 1;
-    if (!cuda_ok(c, (cudaError_t)launch_refine_list(out_device, rgba8 != 0, t->width, t->height, threshold, (unsigned*)list,
-                                                    (unsigned*)counter, (cudaStream_t)s), "pe_render_adaptive: refine list"))
+    if (!cuda_ok(c, c->refine_list.ensure(n_px * 4), "cudaMalloc(refine list)") ||
+        !cuda_ok(c, c->refine_count.ensure(16), "cudaMalloc(refine count)")) return 1;
+    unsigned* list = (unsigned*)c->refine_list.dev;
+    unsigned* counter = (unsigned*)c->refine_count.dev;
+    if (!cuda_ok(c, cudaMemsetAsync(counter, 0, 16, s), "pe_render_adaptive: counter reset")) return 1;
+    if (!cuda_ok(c, (cudaError_t)launch_refine_list(out_device, rgba8 != 0, t->width, t->height, threshold, list, counter, s),
+                 "pe_render_adaptive: refine list"))
         return 1;
     c->launches++;
     if (refined_count_device &&
-        !cuda_ok(c, cudaMemcpyAsync(refined_count_device, counter, 4, cudaMemcpyDeviceToDevice, (cudaStream_t)s), "refined count copy"))
+        !cuda_ok(c, cudaMemcpyAsync(refined_count_device, counter, 4, cudaMemcpyDeviceToDevice, s), "refined count copy"))
         return 1;
 
     // (3) the refine pass: the same program with pe_refine_kernel, `_aa_count` = N
-    const bool had_refine = c->opts.with_refine;
-    c->opts.with_refine = true;
-    const bool ok = select_variant(c);
-    c->opts.with_refine = had_refine;
-    if (!ok) return 1;
+    if (!select_variant(c, false, /*need_refine=*/true)) return 1;
     update_derived(c);
     Variant* v = c->current;
-    if (!upload_uniform_block(c, v->const_ptr, s)) return 1;
-    struct { PeLaunchHost L; const void* list; void* count; } R;
-    std::memset(&R, 0, sizeof R);
-    R.L.out = out_device;
-    R.L.width = t->width;
-    R.L.height = t->height;
-    R.L.strip_rows = t->strip_rows;
-    R.L.strip_step = t->strip_step;
-    R.L.n_strips = 1;
-    R.L.out_full_frame = 1;
-    R.L.tiles_x = (t->width + 7) / 8;
-    R.L.tiles_y = (t->height + 3) / 4;
-    R.L.out_rgba8 = rgba8 ? 1 : 0;
-    R.L.strip_shift = -1;
-    R.list = list;
-    R.count = counter;
+    if (!upload_uniform_block(c, v->inst[0].const_ptr, (CUstream_t)s)) return 1;
+    struct { PeLaunchHost L; const void* list; void* count; } R = {launch_record(c, t, out_device, nullptr, rgba8 != 0), list, counter};
     void* args[] = {&R};
     const unsigned gx = unsigned(c->sm_count * v->refine_blocks_per_sm);
-    CUresult_t r = c->drv->cuLaunchKernel(v->refine, gx, 1, 1, unsigned(c->opts.block_threads), 1, 1, 0, s, args, nullptr);
+    CUresult_t r = c->drv->cuLaunchKernel(v->refine, gx, 1, 1, unsigned(c->opts.block_threads), 1, 1, 0, (CUstream_t)s, args, nullptr);
     if (r != 0) return c->fail("cuLaunchKernel(pe_refine_kernel): " + driver_error(c->drv, r));
     c->launches++;
     return 0;
-}
-
-static bool ensure_scratch(pe_ctx* c, void** p, size_t* have, size_t need) {
-    if (*have >= need) return true;
-    if (*p) cudaFree(*p);
-    *p = nullptr;
-    *have = 0;
-    if (!cuda_ok(c, cudaMalloc(p, need), "cudaMalloc(staging)")) return false;
-    *have = need;
-    return true;
 }
 
 int pe_render_host(pe_ctx* c, const pe_target* t, float* out_host) {
@@ -1193,9 +750,9 @@ int pe_render_host(pe_ctx* c, const pe_target* t, float* out_host) {
     if (!out_host) return c->fail("pe_render_host: out_host is null");
     if (!check_target(c, t) || !bind_device(c)) return 1;
     size_t bytes = pe_target_pixels(t) * 16;
-    if (!ensure_scratch(c, &c->scratch_dev, &c->scratch_bytes, bytes)) return 1;
-    if (pe_render(c, t, c->scratch_dev, nullptr, nullptr)) return 1;
-    if (!cuda_ok(c, cudaMemcpyAsync(out_host, c->scratch_dev, bytes, cudaMemcpyDeviceToHost, c->stream), "D2H copy")) return 1;
+    if (!cuda_ok(c, c->staging.ensure(bytes), "cudaMalloc(staging)")) return 1;
+    if (pe_render(c, t, c->staging.dev, nullptr, nullptr)) return 1;
+    if (!cuda_ok(c, cudaMemcpyAsync(out_host, c->staging.dev, bytes, cudaMemcpyDeviceToHost, c->stream), "D2H copy")) return 1;
     return cuda_ok(c, cudaStreamSynchronize(c->stream), "pe_render_host") ? 0 : 1;
 }
 
@@ -1204,9 +761,9 @@ int pe_render_host_rgba8(pe_ctx* c, const pe_target* t, uint8_t* out_host) {
     if (!out_host) return c->fail("pe_render_host_rgba8: out_host is null");
     if (!check_target(c, t) || !bind_device(c)) return 1;
     size_t n = pe_target_pixels(t);
-    if (!ensure_scratch(c, &c->scratch8_dev, &c->scratch8_bytes, n * 4)) return 1;
-    if (render_impl(c, t, c->scratch8_dev, nullptr, nullptr, true)) return 1;
-    if (!cuda_ok(c, cudaMemcpyAsync(out_host, c->scratch8_dev, n * 4, cudaMemcpyDeviceToHost, c->stream), "D2H copy")) return 1;
+    if (!cuda_ok(c, c->staging8.ensure(n * 4), "cudaMalloc(staging)")) return 1;
+    if (render_impl(c, t, c->staging8.dev, nullptr, nullptr, true)) return 1;
+    if (!cuda_ok(c, cudaMemcpyAsync(out_host, c->staging8.dev, n * 4, cudaMemcpyDeviceToHost, c->stream), "D2H copy")) return 1;
     return cuda_ok(c, cudaStreamSynchronize(c->stream), "pe_render_host_rgba8") ? 0 : 1;
 }
 
@@ -1220,7 +777,7 @@ static bool ensure_pipeline(pe_ctx* c, size_t bytes) {
         }
     }
     for (auto& sl : c->slots)
-        if (!ensure_scratch(c, &sl.dev, &sl.bytes, bytes)) return false;
+        if (!cuda_ok(c, sl.buf.ensure(bytes), "cudaMalloc(staging)")) return false;
     return true;
 }
 
@@ -1236,11 +793,11 @@ static int submit_host(pe_ctx* c, const pe_target* t, uint8_t* out_host, uint64_
     auto& sl = c->slots[tk % PE_PIPELINE_DEPTH];
     // the slot's previous frame (ticket tk - depth) must have left the device before it is overwritten
     if (sl.ticket && !cuda_ok(c, cudaStreamWaitEvent(c->stream, sl.copied, 0), "pipeline wait")) return 1;
-    if (n && render_impl(c, &local, sl.dev, nullptr, nullptr, true)) return 1;
+    if (n && render_impl(c, &local, sl.buf.dev, nullptr, nullptr, true)) return 1;
     if (!cuda_ok(c, cudaEventRecord(sl.rendered, c->stream), "event record") ||
         !cuda_ok(c, cudaStreamWaitEvent(c->copy_stream, sl.rendered, 0), "pipeline wait")) return 1;
     if (!strips_into_frame) {
-        if (n && !cuda_ok(c, cudaMemcpyAsync(out_host, sl.dev, n * 4, cudaMemcpyDeviceToHost, c->copy_stream), "D2H copy")) return 1;
+        if (n && !cuda_ok(c, cudaMemcpyAsync(out_host, sl.buf.dev, n * 4, cudaMemcpyDeviceToHost, c->copy_stream), "D2H copy")) return 1;
     } else {
         // strip k of this rank = global strip strip_first + k * strip_step: contiguous rows of the row-major frame,
         // world strips apart from strip k + 1 -> ONE pitched copy for the whole strips (+ one for a ragged last strip)
@@ -1253,10 +810,10 @@ static int submit_host(pe_ctx* c, const pe_target* t, uint8_t* out_host, uint64_
             else ragged_rows = t->height - row0;
         }
         uint8_t* dst0 = out_host + size_t(t->strip_first) * strip_bytes;
-        if (full && !cuda_ok(c, cudaMemcpy2DAsync(dst0, strip_bytes * size_t(t->strip_step), sl.dev, strip_bytes, strip_bytes, size_t(full),
+        if (full && !cuda_ok(c, cudaMemcpy2DAsync(dst0, strip_bytes * size_t(t->strip_step), sl.buf.dev, strip_bytes, strip_bytes, size_t(full),
                                                   cudaMemcpyDeviceToHost, c->copy_stream), "D2H strip copy")) return 1;
         if (ragged_rows && !cuda_ok(c, cudaMemcpyAsync(dst0 + size_t(full) * strip_bytes * size_t(t->strip_step),
-                                                       (const uint8_t*)sl.dev + size_t(full) * strip_bytes, size_t(ragged_rows) * row_bytes,
+                                                       (const uint8_t*)sl.buf.dev + size_t(full) * strip_bytes, size_t(ragged_rows) * row_bytes,
                                                        cudaMemcpyDeviceToHost, c->copy_stream), "D2H strip copy")) return 1;
     }
     if (!cuda_ok(c, cudaEventRecord(sl.copied, c->copy_stream), "event record")) return 1;
@@ -1322,7 +879,7 @@ int pe_deinterleave_strips(pe_ctx* c, const void* gathered, void* frame, int wid
     if (!gathered || !frame || width <= 0 || height <= 0 || strip_rows <= 0 || n_ranks <= 0 || strips_per_rank <= 0)
         return c->fail("pe_deinterleave_strips: bad arguments");
     if (!bind_device(c)) return 1;
-    cudaStream_t s = stream ? (cudaStream_t)stream : c->stream;
+    const cudaStream_t s = stream_of(c, stream);
     if (!cuda_ok(c, (cudaError_t)launch_deinterleave(gathered, frame, width, height, strip_rows, n_ranks, strips_per_rank,
                                                     c->sm_count, s), "deinterleave")) return 1;
     c->launches++;
@@ -1344,14 +901,9 @@ int pe_device_free(pe_ctx* c, void* p) {
 int pe_scratch_buffer(pe_ctx* c, int slot, size_t bytes, void** out) {
     if (!c || !out || slot < 0 || slot >= 128) return c ? c->fail("pe_scratch_buffer: bad arguments") : 1;
     if (!bind_device(c)) return 1;
-    auto& s = c->user_scratch[slot];
-    if (s.bytes < bytes) {
-        // growing frees the old block: make sure nothing queued still uses it
-        if (s.dev) { cudaDeviceSynchronize(); cudaFree(s.dev); s.dev = nullptr; s.bytes = 0; }
-        if (!cuda_ok(c, cudaMalloc(&s.dev, bytes), "cudaMalloc(scratch)")) return 1;
-        s.bytes = bytes;
-    }
-    *out = s.dev;
+    DeviceBuffer& b = c->caller_slots[slot];
+    if (!cuda_ok(c, b.ensure(bytes), "cudaMalloc(scratch)")) return 1;
+    *out = b.dev;
     return 0;
 }
 
@@ -1365,24 +917,33 @@ int pe_autotune(pe_ctx* c, const pe_target* t, int reps, char* report, size_t re
     if (!check_target(c, t) || !bind_device(c)) return 1;
     if (c->opts.persistent) return 0;                       // the persistent scheduler has its own geometry: nothing to try
     if (reps < 1) reps = 3;
-    struct Cand { int block_threads, min_blocks; bool canon, w_aware; };
+    struct Cand {
+        int block_threads, min_blocks;
+        bool canon, w_aware;
+        void apply(GenOptions& o) const {
+            o.block_threads = block_threads;
+            o.min_blocks = min_blocks;
+            o.canon_rays = canon;
+            o.w_aware = w_aware;
+        }
+    };
     const Cand cands[] = {{512, 2, true, true}, {512, 2, true, false}, {512, 2, false, false}, {1024, 1, true, true}, {1024, 1, false, false}};
-    const GenOptions saved = c->opts;
-    void *scratch = nullptr, *first = nullptr;
     const size_t bytes = (pe_target_pixels(t) ? pe_target_pixels(t) : 1) * 16;
     // the guard: a candidate is only eligible if its frame is, bit for bit, the frame the first candidate (the default variant) gave
-    if (pe_scratch_buffer(c, 127, bytes, &scratch) || pe_scratch_buffer(c, 126, bytes, &first)) return 1;
+    if (!cuda_ok(c, c->tune_frame.ensure(bytes), "cudaMalloc(autotune frame)") ||
+        !cuda_ok(c, c->tune_guard.ensure(bytes), "cudaMalloc(autotune guard)")) return 1;
+    void *scratch = c->tune_frame.dev, *first = c->tune_guard.dev;
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     if (!cuda_ok(c, cudaEventCreate(&e0), "event") || !cuda_ok(c, cudaEventCreate(&e1), "event")) return 1;
     int best = -1;
     float best_ms = 0.0f;
     std::string rep;
     int rc = 0;
+    // the candidates change c->opts; on return `keep_opts` puts back the caller's options -- with the chosen candidate's
+    // launch shape once one is chosen
+    ScopedOverride<GenOptions> keep_opts(&c->opts);
     for (int k = 0; k < int(sizeof cands / sizeof *cands) && !rc; k++) {
-        c->opts.block_threads = cands[k].block_threads;
-        c->opts.min_blocks = cands[k].min_blocks;
-        c->opts.canon_rays = cands[k].canon;
-        c->opts.w_aware = cands[k].w_aware;
+        cands[k].apply(c->opts);
         c->current = nullptr;
         if (render_impl(c, t, scratch, nullptr, nullptr, false)) { rc = 1; break; }            // compile / load + warm-up
         cudaEventRecord(e0, c->stream);
@@ -1413,20 +974,10 @@ int pe_autotune(pe_ctx* c, const pe_target* t, int reps, char* report, size_t re
     cudaEventDestroy(e0);
     cudaEventDestroy(e1);
     cudaDeviceSynchronize();
-    for (int slot : {126}) {                                  // the guard's copy of the first frame is not kept around
-        auto it = c->user_scratch.find(slot);
-        if (it != c->user_scratch.end()) {
-            if (it->second.dev) cudaFree(it->second.dev);
-            c->user_scratch.erase(it);
-        }
-    }
-    c->opts = saved;
+    c->tune_guard.release();                                  // the guard's copy of the first frame is not kept around
     c->current = nullptr;
     if (rc) return 1;
-    c->opts.block_threads = cands[best].block_threads;
-    c->opts.min_blocks = cands[best].min_blocks;
-    c->opts.canon_rays = cands[best].canon;
-    c->opts.w_aware = cands[best].w_aware;
+    cands[best].apply(keep_opts.saved);
     char line[160];
     std::snprintf(line, sizeof line, "chosen: block_threads %d min_blocks %d canon_rays %d w_aware %d\n", cands[best].block_threads,
                   cands[best].min_blocks, cands[best].canon ? 1 : 0, cands[best].w_aware ? 1 : 0);
@@ -1441,9 +992,9 @@ int pe_frames_differ(pe_ctx* c, const void* a, const void* b, size_t bytes, void
     if (!bind_device(c)) return 1;
     *words_out = 0;
     if (bytes == 0) return 0;
-    cudaStream_t s = stream ? (cudaStream_t)stream : c->stream;
-    void* diff = nullptr;
-    if (pe_scratch_buffer(c, 125, 16, &diff)) return 1;
+    const cudaStream_t s = stream_of(c, stream);
+    if (!cuda_ok(c, c->diff_word.ensure(16), "cudaMalloc(difference word)")) return 1;
+    void* diff = c->diff_word.dev;
     if (!cuda_ok(c, cudaMemsetAsync(diff, 0, 16, s), "pe_frames_differ") ||
         !cuda_ok(c, (cudaError_t)launch_count_diff(a, b, bytes / 16, (unsigned*)diff, c->sm_count, s), "pe_frames_differ") ||
         !cuda_ok(c, cudaMemcpyAsync(words_out, diff, 4, cudaMemcpyDeviceToHost, s), "pe_frames_differ") ||
@@ -1455,7 +1006,7 @@ int pe_frames_differ(pe_ctx* c, const void* a, const void* b, size_t bytes, void
 int pe_memcpy_d2h(pe_ctx* c, void* dst, const void* src, size_t bytes, void* stream) {
     if (!c || !dst || !src) return 1;
     if (!bind_device(c)) return 1;
-    cudaStream_t s = stream ? (cudaStream_t)stream : c->stream;
+    const cudaStream_t s = stream_of(c, stream);
     if (!cuda_ok(c, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, s), "D2H copy")) return 1;
     return cuda_ok(c, cudaStreamSynchronize(s), "D2H copy") ? 0 : 1;
 }
@@ -1463,7 +1014,7 @@ int pe_memcpy_d2h(pe_ctx* c, void* dst, const void* src, size_t bytes, void* str
 int pe_signal_u32(pe_ctx* c, void* const* device_ptrs, int n, uint32_t value, void* stream) {
     if (!c || !device_ptrs) return 1;
     if (!bind_device(c)) return 1;
-    cudaStream_t s = stream ? (cudaStream_t)stream : c->stream;
+    const cudaStream_t s = stream_of(c, stream);
     if (!cuda_ok(c, (cudaError_t)launch_signal(device_ptrs, n, value, s), "signal")) return 1;
     c->launches++;
     return 0;
@@ -1472,7 +1023,7 @@ int pe_signal_u32(pe_ctx* c, void* const* device_ptrs, int n, uint32_t value, vo
 int pe_stream_wait_geq_u32(pe_ctx* c, void* local_device_ptr, uint32_t value, void* stream) {
     if (!c || !local_device_ptr) return 1;
     if (!bind_device(c)) return 1;
-    CUstream_t s = stream ? (CUstream_t)stream : (CUstream_t)c->stream;
+    const CUstream_t s = (CUstream_t)stream_of(c, stream);
     CUresult_t r = c->drv->cuStreamWaitValue32(s, (CUdeviceptr_t)local_device_ptr, value, 0 /* CU_STREAM_WAIT_VALUE_GEQ */);
     if (r != 0) return c->fail("cuStreamWaitValue32: " + driver_error(c->drv, r));
     return 0;
@@ -1481,7 +1032,7 @@ int pe_stream_wait_geq_u32(pe_ctx* c, void* local_device_ptr, uint32_t value, vo
 int pe_memset_u32(pe_ctx* c, void* device_ptr, uint32_t value, size_t count, void* stream) {
     if (!c || !device_ptr) return 1;
     if (!bind_device(c)) return 1;
-    CUstream_t s = stream ? (CUstream_t)stream : (CUstream_t)c->stream;
+    const CUstream_t s = (CUstream_t)stream_of(c, stream);
     CUresult_t r = c->drv->cuMemsetD32Async((CUdeviceptr_t)device_ptr, value, count, s);
     if (r != 0) return c->fail("cuMemsetD32Async: " + driver_error(c->drv, r));
     return cuda_ok(c, cudaStreamSynchronize((cudaStream_t)s), "memset") ? 0 : 1;
@@ -1516,7 +1067,7 @@ int pe_average_frames_rgba8(pe_ctx* c, const void* const* frames, int n_frames, 
     if (!c) return 1;
     if (!frames || !out || n_frames < 1) return c->fail("pe_average_frames_rgba8: bad arguments");
     if (!bind_device(c)) return 1;
-    cudaStream_t s = stream ? (cudaStream_t)stream : c->stream;
+    const cudaStream_t s = stream_of(c, stream);
     if (!cuda_ok(c, (cudaError_t)launch_average_rgba8(frames, n_frames, out, n_pixels, c->sm_count, s), "average")) return 1;
     c->launches++;
     return 0;
@@ -1526,7 +1077,7 @@ int pe_quantize_rgba8(pe_ctx* c, const void* in, void* out, size_t n_pixels, voi
     if (!c) return 1;
     if (!in || !out) return c->fail("pe_quantize_rgba8: bad arguments");
     if (!bind_device(c)) return 1;
-    cudaStream_t s = stream ? (cudaStream_t)stream : c->stream;
+    const cudaStream_t s = stream_of(c, stream);
     if (!cuda_ok(c, (cudaError_t)launch_quantize_rgba8(in, out, n_pixels, c->sm_count, s), "quantize")) return 1;
     c->launches++;
     return 0;

@@ -109,7 +109,7 @@ struct GenOptions {
     bool w_aware = true;   // `finite affine matrix * vec4` tests w for exactly 0 / 1 (folded where the compiler knows it): pe_glsl.cuh
     bool unroll_loops = true;  // false: `#pragma unroll 1` on every loop of the user snippets (smaller code, see DESIGN.md)
     // per slot of i[] / per scene matrix: 1 = read it from the constant block even when specialisation is on (slots whose
-    // value kept changing between renders, pe_api.cpp select_variant)
+    // value kept changing between renders, pe_program.cpp select_variant)
     std::vector<char> dynamic_ints, dynamic_mats;
 };
 

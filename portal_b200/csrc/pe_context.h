@@ -1,0 +1,142 @@
+// The context behind the C ABI's opaque `pe_ctx`, shared by pe_api.cpp (entry points, uniform block, launches) and
+// pe_program.cpp (NVRTC, the cubin cache, variant selection, module load and unload).  Not part of the C ABI.
+#pragma once
+#include <cuda_runtime.h>
+
+#include <map>
+#include <memory>
+#include <string>
+#include <vector>
+
+#include "../../include/portal_b200.h"
+#include "pe_codegen.h"
+#include "pe_driver.h"
+
+namespace pe_host {
+
+// One loaded copy of a variant's cubin: its render kernel and its own uniform block on the device.
+struct ProgramInstance {
+    CUmodule_t module = nullptr;
+    CUfunction_t kernel = nullptr;
+    CUdeviceptr_t const_ptr = 0;
+};
+
+struct Variant {
+    std::string source;
+    std::vector<char> cubin;
+    // inst[1] is a second load of the same cubin, with its own copy of the uniform block: two frames of one context can then
+    // be in flight at once (on two streams) -- frame f + 1's uniforms are uploaded while frame f's kernel still reads its own.
+    ProgramInstance inst[2];
+    CUfunction_t probe = nullptr;    // pe_probe_kernel of inst[0] (programs generated with_probe)
+    CUfunction_t refine = nullptr;   // pe_refine_kernel of inst[0] (programs generated with_refine)
+    int refine_blocks_per_sm = 1;
+    int blocks_per_sm = 1;
+};
+
+// Device memory owned by a context, grown (never shrunk) on demand and freed with the context.
+struct DeviceBuffer {
+    void* dev = nullptr;
+    size_t bytes = 0;
+
+    DeviceBuffer() = default;
+    DeviceBuffer(const DeviceBuffer&) = delete;
+    DeviceBuffer& operator=(const DeviceBuffer&) = delete;
+    ~DeviceBuffer() { release(); }
+
+    // At least `need` bytes; growing does not keep the contents.
+    cudaError_t ensure(size_t need) {
+        if (bytes >= need) return cudaSuccess;
+        if (dev) {
+            cudaDeviceSynchronize();   // growing frees the old block: make sure nothing queued still uses it
+            release();
+        }
+        cudaError_t e = cudaMalloc(&dev, need);
+        if (e != cudaSuccess) dev = nullptr;
+        else bytes = need;
+        return e;
+    }
+    void release() {
+        if (dev) cudaFree(dev);
+        dev = nullptr;
+        bytes = 0;
+    }
+};
+
+}  // namespace pe_host
+
+struct pe_ctx {
+    int device = -1;
+    bool has_gpu = false;
+    int sm_count = 132;
+    std::string err;
+
+    pe_host::SceneDesc scene;
+    pe_host::ConstLayout layout;
+    bool layout_valid = false;
+    // slots of the renderer uniforms the render path reads or writes, resolved when the layout is made (floats, then ints)
+    int slot_resolution_x = 0, slot_resolution_y = 0, slot_tan_half_view = 0;
+    int slot_aa_count = 0, slot_aa_start = 0, slot_ray_tracing_depth = 0;
+    pe_host::GenOptions opts;
+    bool lineinfo = true;
+
+    std::vector<uint8_t> cblock;  // host image of the constant block
+    std::map<std::string, std::vector<float>> pending_mat;
+    std::map<std::string, float> pending_f;
+    std::map<std::string, int> pending_i;
+
+    std::map<std::vector<int>, std::unique_ptr<pe_host::Variant>> variants;  // key: specialised ints + matrix structure masks
+    pe_host::Variant* current = nullptr;
+    std::map<std::string, pe_host::DeviceBuffer> textures;
+
+    cudaStream_t stream = nullptr;
+    pe_host::DeviceBuffer queue;                 // the persistent scheduler's tile counter
+    pe_host::DeviceBuffer staging, staging8;     // pe_render_host / pe_render_host_rgba8 readback (staging8: also the probe's)
+    // pe_submit_host_rgba8 pipeline
+    struct Slot { pe_host::DeviceBuffer buf; cudaEvent_t rendered = nullptr, copied = nullptr; uint64_t ticket = 0; };
+    Slot slots[PE_PIPELINE_DEPTH];
+    pe_host::DeviceBuffer caller_slots[128];     // pe_scratch_buffer: the caller's alone
+    // the library's own intermediates: pe_render_adaptive's pixel list and its count + refill cursor, pe_frames_differ's
+    // difference word, pe_autotune's timing frame and its guard's copy of the first candidate's frame
+    pe_host::DeviceBuffer refine_list, refine_count, diff_word, tune_frame, tune_guard;
+    // adaptive de-specialisation: a slot whose value differed between renders more than kMaxRespecialisations times is read
+    // from the constant block from then on (bounds NVRTC compiles when an animation drives an int or a matrix structure)
+    std::vector<int> last_ints, int_changes;
+    std::vector<std::pair<unsigned, unsigned>> last_masks;
+    std::vector<int> mat_changes;
+    bool adapt = true;
+    cudaStream_t copy_stream = nullptr;
+    uint64_t next_ticket = 0;
+    uint64_t launches = 0;
+    const pe_host::DriverApi* drv = nullptr;
+    // Uniform uploads go through a ring of PINNED staging images: cuMemcpyHtoDAsync from pageable memory first synchronises the
+    // stream (CUDA's documented behaviour), which made every frame's upload wait for the previous frame's kernel -- the host
+    // could never run ahead, and the frame pipelines (pe_submit_host_*, two frames in flight) were serialised by it.
+    static constexpr int kStage = 16;
+    uint8_t* ustage = nullptr;
+    size_t ustage_stride = 0;
+    cudaEvent_t ustage_done[kStage] = {nullptr};
+    bool ustage_used[kStage] = {false};
+    int ustage_next = 0;
+
+    int fail(const std::string& m, int code = 1) {
+        err = m;
+        return code;
+    }
+};
+
+namespace pe_host {
+
+// pe_api.cpp: build the layout and the default uniform block on first use.
+void ensure_layout(pe_ctx* c);
+
+// pe_program.cpp.  Make the variant for the current uniforms current (generate / compile / load instance 0 as needed).
+// Beyond what the context's options ask for, a call may need the probe or the refine kernel.  `counted`: the uniforms are
+// the caller's, so their changes count toward adaptive de-specialisation; a call that overrides a uniform for itself
+// passes false.
+bool select_variant(pe_ctx* c, bool need_probe = false, bool need_refine = false, bool counted = true);
+// Load program instance k of `v` (0 or 1) unless it is loaded.
+bool load_instance(pe_ctx* c, Variant& v, int k);
+// Wait for the device, unload every variant but `keep` (nullptr: all) and forget them.
+void unload_variants(pe_ctx* c, const Variant* keep);
+
+}  // namespace pe_host
