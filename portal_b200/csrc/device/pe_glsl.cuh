@@ -597,6 +597,10 @@ template <unsigned Z, unsigned O, unsigned F> struct pe_canon_matrix<smat4<Z, O,
 #ifndef PE_W_AWARE
 #define PE_W_AWARE 1
 #endif
+// Declared ahead of its definition below: `mat4 * smat4` and `cmat4 * smat4` fall back to it, and their call does not depend
+// on the template parameters, so it is looked up where the templates are defined (a snippet's `m * u_mat` with a local
+// mat4 m failed to compile without this).
+PE_FI mat4 operator*(const mat4& a, const mat4& b);
 template <unsigned Z, unsigned O, unsigned F>
 PE_FI vec4 operator*(const smat4<Z, O, F>& m, const vec4& v) {
 #if PE_W_AWARE

@@ -29,14 +29,16 @@ def nvrtc_library():
     return os.path.join(cuda, "lib64", "libnvrtc.so.12")
 
 
-def compile_probe(options=None, include_dir=None):
-    """glsl_probe.cu -> sm_90a cubin bytes (options: OPTIONS; include_dir: the product's device headers)."""
+def compile_probe(options=None, include_dir=None, source=PROBE_SRC, extra=()):
+    """A probe source (glsl_probe.cu by default) -> sm_90a cubin bytes (options: OPTIONS; include_dir: the product's device
+    headers; extra: further options of this probe, such as its own include directory or a -D)."""
     nv = C.CDLL(nvrtc_library())
-    with open(PROBE_SRC, "rb") as f:
+    with open(source, "rb") as f:
         src = f.read()
     prog = C.c_void_p()
-    assert nv.nvrtcCreateProgram(C.byref(prog), src, b"glsl_probe.cu", 0, None, None) == 0
+    assert nv.nvrtcCreateProgram(C.byref(prog), src, os.path.basename(source).encode(), 0, None, None) == 0
     opts = [o.encode() for o in (OPTIONS if options is None else options)] + [b"--include-path=" + (include_dir or DEVICE_DIR).encode()]
+    opts += [o.encode() for o in extra]
     arr = (C.c_char_p * len(opts))(*opts)
     rc = nv.nvrtcCompileProgram(prog, len(opts), arr)
     size = C.c_size_t()
@@ -56,16 +58,17 @@ def compile_probe(options=None, include_dir=None):
 class Probe:
     """The probe's kernels, launched on torch's current stream of cuda:0."""
 
-    def __init__(self, torch, options=None, include_dir=None):
+    def __init__(self, torch, options=None, include_dir=None, source=PROBE_SRC, extra=(),
+                 kernels=("accuracy_unary", "accuracy_binary", "eval_unary", "eval_binary")):
         self.torch = torch
         torch.cuda.init()
         torch.empty(1, device="cuda")                         # makes torch's primary context current on this thread
         self.cu = C.CDLL("libcuda.so.1")
-        self._cubin = compile_probe(options, include_dir)
+        self._cubin = compile_probe(options, include_dir, source, extra)
         self.mod = C.c_void_p()
         self._check(self.cu.cuModuleLoadData(C.byref(self.mod), self._cubin))
         self.fns = {}
-        for name in ("accuracy_unary", "accuracy_binary", "eval_unary", "eval_binary"):
+        for name in kernels:
             f = C.c_void_p()
             self._check(self.cu.cuModuleGetFunction(C.byref(f), self.mod, name.encode()))
             self.fns[name] = f
