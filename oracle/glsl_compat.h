@@ -611,7 +611,7 @@ static inline vec4 texture(const sampler2D& s, const vec2& uv) {
     // keep the float->int conversion defined for wild coordinates
     x0 = clamp(x0, real(-2), real(s.w + 1));
     y0 = clamp(y0, real(-2), real(s.h + 1));
-    int ix = int(x0), iy = int(y0);
+    int ix = pe_int(x0), iy = pe_int(y0);   // the clamp keeps NaN: pe_int maps it to 0 (fx or fy is NaN then too)
     vec4 c00 = pe_texel(s, ix, iy), c10 = pe_texel(s, ix + 1, iy);
     vec4 c01 = pe_texel(s, ix, iy + 1), c11 = pe_texel(s, ix + 1, iy + 1);
     vec4 top = c00 * (real(1) - fx) + c10 * fx;

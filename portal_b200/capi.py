@@ -22,6 +22,7 @@ class PeTarget(C.Structure):
 
 PH_PROBE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double),
                           C.POINTER(C.c_int32), C.POINTER(C.c_int32))
+PH_UPDATE_HOOK = C.CFUNCTYPE(C.c_int, C.c_void_p)
 
 
 class PhFrameParams(C.Structure):

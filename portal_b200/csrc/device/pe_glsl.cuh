@@ -709,7 +709,7 @@ PE_FI vec4 texture(const sampler2D& s, const vec2& uv) {
     float fx = x - x0, fy = y - y0;
     x0 = clamp(x0, -2.0f, float(s.w + 1));
     y0 = clamp(y0, -2.0f, float(s.h + 1));
-    int ix = int(x0), iy = int(y0);
+    int ix = pe_int(x0), iy = pe_int(y0);   // the clamp keeps NaN: pe_int maps it to 0 (fx or fy is NaN then too)
     vec4 c00 = pe_texel(s, ix, iy), c10 = pe_texel(s, ix + 1, iy);
     vec4 c01 = pe_texel(s, ix, iy + 1), c11 = pe_texel(s, ix + 1, iy + 1);
     vec4 top = c00 * (1.0f - fx) + c10 * fx;

@@ -531,11 +531,15 @@ int pe_set_texture(pe_ctx* c, const char* name, const uint8_t* rgba8, int w, int
     if (!bind_device(c)) return 1;
     DeviceBuffer& t = c->textures[name];
     size_t bytes = size_t(w) * size_t(h) * 4;
-    cudaStreamSynchronize(c->stream);
+    // The old image may still be read by a render queued on any stream (a caller's, the pe_submit_host_* pipeline's, a
+    // sharder lane's), not only c->stream: wait for the device before freeing it, as DeviceBuffer::ensure does.
+    // If that wait fails the old image stays allocated and bound.
+    if (t.dev && !cuda_ok(c, cudaDeviceSynchronize(), "pe_set_texture: waiting for queued renders")) return 1;
     t.release();
+    uint8_t* rec = c->cblock.data() + c->layout.off_tex + size_t(it->second) * 16;
+    std::memset(rec, 0, 16);   // until the new image is in place the sampler is unbound, never the freed image
     if (!cuda_ok(c, t.ensure(bytes), "cudaMalloc(texture)")) return 1;
     if (!cuda_ok(c, cudaMemcpy(t.dev, rgba8, bytes, cudaMemcpyHostToDevice), "cudaMemcpy(texture)")) return 1;
-    uint8_t* rec = c->cblock.data() + c->layout.off_tex + size_t(it->second) * 16;
     std::memcpy(rec, &t.dev, 8);
     std::memcpy(rec + 8, &w, 4);
     std::memcpy(rec + 12, &h, 4);

@@ -193,6 +193,25 @@ class HostPlayer:
         self._probe_cb = capi.PH_PROBE_FN(tramp)         # keep the trampoline alive
         self._check(self._lib.ph_player_set_probe(self._p, C.cast(self._probe_cb, C.c_void_p), None))
 
+    def set_update_hook(self, fn):
+        """fn() after every update the player performs (update() and each motion-blur sub-frame), before the frame's
+        uniforms go up: the place to bind the current frame of each video (video_frame_index + pe_set_texture).  An
+        exception aborts the call; None detaches."""
+        if fn is None:
+            self._check(self._lib.ph_player_set_update_hook(self._p, None, None))
+            self._hook_cb = None
+            return
+
+        def tramp(_user):
+            try:
+                fn()
+                return 0
+            except Exception:                       # noqa: BLE001 -- must not propagate through the C frame
+                return 1
+
+        self._hook_cb = capi.PH_UPDATE_HOOK(tramp)       # keep the trampoline alive
+        self._check(self._lib.ph_player_set_update_hook(self._p, C.cast(self._hook_cb, C.c_void_p), None))
+
     def set_run_animations(self, on: bool):
         self._check(self._lib.ph_player_set_run_animations(self._p, int(on)))
 

@@ -4,8 +4,8 @@ ONE frame of a clip: frame index = round((frames - 1) * clamp(uniform, 0, 1)) (s
 Decoding the clip (ffmpeg -> PNG, video.rs:65-110) is image IO and out of scope; what is in scope and checked here, on
 `tests/fixtures/video.ron` (hand-written): both front-ends read the `videos:` section, declare the sampler, agree on the
 uniform table and on the frame index at every time; the generated sm_90a program, run on the host harness with the selected
-frame bound, gives the oracle's pixels bit for bit; an unbound video sampler reads black.  (No GPU needed: the GPU side is
-`pe_set_texture` + a render, which the texture scenes of tests/test_all_scenes_gpu.py cover.)"""
+frame bound, gives the oracle's pixels bit for bit; an unbound video sampler reads black.  (No GPU needed: the GPU side,
+replacing the image between frames and the player's update hook, is tests/test_video_gpu.py.)"""
 import os
 
 import numpy as np
