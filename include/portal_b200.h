@@ -185,11 +185,25 @@ PE_API int pe_host_free(pe_ctx* ctx, void* p);
  * So  adaptive(T) == where(mask_T(F1), F_N, F1)  bit for bit; T < 0 gives F_N, T = 255 gives F1, N = 1 gives pe_render.
  * `rgba8` selects the output format of `out_device` (0: float RGBA, 16 B/pixel; 1: RGBA8).  `refined_count_device`
  * (optional, device uint32) receives the number of refined pixels.  Enqueues three kernel launches on `stream` (NULL: the
- * context's stream) and returns without synchronising.  Only whole-frame targets ({w, h, h, 0, 1, 1, layout}) are accepted;
- * n_strips == 0 renders nothing and succeeds.
+ * context's stream) and returns without synchronising.  Only whole-frame targets ({w, h, h, 0, 1, 1, layout}) are accepted
+ * (pe_render_adaptive_strips takes strip targets); n_strips == 0 renders nothing and succeeds.
  * The first call for a scene compiles a second program (the render program plus pe_refine_kernel, option "with_refine"). */
 PE_API int pe_render_adaptive(pe_ctx* ctx, const pe_target* target, int threshold, int rgba8, void* out_device,
                               void* refined_count_device, void* stream);
+/* Adaptive anti-aliasing of any target, strips of a sharded frame included.  For every pixel p of `target` it writes exactly
+ * where(mask_T(F1), F_N, F1)[p] of the WHOLE frame, the rule pe_render_adaptive states: the 3x3 window of a pixel on a
+ * strip's first or last row reads the neighbouring row of the whole frame even when another rank renders that row, and is
+ * clipped only at the frame's own edges.  So the strips of a split, each rendered here, assemble into pe_render_adaptive's
+ * frame bit for bit.  `refined_count_device` (optional) receives the number of refined pixels of this target; summed over
+ * the targets of a split it is the whole frame's count.
+ * The neighbouring rows that are not the target's own ("halo" rows: row g*S - 1 above and (g+1)*S below each global strip g,
+ * inside the frame; with strip_step 1 only above the first and below the last strip) are rendered by this call, at one
+ * sample and as RGBA8, into buffers the context owns -- never a pe_scratch_buffer slot.  That costs at most 2 / strip_rows of
+ * the one-sample pass and at most two more kernel launches: five in all for a strip target, three (as pe_render_adaptive)
+ * for a whole-frame target.  Accepts every target pe_render does; n_strips == 0 renders nothing, writes no count and
+ * succeeds.  Asynchronous on `stream` (NULL: the context's stream). */
+PE_API int pe_render_adaptive_strips(pe_ctx* ctx, const pe_target* target, int threshold, int rgba8, void* out_device,
+                                     void* refined_count_device, void* stream);
 /* Camera-teleportation probe (replaces teleport_external_ray, src/main.rs:1361-1409 +
  * src/frag.glsl:166-257, 527-547): follow the segment a -> b through the scene's portals (at most
  * 10, `teleport_light_u` forced on) and return where its end point lands -- directly, instead of
@@ -271,6 +285,13 @@ PE_API int pe_sharder_release(pe_sharder* s, void* stream);
  * first): the caller consumes frames one call late.  pe_sharder_flush orders `stream` after the last frame as well. */
 PE_API int pe_sharder_render_overlapped(pe_sharder* s, void* stream, void** prev_frame_out);
 PE_API int pe_sharder_flush(pe_sharder* s, void* stream, void** last_frame_out);
+/* Adaptive anti-aliasing for this rank's strips from the next frame on (on != 0), in every mode: each rank renders its
+ * strips with pe_render_adaptive_strips(threshold) and the assembled frame is pe_render_adaptive's whole frame bit for bit.
+ * Every rank must set the same `threshold` (and the same uniforms, `_aa_count` included).  OWNER: the adaptive strips go
+ * into the ring buffer; overlapped, each lane uses its own program instance and list / halo buffers.  P2P: the strips are
+ * rendered into a local compact buffer and then copied into rank 0's frame with one pitched copy, before the frame is
+ * signalled.  HOST: the device slot holds the adaptive RGBA8 strips.  Off (on == 0) is the default. */
+PE_API int pe_sharder_set_adaptive_aa(pe_sharder* s, int on, int threshold);
 /* HOST: queue this rank's strips of the next frame (returns its number); block until they are in host memory and publish;
  * rank 0: block until every rank's strips of a frame have landed (*frame = the whole RGBA8 frame); give its slot back. */
 PE_API int pe_sharder_submit(pe_sharder* s, uint64_t* frame_no);

@@ -90,6 +90,7 @@ def lib() -> C.CDLL:
         "pe_host_malloc": (i32, [vp, C.c_size_t, C.POINTER(vp)]),
         "pe_host_free": (i32, [vp, vp]),
         "pe_render_adaptive": (i32, [vp, C.POINTER(PeTarget), i32, i32, vp, vp, vp]),
+        "pe_render_adaptive_strips": (i32, [vp, C.POINTER(PeTarget), i32, i32, vp, vp, vp]),
         "pe_probe_ray": (i32, [vp, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_int32),
                                C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
         "pe_autotune": (i32, [vp, C.POINTER(PeTarget), i32, cp, C.c_size_t]),
@@ -118,6 +119,7 @@ def lib() -> C.CDLL:
         "pe_sharder_release": (i32, [vp, vp]),
         "pe_sharder_render_overlapped": (i32, [vp, vp, C.POINTER(vp)]),
         "pe_sharder_flush": (i32, [vp, vp, C.POINTER(vp)]),
+        "pe_sharder_set_adaptive_aa": (i32, [vp, i32, i32]),
         "pe_sharder_submit": (i32, [vp, C.POINTER(C.c_uint64)]),
         "pe_sharder_complete": (i32, [vp, C.c_uint64]),
         "pe_sharder_wait_frame": (i32, [vp, C.c_uint64, C.POINTER(vp)]),

@@ -503,19 +503,19 @@ PE_FI void render_pixel(const PeLaunch& L, int px, int lrow, int grow) {
 #endif
 
 #if PE_WITH_REFINE
-// Adaptive anti-aliasing, second pass (pe_render_adaptive): re-render the pixels of a list with all `_aa_count` samples.
-// The list (packed (y << 16) | x, whole-frame coordinates) and its length come from pe_k_refine_list (pe_kernels.cu).
+// Adaptive AA, second pass: the listed pixels ((local_row << 16) | x, from pe_k_refine_list) with all `_aa_count` samples.
 struct PeRefine {
-    PeLaunch L;              // whole-frame target: local row == global row
+    PeLaunch L;              // the one-sample frame's target (pe_render_adaptive: the whole frame; _strips: any target)
     const unsigned* list;
     unsigned* count;         // [0] list length, [1] refill cursor (zeroed by the host before the list is built)
 };
 namespace pe {
-// List entry i: all samples of its pixel, stored over the one-sample value
-PE_FI void refine_entry(const PeRefine& R, unsigned i) {
+PE_FI void refine_entry(const PeRefine& R, unsigned i) {   // entry i: all samples of its pixel, over the one-sample value
     const unsigned p = R.list[i];
-    const int px = int(p & 0xffffu), y = int(p >> 16);
-    render_pixel(R.L, px, y, y);
+    const int px = int(p & 0xffffu), lrow = int(p >> 16);
+    int grow = lrow;
+    local_to_global_row(R.L, lrow, grow);                  // the render kernel's row mapping; listed pixels are in the frame
+    render_pixel(R.L, px, lrow, grow);
 }
 }  // namespace pe
 // Warp refill from an atomic cursor, as in the persistent scheduler: a warp takes the next 32 list entries when all of its

@@ -5,6 +5,7 @@
 // (/root/reference/src/main.rs:934-1064 new, :1266-1359 set_uniforms, :1411-1428 draw_texture,
 // /root/reference/src/gui/scene.rs:545-658 Scene::set_uniforms, :1112-1176 get_new_material).
 // There is NO CPU rendering path in this library: without a CUDA device pe_render* fail.
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -582,10 +583,9 @@ bool upload_uniform_block(pe_ctx* c, CUdeviceptr_t dst, CUstream_t s) {
     return true;
 }
 
-// The render kernel's launch record for a render of `t` into `out`.  pe_refine_kernel takes the same record for its
-// whole-frame target: it reads only out, width, out_rgba8, bounces and the store index, and with local row == global row
-// the store index does not depend on the layout flag.  tiles_x / tiles_y count the persistent scheduler's 8x4-pixel tiles,
-// a fixed size in device/pe_kernel.cuh.
+// The render kernel's launch record for a render of `t` into `out`.  pe_refine_kernel takes the same record: it maps a
+// list entry's local row to its global row as the render kernel does.  tiles_x / tiles_y count the persistent scheduler's
+// 8x4-pixel tiles, a fixed size in device/pe_kernel.cuh.
 PeLaunchHost launch_record(pe_ctx* c, const pe_target* t, void* out, void* bounces, bool rgba8) {
     PeLaunchHost L;
     std::memset(&L, 0, sizeof L);
@@ -653,6 +653,87 @@ int render_impl(pe_ctx* c, const pe_target* t, void* out_device, void* bounces_d
     return 0;
 }
 
+// The strips of a target that hold frame rows (the last may be ragged) and the local rows they span.
+void visible_strips(const pe_target* t, int& n_vis, int& local_rows) {
+    n_vis = 0;
+    local_rows = 0;
+    for (int k = 0; k < t->n_strips; k++) {
+        const long long row0 = ((long long)t->strip_first + (long long)k * t->strip_step) * t->strip_rows;
+        if (row0 >= t->height) break;
+        n_vis = k + 1;
+        local_rows = k * t->strip_rows + int(std::min<long long>(t->strip_rows, t->height - row0));
+    }
+}
+
+// Adaptive anti-aliasing of target `t` through program instance `instance` and its own list / halo buffers: the one-sample
+// frame, its RGBA8 halo rows (the frame rows next to the target's strips that are not the target's own), the list of edge
+// pixels, and every listed pixel rendered again with all `_aa_count` samples by the program's pe_refine_kernel (the render
+// kernel's own per-pixel code).  Whole-frame target: three launches, no halo.  The caller has checked the target.
+int render_adaptive_impl(pe_ctx* c, const pe_target* t, int threshold, bool rgba8, void* out_device, void* refined_count_device,
+                         cudaStream_t s, int instance) {
+    ensure_layout(c);
+    pe_ctx::AdaptiveBuffers& B = c->adaptive[instance];
+    int n_vis = 0, local_rows = 0;
+    visible_strips(t, n_vis, local_rows);
+    // halo rows, each set a target of 1-row strips: above strip i is row (strip_first + i * step) * S - 1, below it
+    // (strip_first + i * step + 1) * S; strip_step 1 (adjacent strips): only above the first and below the last strip
+    const int S = t->strip_rows, step = t->strip_step;
+    const bool adjacent = step == 1;
+    const int above_first = t->strip_first == 0 ? 1 : 0;   // no row above global strip 0
+    const int above_n = adjacent ? (n_vis > 0 && t->strip_first > 0 ? 1 : 0) : std::max(n_vis - above_first, 0);
+    int below_n = 0;
+    for (int k = adjacent ? n_vis - 1 : 0; k >= 0 && k < n_vis; k++)
+        if (((long long)t->strip_first + (long long)k * step + 1) * S < t->height) below_n++;
+        else break;                                          // the first strip whose next row is past the frame ends them
+    const pe_target above = {t->width, t->height, 1, (t->strip_first + above_first * step) * S - 1, step * S, above_n, 0};
+    const pe_target below = {t->width, t->height, 1, (t->strip_first + (adjacent ? n_vis - 1 : 0) + 1) * S, step * S, below_n, 0};
+    const size_t row_bytes = size_t(t->width) * 4;
+    if (!cuda_ok(c, B.halo_above.ensure(std::max(above_n, 1) * row_bytes), "cudaMalloc(halo rows)") ||
+        !cuda_ok(c, B.halo_below.ensure(std::max(below_n, 1) * row_bytes), "cudaMalloc(halo rows)")) return 1;
+    {
+        // (1) the one-sample frame, straight into the caller's buffer: exactly pe_render(_rgba8) with `_aa_count` = 1, and
+        // its halo rows as RGBA8 (the mask reads unorm8 values; pe_render_rgba8 == pe_quantize_rgba8(pe_render)).  The
+        // override is not a scene change for the specialisation tracker (as `teleport_light_u` in pe_probe_ray).
+        ScopedOverride<int> one_sample(islot(c, c->slot_aa_count), 1);
+        if (render_impl(c, t, out_device, nullptr, s, rgba8, instance, /*counted=*/false)) return 1;
+        if (above_n && render_impl(c, &above, B.halo_above.dev, nullptr, s, true, instance, false)) return 1;
+        if (below_n && render_impl(c, &below, B.halo_below.dev, nullptr, s, true, instance, false)) return 1;
+    }
+
+    // (2) the list of pixels to refine: packed (local row, x), and their count + refill cursor
+    if (!cuda_ok(c, B.refine_list.ensure(std::max<size_t>(size_t(local_rows) * size_t(t->width), 1) * 4), "cudaMalloc(refine list)") ||
+        !cuda_ok(c, B.refine_count.ensure(16), "cudaMalloc(refine count)")) return 1;
+    unsigned* list = (unsigned*)B.refine_list.dev;
+    unsigned* counter = (unsigned*)B.refine_count.dev;
+    if (!cuda_ok(c, cudaMemsetAsync(counter, 0, 16, s), "adaptive anti-aliasing: counter reset")) return 1;
+    const RefineTarget rt = {t->width, t->height, S, t->strip_first, step, t->n_strips, t->full_frame_layout ? 1 : 0, local_rows};
+    if (local_rows > 0) {
+        if (!cuda_ok(c, (cudaError_t)launch_refine_list(out_device, rgba8, rt, (const unsigned*)B.halo_above.dev, above_first,
+                                                         (const unsigned*)B.halo_below.dev, threshold, list, counter, s),
+                     "adaptive anti-aliasing: refine list"))
+            return 1;
+        c->launches++;
+    }
+    if (refined_count_device &&
+        !cuda_ok(c, cudaMemcpyAsync(refined_count_device, counter, 4, cudaMemcpyDeviceToDevice, s), "refined count copy"))
+        return 1;
+
+    // (3) the refine pass: the same program with pe_refine_kernel, `_aa_count` = N, through the same instance
+    if (!select_variant(c, false, /*need_refine=*/true)) return 1;
+    update_derived(c);
+    Variant* v = c->current;
+    if (!load_instance(c, *v, instance)) return 1;
+    if (!upload_uniform_block(c, v->inst[instance].const_ptr, (CUstream_t)s)) return 1;
+    struct { PeLaunchHost L; const void* list; void* count; } R = {launch_record(c, t, out_device, nullptr, rgba8), list, counter};
+    void* args[] = {&R};
+    const unsigned gx = unsigned(c->sm_count * v->refine_blocks_per_sm);
+    CUresult_t r = c->drv->cuLaunchKernel(v->inst[instance].refine, gx, 1, 1, unsigned(c->opts.block_threads), 1, 1, 0, (CUstream_t)s,
+                                          args, nullptr);
+    if (r != 0) return c->fail("cuLaunchKernel(pe_refine_kernel): " + driver_error(c->drv, r));
+    c->launches++;
+    return 0;
+}
+
 }  // namespace
 
 int pe_internal_render(pe_ctx* c, const pe_target* t, void* out_device, void* stream, int rgba8, int instance) {
@@ -700,8 +781,6 @@ int pe_probe_ray(pe_ctx* c, const float a[3], const float b[3], float pos_out[3]
     return 0;
 }
 
-// Adaptive anti-aliasing: a one-sample frame, the list of its edge pixels, and every listed pixel rendered again with all
-// `_aa_count` samples by the program's pe_refine_kernel (the render kernel's own per-pixel code).
 int pe_render_adaptive(pe_ctx* c, const pe_target* t, int threshold, int rgba8, void* out_device, void* refined_count_device,
                        void* stream) {
     if (!c) return 1;
@@ -709,44 +788,18 @@ int pe_render_adaptive(pe_ctx* c, const pe_target* t, int threshold, int rgba8, 
     if (!check_target(c, t) || !bind_device(c)) return 1;
     if (t->n_strips == 0) return 0;   // nothing of this frame belongs to the caller
     if (t->strip_first != 0 || t->n_strips != 1 || t->strip_rows < t->height)
-        return c->fail("pe_render_adaptive: only whole-frame targets ({w, h, h, 0, 1, 1, layout}) are supported -- the 3x3 edge "
-                       "window of a pixel crosses strip boundaries");
-    ensure_layout(c);
-    const cudaStream_t s = stream_of(c, stream);
-    {
-        // (1) the one-sample frame, straight into the caller's buffer: exactly pe_render(_rgba8) with `_aa_count` = 1.  The
-        // override is not a scene change for the specialisation tracker (as `teleport_light_u` in pe_probe_ray).
-        ScopedOverride<int> one_sample(islot(c, c->slot_aa_count), 1);
-        if (render_impl(c, t, out_device, nullptr, s, rgba8 != 0, 0, /*counted=*/false)) return 1;
-    }
+        return c->fail("pe_render_adaptive: only whole-frame targets ({w, h, h, 0, 1, 1, layout}) are supported -- use "
+                       "pe_render_adaptive_strips for strip targets");
+    return render_adaptive_impl(c, t, threshold, rgba8 != 0, out_device, refined_count_device, stream_of(c, stream), 0);
+}
 
-    // (2) the list of pixels to refine: packed pixel indices, and their count + refill cursor
-    const size_t n_px = size_t(t->width) * size_t(t->height);
-    if (!cuda_ok(c, c->refine_list.ensure(n_px * 4), "cudaMalloc(refine list)") ||
-        !cuda_ok(c, c->refine_count.ensure(16), "cudaMalloc(refine count)")) return 1;
-    unsigned* list = (unsigned*)c->refine_list.dev;
-    unsigned* counter = (unsigned*)c->refine_count.dev;
-    if (!cuda_ok(c, cudaMemsetAsync(counter, 0, 16, s), "pe_render_adaptive: counter reset")) return 1;
-    if (!cuda_ok(c, (cudaError_t)launch_refine_list(out_device, rgba8 != 0, t->width, t->height, threshold, list, counter, s),
-                 "pe_render_adaptive: refine list"))
-        return 1;
-    c->launches++;
-    if (refined_count_device &&
-        !cuda_ok(c, cudaMemcpyAsync(refined_count_device, counter, 4, cudaMemcpyDeviceToDevice, s), "refined count copy"))
-        return 1;
-
-    // (3) the refine pass: the same program with pe_refine_kernel, `_aa_count` = N
-    if (!select_variant(c, false, /*need_refine=*/true)) return 1;
-    update_derived(c);
-    Variant* v = c->current;
-    if (!upload_uniform_block(c, v->inst[0].const_ptr, (CUstream_t)s)) return 1;
-    struct { PeLaunchHost L; const void* list; void* count; } R = {launch_record(c, t, out_device, nullptr, rgba8 != 0), list, counter};
-    void* args[] = {&R};
-    const unsigned gx = unsigned(c->sm_count * v->refine_blocks_per_sm);
-    CUresult_t r = c->drv->cuLaunchKernel(v->refine, gx, 1, 1, unsigned(c->opts.block_threads), 1, 1, 0, (CUstream_t)s, args, nullptr);
-    if (r != 0) return c->fail("cuLaunchKernel(pe_refine_kernel): " + driver_error(c->drv, r));
-    c->launches++;
-    return 0;
+int pe_render_adaptive_strips(pe_ctx* c, const pe_target* t, int threshold, int rgba8, void* out_device,
+                              void* refined_count_device, void* stream) {
+    if (!c) return 1;
+    if (!out_device) return c->fail("pe_render_adaptive_strips: out_device is null");
+    if (!check_target(c, t) || !bind_device(c)) return 1;
+    if (t->n_strips == 0) return 0;   // nothing of this frame belongs to the caller
+    return render_adaptive_impl(c, t, threshold, rgba8 != 0, out_device, refined_count_device, stream_of(c, stream), 0);
 }
 
 int pe_render_host(pe_ctx* c, const pe_target* t, float* out_host) {
@@ -785,7 +838,31 @@ static bool ensure_pipeline(pe_ctx* c, size_t bytes) {
     return true;
 }
 
-static int submit_host(pe_ctx* c, const pe_target* t, uint8_t* out_host, uint64_t* ticket, bool strips_into_frame) {
+// Copy a target's compact strips (`bpp` bytes per pixel) to their rows of a whole row-major frame: strip k of the target =
+// global strip strip_first + k * strip_step, contiguous rows of the frame, strip_step strips apart from strip k + 1 -> ONE
+// pitched copy for the whole strips (+ one for a ragged last strip).
+static bool copy_strips(pe_ctx* c, const pe_target* t, void* frame, const void* strips, size_t bpp, cudaMemcpyKind kind,
+                        cudaStream_t s, const char* what) {
+    const size_t row_bytes = size_t(t->width) * bpp, strip_bytes = row_bytes * size_t(t->strip_rows);
+    int full = 0, ragged_rows = 0;
+    for (int k = 0; k < t->n_strips; k++) {
+        const int row0 = (t->strip_first + k * t->strip_step) * t->strip_rows;
+        if (row0 >= t->height) break;
+        if (row0 + t->strip_rows <= t->height) full++;
+        else ragged_rows = t->height - row0;
+    }
+    uint8_t* dst0 = static_cast<uint8_t*>(frame) + size_t(t->strip_first) * strip_bytes;
+    if (full && !cuda_ok(c, cudaMemcpy2DAsync(dst0, strip_bytes * size_t(t->strip_step), strips, strip_bytes, strip_bytes, size_t(full),
+                                              kind, s), what)) return false;
+    if (ragged_rows && !cuda_ok(c, cudaMemcpyAsync(dst0 + size_t(full) * strip_bytes * size_t(t->strip_step),
+                                                   static_cast<const uint8_t*>(strips) + size_t(full) * strip_bytes,
+                                                   size_t(ragged_rows) * row_bytes, kind, s), what)) return false;
+    return true;
+}
+
+// `adaptive`: the device slot holds adaptive anti-aliasing's strips (pe_render_adaptive_strips with `threshold`)
+static int submit_host(pe_ctx* c, const pe_target* t, uint8_t* out_host, uint64_t* ticket, bool strips_into_frame,
+                       bool adaptive = false, int threshold = 0) {
     if (!c) return 1;
     if (!out_host || !ticket) return c->fail("pe_submit_host_rgba8: null argument");
     if (!check_target(c, t) || !bind_device(c)) return 1;
@@ -797,28 +874,14 @@ static int submit_host(pe_ctx* c, const pe_target* t, uint8_t* out_host, uint64_
     auto& sl = c->slots[tk % PE_PIPELINE_DEPTH];
     // the slot's previous frame (ticket tk - depth) must have left the device before it is overwritten
     if (sl.ticket && !cuda_ok(c, cudaStreamWaitEvent(c->stream, sl.copied, 0), "pipeline wait")) return 1;
-    if (n && render_impl(c, &local, sl.buf.dev, nullptr, nullptr, true)) return 1;
+    if (n && (adaptive ? render_adaptive_impl(c, &local, threshold, true, sl.buf.dev, nullptr, c->stream, 0)
+                                         : render_impl(c, &local, sl.buf.dev, nullptr, nullptr, true))) return 1;
     if (!cuda_ok(c, cudaEventRecord(sl.rendered, c->stream), "event record") ||
         !cuda_ok(c, cudaStreamWaitEvent(c->copy_stream, sl.rendered, 0), "pipeline wait")) return 1;
     if (!strips_into_frame) {
         if (n && !cuda_ok(c, cudaMemcpyAsync(out_host, sl.buf.dev, n * 4, cudaMemcpyDeviceToHost, c->copy_stream), "D2H copy")) return 1;
-    } else {
-        // strip k of this rank = global strip strip_first + k * strip_step: contiguous rows of the row-major frame,
-        // world strips apart from strip k + 1 -> ONE pitched copy for the whole strips (+ one for a ragged last strip)
-        const size_t row_bytes = size_t(t->width) * 4, strip_bytes = row_bytes * size_t(t->strip_rows);
-        int full = 0, ragged_rows = 0;
-        for (int k = 0; k < t->n_strips; k++) {
-            const int row0 = (t->strip_first + k * t->strip_step) * t->strip_rows;
-            if (row0 >= t->height) break;
-            if (row0 + t->strip_rows <= t->height) full++;
-            else ragged_rows = t->height - row0;
-        }
-        uint8_t* dst0 = out_host + size_t(t->strip_first) * strip_bytes;
-        if (full && !cuda_ok(c, cudaMemcpy2DAsync(dst0, strip_bytes * size_t(t->strip_step), sl.buf.dev, strip_bytes, strip_bytes, size_t(full),
-                                                  cudaMemcpyDeviceToHost, c->copy_stream), "D2H strip copy")) return 1;
-        if (ragged_rows && !cuda_ok(c, cudaMemcpyAsync(dst0 + size_t(full) * strip_bytes * size_t(t->strip_step),
-                                                       (const uint8_t*)sl.buf.dev + size_t(full) * strip_bytes, size_t(ragged_rows) * row_bytes,
-                                                       cudaMemcpyDeviceToHost, c->copy_stream), "D2H strip copy")) return 1;
+    } else if (!copy_strips(c, t, out_host, sl.buf.dev, 4, cudaMemcpyDeviceToHost, c->copy_stream, "D2H strip copy")) {
+        return 1;
     }
     if (!cuda_ok(c, cudaEventRecord(sl.copied, c->copy_stream), "event record")) return 1;
     sl.ticket = tk;
@@ -833,6 +896,29 @@ int pe_submit_host_rgba8(pe_ctx* c, const pe_target* t, uint8_t* out_host, uint6
 int pe_submit_host_strips_rgba8(pe_ctx* c, const pe_target* t, uint8_t* host_frame, uint64_t* ticket) {
     return submit_host(c, t, host_frame, ticket, true);
 }
+
+}  // extern "C"
+
+int pe_internal_submit_host_strips_adaptive(pe_ctx* c, const pe_target* t, uint8_t* host_frame, uint64_t* ticket, int threshold) {
+    return submit_host(c, t, host_frame, ticket, true, true, threshold);
+}
+
+int pe_internal_render_adaptive(pe_ctx* c, const pe_target* t, int threshold, int rgba8, void* out_device, void* stream, int instance) {
+    if (!c) return 1;
+    if (!out_device) return c->fail("adaptive anti-aliasing: out_device is null");
+    if (!check_target(c, t) || !bind_device(c)) return 1;
+    if (t->n_strips == 0) return 0;
+    return render_adaptive_impl(c, t, threshold, rgba8 != 0, out_device, nullptr, stream_of(c, stream), instance);
+}
+
+int pe_internal_copy_strips(pe_ctx* c, const pe_target* t, void* frame_device, const void* strips_device, size_t bytes_per_pixel,
+                            void* stream) {
+    if (!c || !t || !frame_device || !strips_device) return 1;
+    if (!bind_device(c)) return 1;
+    return copy_strips(c, t, frame_device, strips_device, bytes_per_pixel, cudaMemcpyDefault, stream_of(c, stream), "strip copy") ? 0 : 1;
+}
+
+extern "C" {
 
 int pe_host_register(pe_ctx* c, void* p, size_t bytes) {
     if (!c || !p || bytes == 0) return 1;

@@ -14,10 +14,12 @@
 
 namespace pe_host {
 
-// One loaded copy of a variant's cubin: its render kernel and its own uniform block on the device.
+// One loaded copy of a variant's cubin: its render kernel, its refine kernel (programs generated with_refine) and its own
+// uniform block on the device.
 struct ProgramInstance {
     CUmodule_t module = nullptr;
     CUfunction_t kernel = nullptr;
+    CUfunction_t refine = nullptr;
     CUdeviceptr_t const_ptr = 0;
 };
 
@@ -28,8 +30,7 @@ struct Variant {
     // be in flight at once (on two streams) -- frame f + 1's uniforms are uploaded while frame f's kernel still reads its own.
     ProgramInstance inst[2];
     CUfunction_t probe = nullptr;    // pe_probe_kernel of inst[0] (programs generated with_probe)
-    CUfunction_t refine = nullptr;   // pe_refine_kernel of inst[0] (programs generated with_refine)
-    int refine_blocks_per_sm = 1;
+    int refine_blocks_per_sm = 1;    // pe_refine_kernel (programs generated with_refine)
     int blocks_per_sm = 1;
 };
 
@@ -95,9 +96,13 @@ struct pe_ctx {
     struct Slot { pe_host::DeviceBuffer buf; cudaEvent_t rendered = nullptr, copied = nullptr; uint64_t ticket = 0; };
     Slot slots[PE_PIPELINE_DEPTH];
     pe_host::DeviceBuffer caller_slots[128];     // pe_scratch_buffer: the caller's alone
-    // the library's own intermediates: pe_render_adaptive's pixel list and its count + refill cursor, pe_frames_differ's
-    // difference word, pe_autotune's timing frame and its guard's copy of the first candidate's frame
-    pe_host::DeviceBuffer refine_list, refine_count, diff_word, tune_frame, tune_guard;
+    // the library's own intermediates: pe_frames_differ's difference word, pe_autotune's timing frame and its guard's copy
+    // of the first candidate's frame
+    pe_host::DeviceBuffer diff_word, tune_frame, tune_guard;
+    // adaptive anti-aliasing, one set per program instance (two frames in flight use both): the pixel list, its count +
+    // refill cursor, and the one-sample RGBA8 halo rows above and below the target's strips
+    struct AdaptiveBuffers { pe_host::DeviceBuffer refine_list, refine_count, halo_above, halo_below; };
+    AdaptiveBuffers adaptive[2];
     // adaptive de-specialisation: a slot whose value differed between renders more than kMaxRespecialisations times is read
     // from the constant block from then on (bounds NVRTC compiles when an animation drives an int or a matrix structure)
     std::vector<int> last_ints, int_changes;

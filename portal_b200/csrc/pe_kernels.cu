@@ -201,55 +201,113 @@ __global__ void __launch_bounds__(256) pe_k_count_diff(const uint4* __restrict__
     if ((threadIdx.x & 31) == 0 && mine) atomicAdd(count, mine);
 }
 
-// Adaptive anti-aliasing edge mask (pe_render_adaptive).  Q = the unorm8 r, g, b of the one-sample frame (RGBA8 bytes, or
-// the float frame quantised as pe_k_quantize_rgba8 does); a pixel is refined when, for some channel, max - min of Q over its
-// 3x3 neighbourhood clipped to the frame exceeds `threshold`.  One warp per 8x4 tile: the tile's refined pixels are balloted,
-// lane 0 reserves their list slots with one atomicAdd, and they are written in tile order (lane order), so the refine pass's
-// warps start on neighbouring pixels.  The order of tiles in the list depends on scheduling; the set does not.
-template <bool RGBA8>
-__global__ void __launch_bounds__(256) pe_k_refine_list(const void* __restrict__ frame, int width, int height, int tiles_x,
-                                                        unsigned n_tiles, int threshold, unsigned* __restrict__ list,
-                                                        unsigned* __restrict__ count) {
-    const unsigned tile = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    if (tile >= n_tiles) return;                                  // warp-uniform
-    const unsigned lane = threadIdx.x & 31u;
-    const int x = int(tile % unsigned(tiles_x)) * 8 + int(lane & 7u), y = int(tile / unsigned(tiles_x)) * 4 + int(lane >> 3);
-    bool refine = false;
-    if (x < width && y < height) {
-        unsigned lo[3] = {255u, 255u, 255u}, hi[3] = {0u, 0u, 0u};
-        for (int yy = max(y - 1, 0); yy <= min(y + 1, height - 1); yy++)
-            for (int xx = max(x - 1, 0); xx <= min(x + 1, width - 1); xx++) {
-                const size_t i = size_t(yy) * size_t(width) + size_t(xx);
-                const unsigned q = RGBA8 ? reinterpret_cast<const unsigned*>(frame)[i] : pack8(reinterpret_cast<const float4*>(frame)[i]);
+// Adaptive anti-aliasing edge mask (pe_render_adaptive, pe_render_adaptive_strips).  Q = the unorm8 r, g, b of the
+// one-sample frame (RGBA8 bytes, or the float frame quantised as pe_k_quantize_rgba8 does); a pixel is refined when, for
+// some channel, max - min of Q over its 3x3 neighbourhood clipped to the frame exceeds `threshold`.  The frame is the
+// target's output buffer (compact local rows or the full frame); a neighbour row outside the pixel's strip is read from the
+// buffer when it belongs to the target (strip_step 1: the adjacent strip), else from the halo rows (RGBA8, one row per
+// strip: above[i - above_first], below[i]; strip_step 1: one row each).  One warp per 8x4 tile of local rows: the tile's
+// refined pixels are balloted, lane 0 reserves their list slots with one atomicAdd, and they are written in tile order (lane
+// order), so the refine pass's warps start on neighbouring pixels.  List entries are (local_row << 16) | x.  The order of
+// tiles in the list depends on scheduling; the set does not.
+struct RefineListArgs {
+    const void* frame;
+    const unsigned* above;     // halo row above strip i (i >= above_first), RGBA8
+    const unsigned* below;     // halo row below strip i, RGBA8
+    int width, height, strip_rows, strip_first, strip_step, n_strips, full_frame, above_first;
+    int local_rows;            // local rows that can hold frame rows
+    int tiles_x;
+    unsigned n_tiles;
+    int threshold;
+};
+
+__device__ __forceinline__ void widen(unsigned q, unsigned (&lo)[3], unsigned (&hi)[3]) {
 #pragma unroll
-                for (int ch = 0; ch < 3; ch++) {
-                    const unsigned v = (q >> (8 * ch)) & 0xffu;
-                    lo[ch] = min(lo[ch], v);
-                    hi[ch] = max(hi[ch], v);
+    for (int ch = 0; ch < 3; ch++) {
+        const unsigned v = (q >> (8 * ch)) & 0xffu;
+        lo[ch] = min(lo[ch], v);
+        hi[ch] = max(hi[ch], v);
+    }
+}
+
+// STRIPS = false: a whole-frame target (one strip from row 0 down past the last row): the local row is the row, every
+// neighbour is in the buffer, and the loop is the plain 3x3 window.  The strip logic would cost this pass 40 % (0.13 ->
+// 0.18 ms per 4K float frame, H100).
+template <bool RGBA8, bool STRIPS>
+__global__ void __launch_bounds__(256) pe_k_refine_list(const RefineListArgs A, unsigned* __restrict__ list, unsigned* __restrict__ count) {
+    const unsigned tile = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (tile >= A.n_tiles) return;                                // warp-uniform
+    const unsigned lane = threadIdx.x & 31u;
+    const int x = int(tile % unsigned(A.tiles_x)) * 8 + int(lane & 7u), lrow = int(tile / unsigned(A.tiles_x)) * 4 + int(lane >> 3);
+    bool refine = false;
+    // strip i of the target, row r inside it, global row y
+    const int i = STRIPS ? lrow / A.strip_rows : 0, r = lrow - i * A.strip_rows;
+    const int y = STRIPS ? (A.strip_first + i * A.strip_step) * A.strip_rows + r : lrow;
+    if (x < A.width && lrow < A.local_rows && y < A.height) {
+        unsigned lo[3] = {255u, 255u, 255u}, hi[3] = {0u, 0u, 0u};
+        if (!STRIPS) {
+            for (int yy = max(y - 1, 0); yy <= min(y + 1, A.height - 1); yy++)
+                for (int xx = max(x - 1, 0); xx <= min(x + 1, A.width - 1); xx++) {
+                    const size_t k = size_t(yy) * size_t(A.width) + size_t(xx);
+                    widen(RGBA8 ? reinterpret_cast<const unsigned*>(A.frame)[k] : pack8(reinterpret_cast<const float4*>(A.frame)[k]), lo, hi);
                 }
+        } else {
+            for (int dy = -1; dy <= 1; dy++) {
+                const int yy = y + dy, rr = r + dy;
+                if (yy < 0 || yy >= A.height) continue;              // the frame's own edge
+                const unsigned* row8 = nullptr;                       // an RGBA8 row: a halo, or the buffer of an RGBA8 frame
+                const float4* rowf = nullptr;
+                const bool in_buffer = (rr >= 0 && rr < A.strip_rows) || (A.strip_step == 1 && (rr < 0 ? i > 0 : i < A.n_strips - 1));
+                if (in_buffer) {
+                    const size_t row = size_t(A.full_frame ? yy : lrow + dy) * size_t(A.width);
+                    if (RGBA8) row8 = reinterpret_cast<const unsigned*>(A.frame) + row;
+                    else rowf = reinterpret_cast<const float4*>(A.frame) + row;
+                } else if (rr < 0) {
+                    row8 = A.above + size_t(A.strip_step == 1 ? 0 : i - A.above_first) * size_t(A.width);
+                } else {
+                    row8 = A.below + size_t(A.strip_step == 1 ? 0 : i) * size_t(A.width);
+                }
+                for (int xx = max(x - 1, 0); xx <= min(x + 1, A.width - 1); xx++) widen(row8 ? row8[xx] : pack8(rowf[xx]), lo, hi);
             }
-        const int range = int(max(hi[0] - lo[0], max(hi[1] - lo[1], hi[2] - lo[2])));
-        refine = range > threshold;
+        }
+    const int range = int(max(hi[0] - lo[0], max(hi[1] - lo[1], hi[2] - lo[2])));
+        refine = range > A.threshold;
     }
     const unsigned m = __ballot_sync(0xffffffffu, refine);
     if (m == 0u) return;
     unsigned base = 0;
     if (lane == 0) base = atomicAdd(count, unsigned(__popc(m)));
     base = __shfl_sync(0xffffffffu, base, 0);
-    if (refine) list[base + unsigned(__popc(m & ((1u << lane) - 1u)))] = (unsigned(y) << 16) | unsigned(x);
+    if (refine) list[base + unsigned(__popc(m & ((1u << lane) - 1u)))] = (unsigned(lrow) << 16) | unsigned(x);
 }
 
 }  // namespace
 
 namespace pe_host {
 
-int launch_refine_list(const void* frame, bool rgba8, int width, int height, int threshold, unsigned* list, unsigned* count,
-                       cudaStream_t s) {
-    const int tiles_x = (width + 7) / 8;
-    const unsigned n_tiles = unsigned(tiles_x) * unsigned((height + 3) / 4);
-    const unsigned blocks = (n_tiles + 7u) / 8u;                  // 8 warps = 8 tiles per block
-    if (rgba8) pe_k_refine_list<true><<<blocks, 256, 0, s>>>(frame, width, height, tiles_x, n_tiles, threshold, list, count);
-    else pe_k_refine_list<false><<<blocks, 256, 0, s>>>(frame, width, height, tiles_x, n_tiles, threshold, list, count);
+int launch_refine_list(const void* frame, bool rgba8, const RefineTarget& t, const unsigned* above, int above_first,
+                       const unsigned* below, int threshold, unsigned* list, unsigned* count, cudaStream_t s) {
+    RefineListArgs A;
+    A.frame = frame;
+    A.above = above;
+    A.below = below;
+    A.width = t.width;
+    A.height = t.height;
+    A.strip_rows = t.strip_rows;
+    A.strip_first = t.strip_first;
+    A.strip_step = t.strip_step;
+    A.n_strips = t.n_strips;
+    A.full_frame = t.full_frame_layout;
+    A.above_first = above_first;
+    A.local_rows = t.local_rows;
+    A.tiles_x = (t.width + 7) / 8;
+    A.n_tiles = unsigned(A.tiles_x) * unsigned((t.local_rows + 3) / 4);
+    A.threshold = threshold;
+    const unsigned blocks = (A.n_tiles + 7u) / 8u;                // 8 warps = 8 tiles per block
+    if (blocks == 0) return (int)cudaSuccess;
+    const bool strips = !(t.n_strips == 1 && t.strip_first == 0 && t.strip_rows >= t.height);   // else the whole frame
+    if (rgba8) (strips ? pe_k_refine_list<true, true> : pe_k_refine_list<true, false>)<<<blocks, 256, 0, s>>>(A, list, count);
+    else (strips ? pe_k_refine_list<false, true> : pe_k_refine_list<false, false>)<<<blocks, 256, 0, s>>>(A, list, count);
     return (int)cudaGetLastError();
 }
 

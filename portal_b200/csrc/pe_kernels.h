@@ -12,9 +12,16 @@ int launch_signal(void* const* ptrs, int n, unsigned int value, cudaStream_t s);
 int launch_average_rgba8(const void* const* frames, int n_frames, void* out, size_t n_pixels, int sms, cudaStream_t s);
 // *count += number of 16-byte words in which a and b differ (bitwise); both 16-byte aligned
 int launch_count_diff(const void* a, const void* b, size_t n_words16, unsigned* count, int sms, cudaStream_t s);
-// Adaptive anti-aliasing: append the packed indices ((y << 16) | x) of the pixels of a whole width x height frame (RGBA8 or
-// float RGBA) whose 3x3 unorm8 range exceeds `threshold` to `list`, counting them in count[0] (zeroed by the caller)
-int launch_refine_list(const void* frame, bool rgba8, int width, int height, int threshold, unsigned* list, unsigned* count,
-                       cudaStream_t s);
+// The rows of a render target (pe_target) the edge mask walks: local rows [0, local_rows) are those that can hold frame rows.
+struct RefineTarget {
+    int width, height, strip_rows, strip_first, strip_step, n_strips, full_frame_layout, local_rows;
+};
+// Adaptive anti-aliasing: append the packed entries ((local_row << 16) | x) of the target's pixels whose 3x3 unorm8 range in
+// the whole one-sample frame exceeds `threshold` to `list`, counting them in count[0] (zeroed by the caller).  `frame` is the
+// target's output (RGBA8 or float RGBA); the frame rows next to its strips that are not the target's own are the RGBA8 halo
+// rows `above` (one per strip from strip `above_first` on; strip_step 1: one row above the first strip) and `below` (one
+// per strip; strip_step 1: one row below the last strip).  A whole-frame target needs neither.
+int launch_refine_list(const void* frame, bool rgba8, const RefineTarget& t, const unsigned* above, int above_first,
+                       const unsigned* below, int threshold, unsigned* list, unsigned* count, cudaStream_t s);
 
 }  // namespace pe_host

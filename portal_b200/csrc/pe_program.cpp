@@ -285,7 +285,7 @@ bool select_variant(pe_ctx* c, bool need_probe, bool need_refine, bool counted) 
     if (c->has_gpu && !v->inst[0].module) {
         if (!load_instance(c, *v, 0)) return false;
         if (with_probe && !get_kernel(c, v->inst[0].module, "pe_probe_kernel", &v->probe)) return false;
-        if (with_refine && !get_kernel(c, v->inst[0].module, "pe_refine_kernel", &v->refine, &v->refine_blocks_per_sm)) return false;
+        if (with_refine && !get_kernel(c, v->inst[0].module, "pe_refine_kernel", &v->inst[0].refine, &v->refine_blocks_per_sm)) return false;
     }
     c->current = v;
     return true;
@@ -304,6 +304,7 @@ bool load_instance(pe_ctx* c, Variant& v, int k) {
     }
     if (r != 0) { c->err = "cuModuleLoadData: " + driver_error(d, r); return false; }
     if (!get_kernel(c, in.module, "pe_render_kernel", &in.kernel, &v.blocks_per_sm)) return false;
+    if (k > 0 && v.inst[0].refine && !get_kernel(c, in.module, "pe_refine_kernel", &in.refine)) return false;
     const char* block_symbol = c->opts.uniforms_in_smem ? "PE_C_UPLOAD" : "PE_C";
     size_t const_size = 0;
     r = d->cuModuleGetGlobal(&in.const_ptr, &const_size, in.module, block_symbol);

@@ -150,6 +150,10 @@ struct pe_sharder {
     void* lane_frame[2] = {nullptr, nullptr};
     bool lane_busy[2] = {false, false};
     int ring = 2;
+    // adaptive anti-aliasing (pe_sharder_set_adaptive_aa); P2P renders it into `compact`, a buffer of its own, first
+    bool adaptive = false;
+    int threshold = 0;
+    void* compact = nullptr;
     // host mode
     uint64_t host_frame_no = 0;
     std::map<uint64_t, uint64_t> tickets;
@@ -351,16 +355,29 @@ int pe_sharder_target(pe_sharder* s, pe_target* out) {
     return 0;
 }
 
+int pe_sharder_set_adaptive_aa(pe_sharder* s, int on, int threshold) {
+    if (!s) return 1;
+    if (on && s->mode == PE_SHARD_P2P && !s->compact) {
+        if (pe_device_malloc(s->ctx, s->local_bytes ? s->local_bytes : 16, &s->compact)) return s->fail_ctx("adaptive strips buffer");
+        s->owned.push_back(s->compact);
+    }
+    s->adaptive = on != 0;
+    s->threshold = threshold;
+    return 0;
+}
+
 int pe_sharder_render(pe_sharder* s, void* stream, void** frame_out) {
     if (!s) return 1;
     if (frame_out) *frame_out = nullptr;
     if (s->mode == PE_SHARD_HOST) return s->fail("pe_sharder_render: this sharder delivers to host memory (use pe_sharder_submit)");
     pe_ctx* c = s->ctx;
     const uint32_t f = ++s->frame_no;
+    const int rgba8 = s->format == PE_FRAME_RGBA8;
     if (s->mode == PE_SHARD_OWNER) {
         void* dst = s->local[f % uint32_t(s->ring)];
         if (s->target.n_strips > 0) {
-            const int rc = s->format == PE_FRAME_F32 ? pe_render(c, &s->target, dst, nullptr, stream) : pe_render_rgba8(c, &s->target, dst, stream);
+            const int rc = s->adaptive ? pe_render_adaptive_strips(c, &s->target, s->threshold, rgba8, dst, nullptr, stream)
+                           : s->format == PE_FRAME_F32 ? pe_render(c, &s->target, dst, nullptr, stream) : pe_render_rgba8(c, &s->target, dst, stream);
             if (rc) return s->fail_ctx("render");
         }
         s->current = dst;
@@ -371,7 +388,13 @@ int pe_sharder_render(pe_sharder* s, void* stream, void** frame_out) {
     auto word = [](void* base, int w) { return static_cast<void*>(static_cast<uint32_t*>(base) + w); };
     // a buffer is reused two frames later: not before rank 0's consumer of that frame has been enqueued
     if (s->rank != 0 && f > 2 && pe_stream_wait_geq_u32(c, word(s->sig, kConsumed), f - 2, stream)) return s->fail_ctx("wait consumed");
-    if (s->target.n_strips > 0) {
+    if (s->target.n_strips > 0 && s->adaptive) {
+        // the list and refine passes read and rewrite the strips: render them here, then move them with one pitched copy
+        pe_target local = s->target;
+        local.full_frame_layout = 0;
+        if (pe_render_adaptive_strips(c, &local, s->threshold, rgba8, s->compact, nullptr, stream)) return s->fail_ctx("render");
+        if (pe_internal_copy_strips(c, &local, dst, s->compact, rgba8 ? 4 : 16, stream)) return s->fail_ctx("strip copy");
+    } else if (s->target.n_strips > 0) {
         const int rc = s->format == PE_FRAME_F32 ? pe_render(c, &s->target, dst, nullptr, stream) : pe_render_rgba8(c, &s->target, dst, stream);
         if (rc) return s->fail_ctx("render");
     }
@@ -408,7 +431,9 @@ int pe_sharder_render_overlapped(pe_sharder* s, void* stream, void** prev_frame_
     // the lane starts after what the caller has enqueued so far (e.g. its reader of the buffer this frame overwrites)
     if (cudaEventRecord(s->submitted, user) != cudaSuccess || cudaStreamWaitEvent(s->lane[q], s->submitted, 0) != cudaSuccess)
         return s->fail("pe_sharder_render_overlapped: stream ordering failed");
-    if (s->target.n_strips > 0 && pe_internal_render(s->ctx, &s->target, dst, s->lane[q], s->format == PE_FRAME_RGBA8, q))
+    const int rgba8 = s->format == PE_FRAME_RGBA8;
+    if (s->target.n_strips > 0 && (s->adaptive ? pe_internal_render_adaptive(s->ctx, &s->target, s->threshold, rgba8, dst, s->lane[q], q)
+                                               : pe_internal_render(s->ctx, &s->target, dst, s->lane[q], rgba8, q)))
         return s->fail_ctx("render");
     if (cudaEventRecord(s->lane_done[q], s->lane[q]) != cudaSuccess) return s->fail("pe_sharder_render_overlapped: event record failed");
     s->lane_frame[q] = dst;
@@ -454,7 +479,9 @@ int pe_sharder_submit(pe_sharder* s, uint64_t* frame_no) {
     uint64_t ticket = 0;
     uint8_t* slot = s->map + kHeaderBytes + size_t(f % PE_HOST_RING_DEPTH) * s->frame_bytes;
     pe_target t = s->target;
-    if (pe_submit_host_strips_rgba8(s->ctx, &t, slot, &ticket)) return s->fail_ctx("submit");
+    if (s->adaptive ? pe_internal_submit_host_strips_adaptive(s->ctx, &t, slot, &ticket, s->threshold)
+                    : pe_submit_host_strips_rgba8(s->ctx, &t, slot, &ticket))
+        return s->fail_ctx("submit");
     s->tickets[f] = ticket;
     if (frame_no) *frame_no = f;
     return 0;

@@ -220,13 +220,15 @@ class NativeSharder:
       "p2p"    render kernels store straight into rank 0's frame over NVLink (render() -> assembled frame on rank 0);
       "host"   RGBA8 strips over every GPU's own PCIe link into one shared pinned host frame (submit / complete /
                wait_frame / release_frame).
+    `adaptive_aa` = T turns on adaptive anti-aliasing with threshold T (pe_sharder_set_adaptive_aa): the assembled frame is
+    the single-GPU pe_render_adaptive frame; every rank must pass the same T.
     This class only moves arguments across the boundary; uniforms are the renderer's (set_uniforms is called for you)."""
 
     MODES = {"owner": 0, "p2p": 1, "host": 2}
     FORMATS = {"f32": 0, "rgba8": 1}
 
     def __init__(self, renderer, width: int, height: int, rank: int, world: int, mode: str, fmt: str = "f32",
-                 strip_rows: int = STRIP_ROWS, name: str | None = None):
+                 strip_rows: int = STRIP_ROWS, name: str | None = None, adaptive_aa: int | None = None):
         self.r, self.w, self.h, self.rank, self.world, self.mode, self.fmt = renderer, width, height, rank, world, mode, fmt
         self._lib = renderer._lib
         self._s = C.c_void_p()
@@ -243,6 +245,8 @@ class NativeSharder:
         self.target = PeTarget()
         self._check(self._lib.pe_sharder_target(self._s, C.byref(self.target)))
         self.frame_ptr = None
+        if adaptive_aa is not None:
+            self._check(self._lib.pe_sharder_set_adaptive_aa(self._s, 1, int(adaptive_aa)))
 
     def _check(self, rc):
         if rc:

@@ -341,6 +341,16 @@ class SceneRenderer:
         self._check(self._lib.pe_render_adaptive(self._ctx, C.byref(target), int(threshold), int(rgba8), out_ptr, refined_ptr or None,
                                                  stream or None))
 
+    def draw_texture_adaptive_strips(self, target: PeTarget, out_ptr: int, threshold: int, rgba8: bool = False,
+                                     refined_ptr: int = 0, stream: int = 0):
+        """Adaptive anti-aliasing of any target, strips of a sharded frame included (async, pe_render_adaptive_strips): every
+        pixel of the target is the whole-frame adaptive frame's pixel, bit for bit -- the rows next to the strips that other
+        ranks own are rendered here at one sample.  `refined_ptr` (optional, device uint32) receives this target's number
+        of refined pixels."""
+        self.set_uniforms()
+        self._check(self._lib.pe_render_adaptive_strips(self._ctx, C.byref(target), int(threshold), int(rgba8), out_ptr,
+                                                        refined_ptr or None, stream or None))
+
     def render_host_adaptive(self, width: int, height: int, threshold: int, rgba8: bool = False) -> tuple[np.ndarray, int]:
         """One adaptive frame on the host (float RGBA, or RGBA8) and the number of refined pixels."""
         n = width * height

@@ -7,7 +7,11 @@ segment rendezvous, IPC mappings, flag words, host ring) is exercised on a one-G
 used by THIS CHECKER only, to collect the ranks' strips and verdicts; the sharder itself needs no collective library.
 
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29533 \
-        tools/check_sharder.py portal_in_portal 1920 1080 40 [--same-gpu]
+        tools/check_sharder.py portal_in_portal 1920 1080 40 [--same-gpu] [--adaptive-aa T]
+
+`--adaptive-aa T` checks the same modes with adaptive anti-aliasing on (pe_sharder_set_adaptive_aa, threshold T, every
+frame at aa_count 4) instead: each frame must equal the single-GPU pe_render_adaptive whole frame, and the lines read
+"sharder adaptive <mode> <fmt>: ... bit-identical to single GPU: <bool>".
 """
 import os
 import sys
@@ -24,8 +28,14 @@ from portal_b200.renderer import SceneRenderer, load_scene_ir, load_textures  # 
 
 
 def main():
-    args = [a for a in sys.argv[1:] if not a.startswith("--")]
-    same_gpu = "--same-gpu" in sys.argv
+    argv = sys.argv[1:]
+    adaptive = None
+    if "--adaptive-aa" in argv:
+        k = argv.index("--adaptive-aa")
+        adaptive = int(argv[k + 1])
+        del argv[k:k + 2]
+    args = [a for a in argv if not a.startswith("--")]
+    same_gpu = "--same-gpu" in argv
     scene = args[0] if args else "portal_in_portal"
     w, h, depth = (int(x) for x in (args[1:4] if len(args) > 3 else (1920, 1080, 40)))
     world, rank, local = int(os.environ["WORLD_SIZE"]), int(os.environ["RANK"]), int(os.environ["LOCAL_RANK"])
@@ -38,6 +48,15 @@ def main():
     stream = torch.cuda.Stream()
     sp = stream.cuda_stream
     cam = dict(r.cam)
+    tag = "adaptive " if adaptive is not None else ""
+    if adaptive is not None:
+        r.aa_count = 4
+
+    def reference(fmt):
+        """The single-GPU frame of the current uniforms: pe_render / pe_render_rgba8, or the pe_render_adaptive whole frame."""
+        if adaptive is not None:
+            return r.render_host_adaptive(w, h, adaptive, fmt == "rgba8")[0]
+        return r.render_host(w, h) if fmt == "f32" else r.render_host_rgba8(w, h)
 
     def set_frame(f):
         r.set_cam(cam["look_at"], cam["alpha"] + 0.05 * f, cam["beta"], cam["r"])
@@ -51,7 +70,7 @@ def main():
 
     # ---- owner: strips stay in each rank's HBM; the checker pulls them and assembles
     for fmt, dtype in (("f32", np.float32), ("rgba8", np.uint8)):
-        sh = NativeSharder(r, w, h, rank, world, "owner", fmt)
+        sh = NativeSharder(r, w, h, rank, world, "owner", fmt, adaptive_aa=adaptive)
         for f in range(3):
             set_frame(f)
             ptr = sh.render(sp)
@@ -66,15 +85,15 @@ def main():
                     if y >= 0:
                         frame[y] = st[k]
             set_frame(2)
-            ref = r.render_host(w, h) if fmt == "f32" else r.render_host_rgba8(w, h)
+            ref = reference(fmt)
             same = np.array_equal(frame, ref) if fmt == "rgba8" else np.array_equal(frame.view(np.uint32), ref.view(np.uint32))
-            print(f"sharder owner {fmt}: world {world} {scene} {w}x{h} -> bit-identical to single GPU: {same}", flush=True)
+            print(f"sharder {tag}owner {fmt}: world {world} {scene} {w}x{h} -> bit-identical to single GPU: {same}", flush=True)
             ok = ok and same
         dist.barrier()
         sh.close()
 
     # ---- owner, two frames in flight: every call returns the PREVIOUS frame; 6 frames with a moving camera
-    sh = NativeSharder(r, w, h, rank, world, "owner", "f32")
+    sh = NativeSharder(r, w, h, rank, world, "owner", "f32", adaptive_aa=adaptive)
     rows = local_rows(h, rank, world)
     same = True
 
@@ -91,7 +110,7 @@ def main():
                     frame[y] = st[k]
         torch.cuda.synchronize()          # the frame still in flight reads a uniform block the reference render below would overwrite
         set_frame(f)
-        return bool(np.array_equal(frame.view(np.uint32), r.render_host(w, h).view(np.uint32)))
+        return bool(np.array_equal(frame.view(np.uint32), reference("f32").view(np.uint32)))
 
     for f in range(6):
         set_frame(f)
@@ -102,14 +121,14 @@ def main():
             same = check_owner_frame(prev, f - 1) and same
     same = check_owner_frame(sh.flush(sp), 5) and same
     if rank == 0:
-        print(f"sharder owner overlapped f32: world {world} {scene} {w}x{h} x 6 frames -> bit-identical to single GPU: {same}", flush=True)
+        print(f"sharder {tag}owner overlapped f32: world {world} {scene} {w}x{h} x 6 frames -> bit-identical to single GPU: {same}", flush=True)
         ok = ok and same
     dist.barrier()
     sh.close()
 
     # ---- p2p: kernels store into rank 0's frame; 5 frames through 2 buffers exercise the recycling flags
     for fmt, dtype in (("f32", np.float32), ("rgba8", np.uint8)):
-        sh = NativeSharder(r, w, h, rank, world, "p2p", fmt)
+        sh = NativeSharder(r, w, h, rank, world, "p2p", fmt, adaptive_aa=adaptive)
         same = True
         for f in range(5):
             set_frame(f)
@@ -117,17 +136,17 @@ def main():
             if rank == 0:
                 got = d2h(ptr, (h, w, 4), dtype)          # stream-ordered behind every rank's strips
                 sh.release(sp)
-                ref = r.render_host(w, h) if fmt == "f32" else r.render_host_rgba8(w, h)
+                ref = reference(fmt)
                 same = same and (np.array_equal(got, ref) if fmt == "rgba8" else np.array_equal(got.view(np.uint32), ref.view(np.uint32)))
         stream.synchronize()
         dist.barrier()
         if rank == 0:
-            print(f"sharder p2p {fmt}: world {world} {scene} {w}x{h} x 5 frames -> bit-identical to single GPU: {same}", flush=True)
+            print(f"sharder {tag}p2p {fmt}: world {world} {scene} {w}x{h} x 5 frames -> bit-identical to single GPU: {same}", flush=True)
             ok = ok and same
         sh.close()
 
     # ---- host: RGBA8 strips over every rank's PCIe link into one shared pinned frame; 15 frames through a ring of 6 (4 device slots)
-    sh = NativeSharder(r, w, h, rank, world, "host", "rgba8")
+    sh = NativeSharder(r, w, h, rank, world, "host", "rgba8", adaptive_aa=adaptive)
     frames, prev, same = 15, None, True
 
     def finish(f):
@@ -136,7 +155,7 @@ def main():
             got = sh.wait_frame(f).copy()
             sh.release_frame(f)
             set_frame(f)
-            return np.array_equal(got, r.render_host_rgba8(w, h))
+            return np.array_equal(got, reference("rgba8"))
         return True
 
     for f in range(frames):
@@ -149,7 +168,8 @@ def main():
     dist.barrier()
     sh.close()
     if rank == 0:
-        print(f"sharder host rgba8: world {world} {scene} {w}x{h} x {frames} frames -> identical to single GPU: {same}", flush=True)
+        same_as = "bit-identical" if adaptive is not None else "identical"
+        print(f"sharder {tag}host rgba8: world {world} {scene} {w}x{h} x {frames} frames -> {same_as} to single GPU: {same}", flush=True)
         ok = ok and same
     verdict = [ok]
     dist.broadcast_object_list(verdict, src=0)
