@@ -312,6 +312,25 @@ PE_API int pe_quantize_rgba8(pe_ctx* ctx, const void* rgba_f32_device, void* rgb
  * reference has no counterpart: its frames are compared by eye, SURVEY.md section 4). */
 PE_API int pe_frames_differ(pe_ctx* ctx, const void* a_device, const void* b_device, size_t bytes, void* stream, uint32_t* words_out);
 
+/* ---- PNG files encoded on the device (no counterpart in the reference, whose export_png encodes on the CPU) ---------------
+ * The file is a pure function of the pixels, restated sequentially in tests/host_harness/png_spec.cpp and described in
+ * DESIGN.md section 5.2: 8-bit RGBA, no interlace; the row filters of ph_png_encode_rgba8 (so the decompressed image data is
+ * byte for byte that encoder's); a zlib stream of 16 KiB segments, each greedy LZ77 with fixed Huffman codes over a window
+ * primed with the 32 KiB before it (or stored, when that is shorter); IDAT chunks of 8 KiB.  A file decodes to exactly the
+ * frame's pixels.  Its bytes do not depend on the GPU, the stream or scheduling.  One context encodes on one stream at a
+ * time, as it renders: the work space is the context's own (never a pe_scratch_buffer slot). */
+/* Upper bound of the PNG file pe_encode_png_rgba8 writes for a width x height frame (0 if the size is invalid, or the file
+ * could exceed 2^31 - 1 bytes). */
+PE_API size_t pe_png_bound(int width, int height);
+/* PNG file of a row-major RGBA8 frame in device memory (4-byte aligned), encoded on the device.  Asynchronous on `stream`
+ * (NULL: the context's stream): five kernel launches.  Writes the file into png_device (capacity >= pe_png_bound, else
+ * refused before any launch) and its length into *size_device (uint64).  The frame is only read. */
+PE_API int pe_encode_png_rgba8(pe_ctx* ctx, const void* rgba8_device, int width, int height, void* png_device,
+                               size_t capacity, void* size_device, void* stream);
+/* Synchronous form on the context's stream: the file lands in host memory; *size_out = its length. */
+PE_API int pe_encode_png_host(pe_ctx* ctx, const void* rgba8_device, int width, int height, uint8_t* png_host,
+                              size_t capacity, size_t* size_out);
+
 #ifdef __cplusplus
 }
 #endif

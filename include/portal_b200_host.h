@@ -183,6 +183,15 @@ PE_API int ph_player_render_motion_blur_frame(ph_player* pl, pe_ctx* ctx, const 
  * `threshold` -- one sample everywhere, all aa_count samples where the one-sample frame has an edge.  ph_player_render_frame
  * then stages the frame in the context's scratch slot 0.  The scene-level ph_render_* functions are not affected. */
 PE_API int ph_player_set_adaptive_aa(ph_player* pl, int on, int threshold);
+/* PNG twins of ph_player_render_frame (RGBA8) and ph_player_render_motion_blur_frame: the same frame, rendered the same way
+ * (adaptive anti-aliasing, stereo and the update hook included), encoded on the device by pe_encode_png_rgba8 instead of
+ * read back.  The file (*len bytes) goes into `png` (capacity >= pe_png_bound(width, height)).  The frame is staged in the
+ * context's scratch slot 0; the motion-blur sub-frames use slots 1 .. motion_blur_frames, as in the RGBA8 twin. */
+PE_API int ph_player_render_frame_png(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, uint8_t* png, size_t capacity,
+                                      size_t* len);
+PE_API int ph_player_render_motion_blur_frame_png(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index,
+                                                  int frame_count, int motion_blur_frames, double duration_seconds,
+                                                  uint8_t* png, size_t capacity, size_t* len);
 
 /* ---- image files either side of the path ------------------------------------------------------------------------
  * Textures reach the reference as PNG files (Texture2D::from_file_with_format, src/main.rs:1066-1085) and frames leave it as

@@ -110,6 +110,9 @@ def lib() -> C.CDLL:
         "pe_average_frames_rgba8": (i32, [vp, C.POINTER(vp), i32, vp, C.c_size_t, vp]),
         "pe_quantize_rgba8": (i32, [vp, vp, vp, C.c_size_t, vp]),
         "pe_frames_differ": (i32, [vp, vp, vp, C.c_size_t, vp, C.POINTER(C.c_uint32)]),
+        "pe_png_bound": (C.c_size_t, [i32, i32]),
+        "pe_encode_png_rgba8": (i32, [vp, vp, i32, i32, vp, C.c_size_t, vp, vp]),
+        "pe_encode_png_host": (i32, [vp, vp, i32, i32, vp, C.c_size_t, C.POINTER(C.c_size_t)]),
         "pe_shard_target": (i32, [i32, i32, i32, i32, i32, i32, C.POINTER(PeTarget)]),
         "pe_sharder_create": (i32, [vp, cp, i32, i32, i32, i32, i32, i32, i32, C.POINTER(vp)]),
         "pe_sharder_destroy": (None, [vp]),
@@ -177,6 +180,9 @@ def lib() -> C.CDLL:
         "ph_player_render_frame": (i32, [vp, vp, C.POINTER(PhFrameParams), vp, i32]),
         "ph_player_render_motion_blur_frame": (i32, [vp, vp, C.POINTER(PhFrameParams), i32, i32, i32, C.c_double, vp]),
         "ph_player_set_adaptive_aa": (i32, [vp, i32, i32]),
+        "ph_player_render_frame_png": (i32, [vp, vp, C.POINTER(PhFrameParams), vp, C.c_size_t, C.POINTER(C.c_size_t)]),
+        "ph_player_render_motion_blur_frame_png": (i32, [vp, vp, C.POINTER(PhFrameParams), i32, i32, i32, C.c_double, vp, C.c_size_t,
+                                                         C.POINTER(C.c_size_t)]),
     })
     for name, (res, args) in sig.items():
         fn = getattr(L, name)
@@ -194,3 +200,19 @@ def exported_symbols():
 
 def b(s: str) -> bytes:
     return s.encode("utf-8")
+
+
+def encode_png_device(ctx, rgba8) -> bytes:
+    """PNG file of a CUDA uint8 tensor [h, w, 4] (contiguous) encoded on the device by pe_encode_png_host on context `ctx`
+    (a pe_ctx pointer: SceneRenderer._ctx / HostRenderer._ctx)."""
+    if rgba8.dim() != 3 or rgba8.shape[2] != 4 or not rgba8.is_cuda or str(rgba8.dtype) != "torch.uint8" or not rgba8.is_contiguous():
+        raise ValueError("frame must be a contiguous CUDA uint8 tensor [h, w, 4]")
+    L = lib()
+    h, w = int(rgba8.shape[0]), int(rgba8.shape[1])
+    cap = L.pe_png_bound(w, h)
+    if cap == 0:
+        raise PortalB200Error(f"pe_png_bound: no PNG for a {w} x {h} frame")
+    out, n = (C.c_uint8 * cap)(), C.c_size_t()
+    if L.pe_encode_png_host(ctx, C.c_void_p(rgba8.data_ptr()), w, h, out, cap, C.byref(n)):
+        raise PortalB200Error(L.pe_last_error(ctx).decode(errors="replace"))
+    return bytes(memoryview(out)[:n.value])

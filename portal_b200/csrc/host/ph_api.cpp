@@ -560,24 +560,44 @@ int ph_scene_camera_name(ph_scene* s, int k, const char** name) {
     return 0;
 }
 
+// The uniforms of a player frame: the scene's, the renderer's for the player's camera, and the stereo eyes.
+static int upload_player_uniforms(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p) {
+    const ph::OrbitCam& c = pl->player.cam;
+    if (ph_scene_upload_uniforms(pl->s, ctx) || upload_renderer_uniforms_cam(pl->s, ctx, p, c.get_matrix(), c.teleport_matrix, c.in_subspace)) return pfail(pl, pl->s->err);
+    return upload_stereo_uniforms(pl, ctx);
+}
+
+// The frame into device memory `dev` (RGBA8 or float RGBA): adaptively when the player is set so.
+static int render_player_device(ph_player* pl, pe_ctx* ctx, const pe_target* t, int rgba8, void* dev) {
+    if (pl->adaptive_aa) return pe_render_adaptive(ctx, t, pl->adaptive_threshold, rgba8, dev, nullptr, nullptr);
+    return rgba8 ? pe_render_rgba8(ctx, t, dev, nullptr) : pe_render(ctx, t, dev, nullptr, nullptr);
+}
+
 int ph_player_render_frame(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, void* out_host, int rgba8) {
     if (!pl || !ctx || !p || !out_host) return 1;
-    const ph::OrbitCam& c = pl->player.cam;
-    if (ph_scene_upload_uniforms(pl->s, ctx)) return pfail(pl, pl->s->err);
-    if (upload_renderer_uniforms_cam(pl->s, ctx, p, c.get_matrix(), c.teleport_matrix, c.in_subspace)) return pfail(pl, pl->s->err);
-    if (upload_stereo_uniforms(pl, ctx)) return 1;
+    if (upload_player_uniforms(pl, ctx, p)) return 1;
     pe_target t = {p->width, p->height, p->height, 0, 1, 1, 1};
     int rc;
     if (pl->adaptive_aa) {
         // the frame lands in scratch slot 0 (reused by every frame) and is read back from there
         const size_t bytes = size_t(p->width) * size_t(p->height) * (rgba8 ? 4 : 16);
         void* dev = nullptr;
-        rc = pe_scratch_buffer(ctx, 0, bytes, &dev) || pe_render_adaptive(ctx, &t, pl->adaptive_threshold, rgba8, dev, nullptr, nullptr) ||
-             pe_memcpy_d2h(ctx, out_host, dev, bytes, nullptr);
+        rc = pe_scratch_buffer(ctx, 0, bytes, &dev) || render_player_device(pl, ctx, &t, rgba8, dev) || pe_memcpy_d2h(ctx, out_host, dev, bytes, nullptr);
     } else {
         rc = rgba8 ? pe_render_host_rgba8(ctx, &t, (uint8_t*)out_host) : pe_render_host(ctx, &t, (float*)out_host);
     }
     if (rc) return pfail(pl, std::string("render failed: ") + pe_last_error(ctx));
+    return 0;
+}
+
+int ph_player_render_frame_png(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, uint8_t* png, size_t capacity, size_t* len) {
+    if (!pl || !ctx || !p || !png || !len) return 1;
+    if (upload_player_uniforms(pl, ctx, p)) return 1;
+    pe_target t = {p->width, p->height, p->height, 0, 1, 1, 1};
+    void* dev = nullptr;
+    if (pe_scratch_buffer(ctx, 0, size_t(p->width) * size_t(p->height) * 4, &dev) || render_player_device(pl, ctx, &t, 1, dev))
+        return pfail(pl, std::string("render failed: ") + pe_last_error(ctx));
+    if (pe_encode_png_host(ctx, dev, p->width, p->height, png, capacity, len)) return pfail(pl, std::string("PNG encoding failed: ") + pe_last_error(ctx));
     return 0;
 }
 
@@ -588,15 +608,15 @@ int ph_player_set_adaptive_aa(ph_player* pl, int on, int threshold) {
     return 0;
 }
 
-int ph_player_render_motion_blur_frame(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index, int frame_count,
-                                       int motion_blur_frames, double duration_seconds, uint8_t* out_host) {
-    if (!pl || !ctx || !p || !out_host) return 1;
+// The device half of ph_player_render_motion_blur_frame: the sub-frames and their gamma-2 average, left in scratch slot 0
+// (*out8); the sub-frames use slots 1 .. motion_blur_frames.
+static int motion_blur_device(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index, int frame_count, int motion_blur_frames,
+                              double duration_seconds, void** out8) {
     if (frame_count < 1 || motion_blur_frames < 1 || motion_blur_frames > 64 || frame_index < 0)
         return pfail(pl, "ph_player_render_motion_blur_frame: bad frame arguments");
     const size_t n = size_t(p->width) * size_t(p->height);
-    void* out8 = nullptr;
     std::vector<void*> sub(size_t(motion_blur_frames), nullptr);
-    int rc = pe_scratch_buffer(ctx, 0, n * 4, &out8);
+    int rc = pe_scratch_buffer(ctx, 0, n * 4, out8);
     for (size_t j = 0; j < sub.size(); j++) rc |= pe_scratch_buffer(ctx, 1 + int(j), n * 4, &sub[j]);
     if (rc) pl->err = std::string("device allocation failed: ") + pe_last_error(ctx);
     pe_target t = {p->width, p->height, p->height, 0, 1, 1, 1};
@@ -607,23 +627,36 @@ int ph_player_render_motion_blur_frame(ph_player* pl, pe_ctx* ctx, const ph_fram
         q.aa_start = j;  // main.rs:1797
         if (!pl->player.update(tt * duration_seconds)) { pl->err = pl->player.error; rc = 1; break; }   // self.update(memory, t * duration)
         if (pl->hook && pl->hook(pl->hook_user)) { pl->err = "the update hook failed"; rc = 1; break; }   // ... whose tail swaps video frames
-        const ph::OrbitCam& c = pl->player.cam;
-        if (ph_scene_upload_uniforms(pl->s, ctx) || upload_renderer_uniforms_cam(pl->s, ctx, &q, c.get_matrix(), c.teleport_matrix, c.in_subspace)) {
-            pl->err = pl->s->err;
+        if (upload_player_uniforms(pl, ctx, &q)) {
             rc = 1;
-        } else if (upload_stereo_uniforms(pl, ctx)) {
-            rc = 1;
-        } else if (pl->adaptive_aa ? pe_render_adaptive(ctx, &t, pl->adaptive_threshold, 1, sub[size_t(j)], nullptr, nullptr)
-                                   : pe_render_rgba8(ctx, &t, sub[size_t(j)], nullptr)) {
+        } else if (render_player_device(pl, ctx, &t, 1, sub[size_t(j)])) {
             pl->err = std::string("render failed: ") + pe_last_error(ctx);
             rc = 1;
         }
     }
-    if (!rc && (pe_average_frames_rgba8(ctx, sub.data(), motion_blur_frames, out8, n, nullptr) || pe_memcpy_d2h(ctx, out_host, out8, n * 4, nullptr))) {
+    if (!rc && pe_average_frames_rgba8(ctx, sub.data(), motion_blur_frames, *out8, n, nullptr)) {
         pl->err = std::string("motion-blur average failed: ") + pe_last_error(ctx);
         rc = 1;
     }
     return rc ? 1 : 0;
+}
+
+int ph_player_render_motion_blur_frame(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index, int frame_count,
+                                       int motion_blur_frames, double duration_seconds, uint8_t* out_host) {
+    if (!pl || !ctx || !p || !out_host) return 1;
+    void* out8 = nullptr;
+    if (motion_blur_device(pl, ctx, p, frame_index, frame_count, motion_blur_frames, duration_seconds, &out8)) return 1;
+    if (pe_memcpy_d2h(ctx, out_host, out8, size_t(p->width) * size_t(p->height) * 4, nullptr)) return pfail(pl, std::string("motion-blur average failed: ") + pe_last_error(ctx));
+    return 0;
+}
+
+int ph_player_render_motion_blur_frame_png(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index, int frame_count,
+                                           int motion_blur_frames, double duration_seconds, uint8_t* png, size_t capacity, size_t* len) {
+    if (!pl || !ctx || !p || !png || !len) return 1;
+    void* out8 = nullptr;
+    if (motion_blur_device(pl, ctx, p, frame_index, frame_count, motion_blur_frames, duration_seconds, &out8)) return 1;
+    if (pe_encode_png_host(ctx, out8, p->width, p->height, png, capacity, len)) return pfail(pl, std::string("PNG encoding failed: ") + pe_last_error(ctx));
+    return 0;
 }
 
 // ---- image files (ph_png.cpp)

@@ -15,8 +15,9 @@
 // --adaptive-aa T (not in the reference; off by default): every frame / sub-frame is traced with one sample, and with all
 // --aa-count samples only where that frame has an edge (a 3x3 unorm8 range above T, pe_render_adaptive).
 //
-// Output: the RGBA8 frame the reference hands to export_png (main.rs:2939-2943) as a PNG when the name ends in .png
-// (ph_png_encode_rgba8), as raw RGBA8 for .rgba, else as a binary PPM (P6, alpha dropped).  Textures: every texture of the
+// Output: the RGBA8 frame the reference hands to export_png (main.rs:2939-2943) as a PNG when the name ends in .png (encoded
+// on the device: ph_player_render_frame_png / ph_player_render_motion_blur_frame_png, pe_encode_png_rgba8), as raw RGBA8 for
+// .rgba, else as a binary PPM (P6, alpha dropped).  Textures: every texture of the
 // scene is loaded from its stored path (a PNG, relative to --assets, default the working directory) like reload_textures
 // (main.rs:1066-1085) -- a file that cannot be read is reported and the sampler stays unbound, as there; --texture overrides one
 // by name (PNG, or raw RGBA8 with :WxH).  Videos: the frames of video_png/<stem>/*.png, sorted, the one the video's uniform
@@ -51,16 +52,18 @@ static bool ends_with(const std::string& s, const char* suffix) {
     return s.size() >= n && s.compare(s.size() - n, n, suffix) == 0;
 }
 
+static bool write_bytes(const std::string& output, const std::vector<uint8_t>& bytes, size_t n) {
+    std::ofstream out(output, std::ios::binary);
+    if (!out) return false;
+    out.write(reinterpret_cast<const char*>(bytes.data()), std::streamsize(n));
+    return bool(out);
+}
+
+// .rgba / .ppm frames (PNG frames are encoded on the device and written by write_bytes)
 static bool write_image(const std::string& output, const std::vector<uint8_t>& px, int width, int height) {
     std::ofstream out(output, std::ios::binary);
     if (!out) return false;
-    if (ends_with(output, ".png")) {             // Image::export_png (main.rs:2939-2943)
-        uint8_t* png = nullptr;
-        size_t n = 0;
-        if (ph_png_encode_rgba8(px.data(), width, height, &png, &n)) return false;
-        out.write(reinterpret_cast<const char*>(png), std::streamsize(n));
-        ph_png_free(png);
-    } else if (ends_with(output, ".rgba")) {
+    if (ends_with(output, ".rgba")) {
         out.write(reinterpret_cast<const char*>(px.data()), std::streamsize(px.size()));
     } else {
         out << "P6\n" << width << " " << height << "\n255\n";
@@ -274,14 +277,19 @@ int main(int argc, char** argv) {
         width *= 2;
         ph_player_set_stereo(player, 1, 0.07, 0);
     }
-    std::vector<uint8_t> px(size_t(width) * size_t(height) * 4);
+    const bool png = frame_cmd ? ends_with(output, ".png") : frame_ext == ".png";       // Image::export_png (main.rs:2939-2943)
+    // one buffer for the frame: RGBA8 pixels, or a PNG file of at most pe_png_bound bytes
+    std::vector<uint8_t> px(png ? pe_png_bound(width, height) : size_t(width) * size_t(height) * 4);
+    if (px.empty()) { std::fprintf(stderr, "no PNG for a %d x %d frame\n", width, height); return 1; }
+    size_t png_len = 0;
     ph_frame_params p = {width, height, depth, aa, 0, 0, {0, 0, 0}, 0, 0, 0};
     if (frame_cmd) {
-        if (ph_player_update(player, time) || ph_player_render_frame(player, ctx, &p, px.data(), 1)) {   // main.rs:2928-2929
+        if (ph_player_update(player, time) ||                                                          // main.rs:2928-2929
+            (png ? ph_player_render_frame_png(player, ctx, &p, px.data(), px.size(), &png_len) : ph_player_render_frame(player, ctx, &p, px.data(), 1))) {
             std::fprintf(stderr, "%s\n", ph_player_last_error(player));
             return 1;
         }
-        if (!write_image(output, px, width, height)) { std::fprintf(stderr, "cannot write %s\n", output.c_str()); return 1; }
+        if (!(png ? write_bytes(output, px, png_len) : write_image(output, px, width, height))) { std::fprintf(stderr, "cannot write %s\n", output.c_str()); return 1; }
         std::printf("Rendered `%s` to `%s`\n", scene_path.c_str(), output.c_str());
     } else {
         // --animations a,b: render_named_animations (main.rs:1876-1930); otherwise render_all_animations (:1932-1974): every
@@ -319,12 +327,13 @@ int main(int argc, char** argv) {
             const int todo = max_frames >= 0 && max_frames < count ? max_frames : count;
             for (int i = 0; i < todo; i++) {
                 if (skip_existing && file_exists(dir + "/frame_" + std::to_string(i) + frame_ext)) continue;   // resumes like main.rs:1789-1793
-                if (ph_player_render_motion_blur_frame(player, ctx, &p, i, count, motion_blur, double(duration32), px.data())) {
+                if (png ? ph_player_render_motion_blur_frame_png(player, ctx, &p, i, count, motion_blur, double(duration32), px.data(), px.size(), &png_len)
+                        : ph_player_render_motion_blur_frame(player, ctx, &p, i, count, motion_blur, double(duration32), px.data())) {
                     std::fprintf(stderr, "%s\n", ph_player_last_error(player));
                     return 1;
                 }
                 const std::string name = dir + "/frame_" + std::to_string(i) + frame_ext;
-                if (!write_image(name, px, width, height)) { std::fprintf(stderr, "cannot write %s\n", name.c_str()); return 1; }
+                if (!(png ? write_bytes(name, px, png_len) : write_image(name, px, width, height))) { std::fprintf(stderr, "cannot write %s\n", name.c_str()); return 1; }
                 std::printf("\r%d/%d done      ", i + 1, count);
                 std::fflush(stdout);
             }

@@ -1173,4 +1173,42 @@ int pe_quantize_rgba8(pe_ctx* c, const void* in, void* out, size_t n_pixels, voi
     return 0;
 }
 
+// ------------------------------------------------------------------------------ PNG encoding (pe_png.cu)
+size_t pe_png_bound(int width, int height) { return png_bound(width, height); }
+
+int pe_encode_png_rgba8(pe_ctx* c, const void* rgba8, int width, int height, void* png, size_t capacity, void* size_device, void* stream) {
+    if (!c) return 1;
+    if (!rgba8 || !png || !size_device) return c->fail("pe_encode_png_rgba8: null argument");
+    if (width < 1 || height < 1) return c->fail("pe_encode_png_rgba8: width and height must be at least 1");
+    const size_t bound = png_bound(width, height);
+    if (!bound) return c->fail("pe_encode_png_rgba8: frame too large (its PNG could exceed 2^31 - 1 bytes)");
+    if (capacity < bound) return c->fail("pe_encode_png_rgba8: capacity " + std::to_string(capacity) + " is below pe_png_bound = " + std::to_string(bound));
+    if (uintptr_t(rgba8) & 3) return c->fail("pe_encode_png_rgba8: the frame must be 4-byte aligned");
+    if (!bind_device(c)) return 1;
+    if (!cuda_ok(c, c->png_work.ensure(png_workspace_bytes(width, height)), "cudaMalloc(PNG work space)")) return 1;
+    if (!cuda_ok(c, (cudaError_t)launch_png_encode(rgba8, width, height, c->png_work.dev, png, size_device, stream_of(c, stream)), "pe_encode_png_rgba8"))
+        return 1;
+    c->launches += 5;
+    return 0;
+}
+
+int pe_encode_png_host(pe_ctx* c, const void* rgba8, int width, int height, uint8_t* png_host, size_t capacity, size_t* size_out) {
+    if (!c) return 1;
+    if (!rgba8 || !png_host || !size_out) return c->fail("pe_encode_png_host: null argument");
+    if (width < 1 || height < 1) return c->fail("pe_encode_png_host: width and height must be at least 1");
+    const size_t bound = png_bound(width, height);
+    if (!bound) return c->fail("pe_encode_png_host: frame too large (its PNG could exceed 2^31 - 1 bytes)");
+    if (capacity < bound) return c->fail("pe_encode_png_host: capacity " + std::to_string(capacity) + " is below pe_png_bound = " + std::to_string(bound));
+    if (!bind_device(c)) return 1;
+    if (!cuda_ok(c, c->png_file.ensure(bound), "cudaMalloc(PNG file)") || !cuda_ok(c, c->png_size.ensure(8), "cudaMalloc(PNG length)")) return 1;
+    if (pe_encode_png_rgba8(c, rgba8, width, height, c->png_file.dev, c->png_file.bytes, c->png_size.dev, nullptr)) return 1;
+    uint64_t n = 0;
+    if (!cuda_ok(c, cudaMemcpyAsync(&n, c->png_size.dev, 8, cudaMemcpyDeviceToHost, c->stream), "pe_encode_png_host") ||
+        !cuda_ok(c, cudaStreamSynchronize(c->stream), "pe_encode_png_host") ||
+        !cuda_ok(c, cudaMemcpyAsync(png_host, c->png_file.dev, size_t(n), cudaMemcpyDeviceToHost, c->stream), "pe_encode_png_host") ||
+        !cuda_ok(c, cudaStreamSynchronize(c->stream), "pe_encode_png_host")) return 1;
+    *size_out = size_t(n);
+    return 0;
+}
+
 }  // extern "C"

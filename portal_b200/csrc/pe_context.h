@@ -103,6 +103,9 @@ struct pe_ctx {
     // refill cursor, and the one-sample RGBA8 halo rows above and below the target's strips
     struct AdaptiveBuffers { pe_host::DeviceBuffer refine_list, refine_count, halo_above, halo_below; };
     AdaptiveBuffers adaptive[2];
+    // pe_encode_png_rgba8's work space: filtered stream, per-segment deflate output, segment sizes / offsets / checksums; and
+    // pe_encode_png_host's device copy of the file and its length
+    pe_host::DeviceBuffer png_work, png_file, png_size;
     // adaptive de-specialisation: a slot whose value differed between renders more than kMaxRespecialisations times is read
     // from the constant block from then on (bounds NVRTC compiles when an animation drives an int or a matrix structure)
     std::vector<int> last_ints, int_changes;

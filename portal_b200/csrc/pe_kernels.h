@@ -24,4 +24,14 @@ struct RefineTarget {
 int launch_refine_list(const void* frame, bool rgba8, const RefineTarget& t, const unsigned* above, int above_first,
                        const unsigned* below, int threshold, unsigned* list, unsigned* count, cudaStream_t s);
 
+// PNG encoding on the device (pe_png.cu; the encoding is tests/host_harness/png_spec.cpp): the filtered stream is deflated in
+// segments of kPngSegment bytes, the zlib stream is cut into IDAT chunks of kPngChunk bytes.
+constexpr size_t kPngSegment = 16384, kPngChunk = 8192;
+// Upper bound of the file for a width x height frame; 0 when the size is invalid or the bound does not fit an int32.
+size_t png_bound(int width, int height);
+// Bytes of device work space launch_png_encode needs for a width x height frame (16-byte aligned base).
+size_t png_workspace_bytes(int width, int height);
+// Enqueue the five kernels: RGBA8 frame -> PNG file at `png` (capacity >= png_bound), its length in *(uint64*)size_out.
+int launch_png_encode(const void* rgba8, int width, int height, void* work, void* png, void* size_out, cudaStream_t s);
+
 }  // namespace pe_host

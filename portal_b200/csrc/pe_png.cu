@@ -1,0 +1,411 @@
+// PNG encoder on the device (pe_encode_png_rgba8).  The encoding is restated sequentially in tests/host_harness/png_spec.cpp
+// and described in DESIGN.md section 5.2; these kernels produce its bytes exactly:
+//
+//   pe_k_png_filter    one warp per row: the five candidate filters' costs (sum of min(v, 256 - v)) by warp reductions,
+//                      the smallest (lowest type on a tie) written as type byte + filtered row into the filtered stream F
+//   pe_k_png_deflate   one CTA per kPngSegment bytes of F: the segment and the 32 KiB before it in shared memory, hash chains
+//                      of that window built by one warp (__match_any_sync resolves the positions of one step), then the
+//                      greedy parse by the same warp -- the chain candidates of a token compared 32 bytes per step -- into a
+//                      fixed-Huffman block (or a stored one when that is shorter); also the segment's Adler-32 sums
+//   pe_k_png_scan      one CTA: segment offsets in the zlib stream, the combined Adler-32, signature + IHDR, zlib header,
+//                      checksum, IEND and the file's length
+//   pe_k_png_gather    one CTA per segment: its bytes to their place in the file, around the IDAT chunk headers
+//   pe_k_png_chunks    one thread per IDAT chunk: length, type and CRC-32
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include "pe_kernels.h"
+
+namespace {
+
+using pe_host::kPngChunk;
+using pe_host::kPngSegment;
+constexpr int kWindow = 32768, kHashBits = 15, kChain = 16, kWarp = 32;
+constexpr unsigned kFull = 0xFFFFFFFFu, kNone = 0xFFFFu;
+constexpr size_t kSegCap = kPngSegment + kPngSegment / 8 + 128;     // fixed codes cost at most 9 bits per byte, plus the framing
+constexpr int kDeflateThreads = 512;
+constexpr size_t kDataBytes = kWindow + kPngSegment + 16;
+constexpr size_t kDeflateSmem = kDataBytes + 2 * (kWindow + kPngSegment) + 2 * (size_t(1) << kHashBits);
+constexpr uint32_t kAdlerMod = 65521u;
+
+__constant__ uint16_t c_len_base[29] = {3, 4, 5, 6, 7, 8, 9, 10, 11, 13, 15, 17, 19, 23, 27, 31, 35, 43, 51, 59, 67, 83, 99, 115, 131, 163, 195, 227, 258};
+__constant__ uint8_t c_len_extra[29] = {0, 0, 0, 0, 0, 0, 0, 0, 1, 1, 1, 1, 2, 2, 2, 2, 3, 3, 3, 3, 4, 4, 4, 4, 5, 5, 5, 5, 0};
+__constant__ uint16_t c_dist_base[30] = {1, 2, 3, 4, 5, 7, 9, 13, 17, 25, 33, 49, 65, 97, 129, 193, 257, 385, 513, 769, 1025, 1537, 2049, 3073, 4097, 6145, 8193, 12289, 16385, 24577};
+__constant__ uint8_t c_dist_extra[30] = {0, 0, 0, 0, 1, 1, 2, 2, 3, 3, 4, 4, 5, 5, 6, 6, 7, 7, 8, 8, 9, 9, 10, 10, 11, 11, 12, 12, 13, 13};
+
+// File offset of byte z of the zlib stream: the stream is cut into IDAT chunks of kPngChunk bytes, each framed by 8 bytes
+// (length, type) before and 4 (CRC) after; signature + IHDR take the first 33.
+__device__ __forceinline__ size_t file_offset(size_t z) { return 33 + (z / kPngChunk) * (kPngChunk + 12) + 8 + z % kPngChunk; }
+
+__device__ __forceinline__ int paeth(int a, int b, int c) {
+    const int p = a + b - c, pa = abs(p - a), pb = abs(p - b), pc = abs(p - c);
+    return (pa <= pb && pa <= pc) ? a : (pb <= pc ? b : c);
+}
+
+// The filtered byte of filter `ft` for sample `x` with left a, up b, up-left c.
+__device__ __forceinline__ unsigned filtered(int ft, int x, int a, int b, int c) {
+    const int pred = ft == 0 ? 0 : ft == 1 ? a : ft == 2 ? b : ft == 3 ? ((a + b) >> 1) : paeth(a, b, c);
+    return unsigned(x - pred) & 0xFFu;
+}
+
+__global__ void __launch_bounds__(256) pe_k_png_filter(const uint8_t* __restrict__ rgba, uint8_t* __restrict__ out, int width, int height) {
+    const int y = int(blockIdx.x) * 8 + int(threadIdx.x >> 5), lane = int(threadIdx.x & 31);
+    if (y >= height) return;
+    const size_t rb = size_t(width) * 4;
+    const uint32_t* cur = reinterpret_cast<const uint32_t*>(rgba + size_t(y) * rb);
+    const uint32_t* up = y ? cur - width : nullptr;
+    uint32_t cost[5] = {0, 0, 0, 0, 0};
+    for (int px = lane; px < width; px += kWarp) {
+        const uint32_t x = cur[px], a = px ? cur[px - 1] : 0u, b = up ? up[px] : 0u, c = (up && px) ? up[px - 1] : 0u;
+        for (int k = 0; k < 4; k++) {
+            const int s = 8 * k, xv = int((x >> s) & 0xFF), av = int((a >> s) & 0xFF), bv = int((b >> s) & 0xFF), cv = int((c >> s) & 0xFF);
+#pragma unroll
+            for (int ft = 0; ft < 5; ft++) {
+                const unsigned v = filtered(ft, xv, av, bv, cv);
+                cost[ft] += v < 128 ? v : 256 - v;
+            }
+        }
+    }
+    int best = 0;
+    uint32_t best_cost = 0;
+#pragma unroll
+    for (int ft = 0; ft < 5; ft++) {
+        uint32_t v = cost[ft];
+        for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
+        if (ft == 0 || v < best_cost) { best_cost = v; best = ft; }
+    }
+    uint8_t* dst = out + size_t(y) * (rb + 1);
+    if (lane == 0) dst[0] = uint8_t(best);
+    for (int px = lane; px < width; px += kWarp) {
+        const uint32_t x = cur[px], a = px ? cur[px - 1] : 0u, b = up ? up[px] : 0u, c = (up && px) ? up[px - 1] : 0u;
+        for (int k = 0; k < 4; k++) {
+            const int s = 8 * k;
+            dst[1 + 4 * size_t(px) + k] = uint8_t(filtered(best, int((x >> s) & 0xFF), int((a >> s) & 0xFF), int((b >> s) & 0xFF), int((c >> s) & 0xFF)));
+        }
+    }
+}
+
+// Bit writer of one lane: LSB first, whole bytes go straight to `out`.
+struct BitOut {
+    uint8_t* out;
+    uint32_t pos = 0;
+    uint64_t buf = 0;
+    int cnt = 0;
+    __device__ void put(uint32_t v, int k) {
+        buf |= uint64_t(v) << cnt;
+        cnt += k;
+        while (cnt >= 8) { out[pos++] = uint8_t(buf); buf >>= 8; cnt -= 8; }
+    }
+    __device__ void code(uint32_t c, int k) { put(__brev(c) >> (32 - k), k); }       // Huffman codes go MSB first
+    __device__ void align() { if (cnt) put(0, 8 - cnt); }
+    __device__ void literal(int sym) {                                                  // RFC 1951 3.2.6
+        if (sym < 144) code(0x30u + uint32_t(sym), 8);
+        else if (sym < 256) code(0x190u + uint32_t(sym - 144), 9);
+        else if (sym < 280) code(uint32_t(sym - 256), 7);
+        else code(0xC0u + uint32_t(sym - 280), 8);
+    }
+};
+
+// meta[4 * seg] = {deflate bytes of the segment, Adler-32 s1 sum, Adler-32 weighted sum, 0}
+__global__ void __launch_bounds__(kDeflateThreads, 1) pe_k_png_deflate(const uint8_t* __restrict__ f, size_t n_total, uint8_t* __restrict__ staging,
+                                                                      uint32_t* __restrict__ meta) {
+    extern __shared__ __align__(16) uint8_t smem[];
+    uint8_t* data = smem;                                                              // F[wb, s1)
+    uint16_t* prev = reinterpret_cast<uint16_t*>(smem + kDataBytes);                  // distance to the previous same-hash position (0: none)
+    uint16_t* head = prev + (kWindow + kPngSegment);                                   // latest window position per hash (kNone: none)
+    __shared__ uint64_t red[2][kDeflateThreads / kWarp];
+    __shared__ uint32_t fixed_size;
+    const int tid = int(threadIdx.x), lane = tid & 31, warp = tid >> 5;
+    const size_t seg = blockIdx.x, s0 = seg * kPngSegment, s1 = min(n_total, s0 + kPngSegment);
+    const size_t wb = s0 > size_t(kWindow) ? s0 - kWindow : 0;
+    const int n = int(s1 - wb), i0 = int(s0 - wb);
+    const bool last = s1 == n_total;
+    // wb is a multiple of kPngSegment, so F + wb is 16-byte aligned (F is)
+    const uint4* src = reinterpret_cast<const uint4*>(f + wb);
+    for (int k = tid; k < n / 16; k += kDeflateThreads) reinterpret_cast<uint4*>(data)[k] = src[k];
+    for (int k = (n / 16) * 16 + tid; k < n; k += kDeflateThreads) data[k] = f[wb + size_t(k)];
+    for (int k = tid; k < (1 << kHashBits); k += kDeflateThreads) head[k] = uint16_t(kNone);
+    __syncthreads();
+    // Adler-32 sums of the segment: s1 = sum x_j, s2 = sum (L - j) x_j (combined over segments by pe_k_png_scan)
+    uint64_t a = 0, b = 0;
+    for (int r = i0 + tid; r < n; r += kDeflateThreads) { a += data[r]; b += uint64_t(n - r) * data[r]; }
+    for (int o = 16; o; o >>= 1) { a += __shfl_xor_sync(kFull, a, o); b += __shfl_xor_sync(kFull, b, o); }
+    if (lane == 0) { red[0][warp] = a; red[1][warp] = b; }
+    if (warp == 0) {
+        // hash chains of the window: prev[r] = r - (the nearest earlier position with r's hash), positions r with r + 3 <= n
+        for (int base = 0; base < n; base += kWarp) {
+            const int r = base + lane;
+            const bool valid = r + 3 <= n;
+            const unsigned key = valid ? (((unsigned(data[r]) << 10) ^ (unsigned(data[r + 1]) << 5) ^ unsigned(data[r + 2])) & ((1u << kHashBits) - 1))
+                                       : 0x10000u + unsigned(lane);
+            const unsigned m = __match_any_sync(kFull, key), lower = m & ((1u << lane) - 1u);
+            const unsigned hd = valid ? head[key] : kNone;
+            unsigned pv = 0;
+            if (lower) pv = unsigned(lane - (31 - __clz(lower)));
+            else if (hd != kNone && unsigned(r) - hd <= unsigned(kWindow)) pv = unsigned(r) - hd;
+            if (r < n) prev[r] = uint16_t(valid ? pv : 0u);
+            __syncwarp();
+            if (valid && (m >> lane) == 1u) head[key] = uint16_t(r);
+            __syncwarp();
+        }
+        // greedy parse; every lane takes the same decisions, lane 0 writes the bits
+        BitOut bo{staging + seg * kSegCap};
+        if (lane == 0) { bo.put(last ? 1u : 0u, 1); bo.put(1, 2); }
+        for (int i = i0; i < n;) {
+            int best_len = 0, best_dist = 0;
+            if (i + 3 <= n) {
+                const int max_len = min(258, n - i);
+                int d = prev[i], c = i - d, dist = d;
+                for (int probe = 0; probe < kChain && d != 0 && dist <= kWindow; probe++) {
+                    if (best_len == 0 || data[c + best_len] == data[i + best_len]) {
+                        int l = 0;
+                        for (;;) {
+                            const int k = l + lane;
+                            const bool eq = k < max_len && data[c + k] == data[i + k];
+                            const unsigned ne = __ballot_sync(kFull, !eq);
+                            if (ne) { l += __ffs(int(ne)) - 1; break; }
+                            l += kWarp;
+                        }
+                        if (l > best_len) {
+                            best_len = l;
+                            best_dist = dist;
+                            if (l == max_len) break;
+                        }
+                    }
+                    d = prev[c];
+                    c -= d;
+                    dist += d;
+                }
+            }
+            if (best_len >= 3) {
+                if (lane == 0) {
+                    int li = 28;
+                    while (c_len_base[li] > best_len) li--;
+                    bo.literal(257 + li);
+                    bo.put(uint32_t(best_len - c_len_base[li]), c_len_extra[li]);
+                    int di = 29;
+                    while (c_dist_base[di] > best_dist) di--;
+                    bo.code(uint32_t(di), 5);
+                    bo.put(uint32_t(best_dist - c_dist_base[di]), c_dist_extra[di]);
+                }
+                i += best_len;
+            } else {
+                if (lane == 0) bo.literal(data[i]);
+                i++;
+            }
+        }
+        if (lane == 0) {
+            bo.literal(256);
+            if (!last) {                                          // empty stored block: the segment ends byte-aligned
+                bo.put(0, 3);
+                bo.align();
+                bo.put(0xFFFF0000u, 32);
+            } else {
+                bo.align();
+            }
+            fixed_size = bo.pos;
+        }
+    }
+    __syncthreads();
+    const uint32_t len = uint32_t(s1 - s0);
+    uint32_t size = fixed_size;
+    if (size > len + 5) {                                         // stored is shorter
+        uint8_t* o = staging + seg * kSegCap;
+        if (tid == 0) {
+            o[0] = last ? 1 : 0;
+            o[1] = uint8_t(len);
+            o[2] = uint8_t(len >> 8);
+            o[3] = uint8_t(~len);
+            o[4] = uint8_t(~len >> 8);
+        }
+        for (int k = tid; k < int(len); k += kDeflateThreads) o[5 + k] = data[i0 + k];
+        size = len + 5;
+    }
+    if (tid == 0) {
+        uint64_t sa = 0, sb = 0;
+        for (int w = 0; w < kDeflateThreads / kWarp; w++) { sa += red[0][w]; sb += red[1][w]; }
+        meta[4 * seg] = size;
+        meta[4 * seg + 1] = uint32_t(sa % kAdlerMod);
+        meta[4 * seg + 2] = uint32_t(sb % kAdlerMod);
+        meta[4 * seg + 3] = 0;
+    }
+}
+
+__device__ __forceinline__ void put_be32(uint8_t* p, uint32_t v) {
+    p[0] = uint8_t(v >> 24); p[1] = uint8_t(v >> 16); p[2] = uint8_t(v >> 8); p[3] = uint8_t(v);
+}
+
+struct PngHeader { uint8_t b[33]; };
+
+// One CTA of 1024 threads.  offs[seg] = zlib-stream offset of the segment's first byte; zlen[0] = zlib stream length.
+__global__ void __launch_bounds__(1024) pe_k_png_scan(const uint32_t* __restrict__ meta, int n_seg, size_t n_total, PngHeader hdr,
+                                                      uint32_t* __restrict__ offs, uint32_t* __restrict__ zlen, uint8_t* __restrict__ png,
+                                                      unsigned long long* __restrict__ size_out) {
+    __shared__ uint32_t warp_sum[32];
+    __shared__ uint64_t adler_part[2][32];
+    __shared__ uint32_t carry;
+    const int tid = int(threadIdx.x), lane = tid & 31, warp = tid >> 5;
+    if (tid == 0) carry = 2;                                      // after the zlib header
+    uint64_t sa = 0, sb = 0;
+    for (int base = 0; base < n_seg; base += 1024) {
+        const int seg = base + tid;
+        uint32_t v = seg < n_seg ? meta[4 * seg] : 0u;
+        if (seg < n_seg) {
+            const size_t s1 = min(n_total, size_t(seg + 1) * kPngSegment);
+            const uint64_t A = meta[4 * seg + 1], B = meta[4 * seg + 2];
+            sa += A;
+            sb += ((n_total - s1) % kAdlerMod) * A + B;
+            sb %= kAdlerMod;
+        }
+        uint32_t incl = v;
+        for (int o = 1; o < 32; o <<= 1) {
+            const uint32_t t = __shfl_up_sync(kFull, incl, o);
+            if (lane >= o) incl += t;
+        }
+        if (lane == 31) warp_sum[warp] = incl;
+        __syncthreads();
+        if (warp == 0) {
+            uint32_t w = warp_sum[lane], wi = w;
+            for (int o = 1; o < 32; o <<= 1) {
+                const uint32_t t = __shfl_up_sync(kFull, wi, o);
+                if (lane >= o) wi += t;
+            }
+            warp_sum[lane] = wi - w;                              // exclusive over warps
+        }
+        __syncthreads();
+        if (seg < n_seg) offs[seg] = carry + warp_sum[warp] + incl - v;
+        __syncthreads();
+        if (tid == 1023) carry += warp_sum[31] + incl;
+        __syncthreads();
+    }
+    for (int o = 16; o; o >>= 1) { sa += __shfl_xor_sync(kFull, sa, o); sb += __shfl_xor_sync(kFull, sb, o); }
+    if (lane == 0) { adler_part[0][warp] = sa % kAdlerMod; adler_part[1][warp] = sb % kAdlerMod; }
+    __syncthreads();
+    if (tid < 33) png[tid] = hdr.b[tid];
+    if (tid == 0) {
+        uint64_t A = 0, B = 0;
+        for (int w = 0; w < 32; w++) { A += adler_part[0][w]; B += adler_part[1][w]; }
+        const uint32_t s1 = uint32_t((1 + A) % kAdlerMod), s2 = uint32_t((n_total % kAdlerMod + B) % kAdlerMod);
+        const uint32_t adler = (s2 << 16) | s1;
+        const uint32_t z = carry + 4;
+        *zlen = z;
+        png[file_offset(0)] = 0x78;
+        png[file_offset(1)] = 0x9C;
+        for (int k = 0; k < 4; k++) png[file_offset(carry + k)] = uint8_t(adler >> (24 - 8 * k));
+        const size_t chunks = (size_t(z) + kPngChunk - 1) / kPngChunk;
+        uint8_t* iend = png + 33 + chunks * 12 + z;
+        const uint8_t tail[12] = {0, 0, 0, 0, 'I', 'E', 'N', 'D', 0xAE, 0x42, 0x60, 0x82};
+        for (int k = 0; k < 12; k++) iend[k] = tail[k];
+        *size_out = 33 + chunks * 12 + z + 12;
+    }
+}
+
+__global__ void __launch_bounds__(256) pe_k_png_gather(const uint8_t* __restrict__ staging, const uint32_t* __restrict__ meta,
+                                                       const uint32_t* __restrict__ offs, uint8_t* __restrict__ png) {
+    const size_t seg = blockIdx.x;
+    const uint32_t size = meta[4 * seg], off = offs[seg];
+    const uint8_t* s = staging + seg * kSegCap;
+    for (uint32_t k = threadIdx.x; k < size; k += blockDim.x) png[file_offset(size_t(off) + k)] = s[k];
+}
+
+__global__ void __launch_bounds__(128) pe_k_png_chunks(const uint32_t* __restrict__ zlen, uint8_t* __restrict__ png) {
+    __shared__ uint32_t table[256];
+    for (int i = int(threadIdx.x); i < 256; i += blockDim.x) {
+        uint32_t c = uint32_t(i);
+        for (int k = 0; k < 8; k++) c = (c & 1u) ? 0xEDB88320u ^ (c >> 1) : c >> 1;
+        table[i] = c;
+    }
+    __syncthreads();
+    const size_t z = *zlen, k = size_t(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (k * kPngChunk >= z) return;
+    const uint32_t len = uint32_t(min(size_t(kPngChunk), z - k * kPngChunk));
+    uint8_t* q = png + 33 + k * (kPngChunk + 12);
+    put_be32(q, len);
+    const uint8_t type[4] = {'I', 'D', 'A', 'T'};
+    uint32_t c = 0xFFFFFFFFu;
+    for (int i = 0; i < 4; i++) {
+        q[4 + i] = type[i];
+        c = table[(c ^ type[i]) & 0xFFu] ^ (c >> 8);
+    }
+    for (uint32_t i = 0; i < len; i++) c = table[(c ^ q[8 + i]) & 0xFFu] ^ (c >> 8);
+    put_be32(q + 8 + len, ~c);
+}
+
+uint32_t host_crc32(const uint8_t* d, size_t n) {
+    uint32_t c = 0xFFFFFFFFu;
+    for (size_t i = 0; i < n; i++) {
+        c ^= d[i];
+        for (int k = 0; k < 8; k++) c = (c & 1u) ? 0xEDB88320u ^ (c >> 1) : c >> 1;
+    }
+    return ~c;
+}
+
+struct Layout {
+    size_t n_total, n_seg, filtered, staging, meta, offs, zlen, total;
+};
+
+Layout layout(int width, int height) {
+    Layout L;
+    L.n_total = size_t(height) * (size_t(width) * 4 + 1);
+    L.n_seg = (L.n_total + kPngSegment - 1) / kPngSegment;
+    auto up = [](size_t v) { return (v + 255) & ~size_t(255); };
+    L.filtered = 0;
+    L.staging = up(L.n_total);
+    L.meta = L.staging + up(L.n_seg * kSegCap);
+    L.offs = L.meta + up(L.n_seg * 16);
+    L.zlen = L.offs + up(L.n_seg * 4);
+    L.total = L.zlen + 256;
+    return L;
+}
+
+}  // namespace
+
+namespace pe_host {
+
+size_t png_bound(int width, int height) {
+    if (width < 1 || height < 1) return 0;
+    const size_t n_total = size_t(height) * (size_t(width) * 4 + 1), n_seg = (n_total + kPngSegment - 1) / kPngSegment;
+    const size_t z = 2 + n_total + 5 * n_seg + 4;                  // every segment is at most its stored form
+    const size_t bound = 33 + z + 12 * ((z + kPngChunk - 1) / kPngChunk) + 12;
+    return bound > size_t(INT32_MAX) ? 0 : bound;
+}
+
+size_t png_workspace_bytes(int width, int height) { return layout(width, height).total; }
+
+int launch_png_encode(const void* rgba8, int width, int height, void* work, void* png, void* size_out, cudaStream_t s) {
+    const Layout L = layout(width, height);
+    uint8_t* w = static_cast<uint8_t*>(work);
+    uint8_t* filtered = w + L.filtered;
+    uint8_t* staging = w + L.staging;
+    uint32_t* meta = reinterpret_cast<uint32_t*>(w + L.meta);
+    uint32_t* offs = reinterpret_cast<uint32_t*>(w + L.offs);
+    uint32_t* zlen = reinterpret_cast<uint32_t*>(w + L.zlen);
+    PngHeader hdr;
+    const uint8_t sig[8] = {0x89, 'P', 'N', 'G', '\r', '\n', 0x1A, '\n'};
+    for (int k = 0; k < 8; k++) hdr.b[k] = sig[k];
+    uint8_t* ihdr = hdr.b + 8;                                     // length, type, 13 bytes of data, CRC
+    const uint8_t fixed[8] = {0, 0, 0, 13, 'I', 'H', 'D', 'R'};
+    for (int k = 0; k < 8; k++) ihdr[k] = fixed[k];
+    for (int k = 0; k < 4; k++) {
+        ihdr[8 + k] = uint8_t(uint32_t(width) >> (24 - 8 * k));
+        ihdr[12 + k] = uint8_t(uint32_t(height) >> (24 - 8 * k));
+    }
+    ihdr[16] = 8;                                                  // bit depth
+    ihdr[17] = 6;                                                  // RGBA
+    ihdr[18] = ihdr[19] = ihdr[20] = 0;
+    const uint32_t crc = host_crc32(ihdr + 4, 17);
+    for (int k = 0; k < 4; k++) ihdr[21 + k] = uint8_t(crc >> (24 - 8 * k));
+
+    cudaError_t e = cudaFuncSetAttribute(pe_k_png_deflate, cudaFuncAttributeMaxDynamicSharedMemorySize, int(kDeflateSmem));
+    if (e != cudaSuccess) return int(e);
+    pe_k_png_filter<<<unsigned((height + 7) / 8), 256, 0, s>>>(static_cast<const uint8_t*>(rgba8), filtered, width, height);
+    pe_k_png_deflate<<<unsigned(L.n_seg), kDeflateThreads, kDeflateSmem, s>>>(filtered, L.n_total, staging, meta);
+    pe_k_png_scan<<<1, 1024, 0, s>>>(meta, int(L.n_seg), L.n_total, hdr, offs, zlen, static_cast<uint8_t*>(png),
+                                     static_cast<unsigned long long*>(size_out));
+    pe_k_png_gather<<<unsigned(L.n_seg), 256, 0, s>>>(staging, meta, offs, static_cast<uint8_t*>(png));
+    const size_t max_chunks = (png_bound(width, height) + kPngChunk - 1) / kPngChunk;
+    pe_k_png_chunks<<<unsigned((max_chunks + 127) / 128), 128, 0, s>>>(zlen, static_cast<uint8_t*>(png));
+    return int(cudaGetLastError());
+}
+
+}  // namespace pe_host
