@@ -331,6 +331,25 @@ PE_API int pe_encode_png_rgba8(pe_ctx* ctx, const void* rgba8_device, int width,
 PE_API int pe_encode_png_host(pe_ctx* ctx, const void* rgba8_device, int width, int height, uint8_t* png_host,
                               size_t capacity, size_t* size_out);
 
+/* ---- 16 bits per channel (opt-in; no counterpart in the reference, whose frames are 8-bit) ---------------------------------
+ * For a 10-bit video encode: the float frame of pe_render (or pe_render_adaptive with rgba8 = 0) quantised to unorm16 instead
+ * of unorm8.  An RGBA16 pixel is four uint16 (r, g, b, a) in host byte order, 8 B.  Same argument rules as the RGBA8 forms. */
+/* float RGBA -> RGBA16: q = round_half_even(f32(clamp(v, 0, 1) * 65535)), NaN -> 0.  `rgba_f32_device` 16-byte aligned,
+ * `rgba16_device` 8-byte aligned.  Device pointers; asynchronous on `stream`. */
+PE_API int pe_quantize_rgba16(pe_ctx* ctx, const void* rgba_f32_device, void* rgba16_device, size_t n_pixels, void* stream);
+/* Motion-blur average of 1 <= n <= 64 RGBA16 frames in gamma-2 space, exactly in integers: per channel
+ * m = floor(sum_j q_j^2 / n), out = floor(sqrt(m) + 1/2); alpha = 65535.  Frames and output 8-byte aligned. */
+PE_API int pe_average_frames_rgba16(pe_ctx* ctx, const void* const* frames_device, int n_frames, void* out_device,
+                                    size_t n_pixels, void* stream);
+/* 16-bit PNG (DESIGN.md section 5.3): the encoding above with IHDR bit depth 16, big-endian samples (8 bytes per pixel, row
+ * bytes 8 * width, filters' left neighbour 8 bytes back); restated in tests/host_harness/png16_spec.cpp.  The frame must be
+ * 8-byte aligned.  Bound, device and host forms as for RGBA8, the same work space. */
+PE_API size_t pe_png_bound_rgba16(int width, int height);
+PE_API int pe_encode_png_rgba16(pe_ctx* ctx, const void* rgba16_device, int width, int height, void* png_device,
+                                size_t capacity, void* size_device, void* stream);
+PE_API int pe_encode_png_host_rgba16(pe_ctx* ctx, const void* rgba16_device, int width, int height, uint8_t* png_host,
+                                     size_t capacity, size_t* size_out);
+
 #ifdef __cplusplus
 }
 #endif

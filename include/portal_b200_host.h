@@ -192,6 +192,23 @@ PE_API int ph_player_render_frame_png(ph_player* pl, pe_ctx* ctx, const ph_frame
 PE_API int ph_player_render_motion_blur_frame_png(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index,
                                                   int frame_count, int motion_blur_frames, double duration_seconds,
                                                   uint8_t* png, size_t capacity, size_t* len);
+/* 16-bit twins (opt-in, for 10-bit video encodes; the reference's frames are 8-bit): the same frame, rendered the same way
+ * (adaptive anti-aliasing, stereo and the update hook included) but as floats -- pe_render, or pe_render_adaptive with rgba8 = 0
+ * -- and quantised by pe_quantize_rgba16 instead of to unorm8.  The motion-blur twins run the same sub-frame loop (time,
+ * `_aa_start` = j, update, upload) with RGBA16 sub-frames averaged by pe_average_frames_rgba16.  Output: RGBA16 pixels
+ * (w * h * 4 uint16, host byte order) or a 16-bit PNG encoded by pe_encode_png_rgba16 (capacity >= pe_png_bound_rgba16).
+ * Scratch slots: the frame is staged as RGBA16 in slot 0.  Single frames render their floats into slot 1.  Motion blur with
+ * M sub-frames keeps them in slots 1 .. M (8 B per pixel each) and renders each one's floats into slot M + 1 (16 B per pixel):
+ * 8 * (M + 1) + 16 bytes per pixel, 17.8 GB (16.6 GiB) at 7680 x 4320 with M = 64 (the RGBA8 path: 4 * (M + 1)). */
+PE_API int ph_player_render_frame_rgba16(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, uint16_t* out_host_rgba16);
+PE_API int ph_player_render_frame_png16(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, uint8_t* png, size_t capacity,
+                                        size_t* len);
+PE_API int ph_player_render_motion_blur_frame_rgba16(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index,
+                                                     int frame_count, int motion_blur_frames, double duration_seconds,
+                                                     uint16_t* out_host_rgba16);
+PE_API int ph_player_render_motion_blur_frame_png16(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index,
+                                                    int frame_count, int motion_blur_frames, double duration_seconds,
+                                                    uint8_t* png, size_t capacity, size_t* len);
 
 /* ---- image files either side of the path ------------------------------------------------------------------------
  * Textures reach the reference as PNG files (Texture2D::from_file_with_format, src/main.rs:1066-1085) and frames leave it as

@@ -113,6 +113,11 @@ def lib() -> C.CDLL:
         "pe_png_bound": (C.c_size_t, [i32, i32]),
         "pe_encode_png_rgba8": (i32, [vp, vp, i32, i32, vp, C.c_size_t, vp, vp]),
         "pe_encode_png_host": (i32, [vp, vp, i32, i32, vp, C.c_size_t, C.POINTER(C.c_size_t)]),
+        "pe_quantize_rgba16": (i32, [vp, vp, vp, C.c_size_t, vp]),
+        "pe_average_frames_rgba16": (i32, [vp, C.POINTER(vp), i32, vp, C.c_size_t, vp]),
+        "pe_png_bound_rgba16": (C.c_size_t, [i32, i32]),
+        "pe_encode_png_rgba16": (i32, [vp, vp, i32, i32, vp, C.c_size_t, vp, vp]),
+        "pe_encode_png_host_rgba16": (i32, [vp, vp, i32, i32, vp, C.c_size_t, C.POINTER(C.c_size_t)]),
         "pe_shard_target": (i32, [i32, i32, i32, i32, i32, i32, C.POINTER(PeTarget)]),
         "pe_sharder_create": (i32, [vp, cp, i32, i32, i32, i32, i32, i32, i32, C.POINTER(vp)]),
         "pe_sharder_destroy": (None, [vp]),
@@ -183,6 +188,11 @@ def lib() -> C.CDLL:
         "ph_player_render_frame_png": (i32, [vp, vp, C.POINTER(PhFrameParams), vp, C.c_size_t, C.POINTER(C.c_size_t)]),
         "ph_player_render_motion_blur_frame_png": (i32, [vp, vp, C.POINTER(PhFrameParams), i32, i32, i32, C.c_double, vp, C.c_size_t,
                                                          C.POINTER(C.c_size_t)]),
+        "ph_player_render_frame_rgba16": (i32, [vp, vp, C.POINTER(PhFrameParams), vp]),
+        "ph_player_render_frame_png16": (i32, [vp, vp, C.POINTER(PhFrameParams), vp, C.c_size_t, C.POINTER(C.c_size_t)]),
+        "ph_player_render_motion_blur_frame_rgba16": (i32, [vp, vp, C.POINTER(PhFrameParams), i32, i32, i32, C.c_double, vp]),
+        "ph_player_render_motion_blur_frame_png16": (i32, [vp, vp, C.POINTER(PhFrameParams), i32, i32, i32, C.c_double, vp, C.c_size_t,
+                                                           C.POINTER(C.c_size_t)]),
     })
     for name, (res, args) in sig.items():
         fn = getattr(L, name)
@@ -214,5 +224,21 @@ def encode_png_device(ctx, rgba8) -> bytes:
         raise PortalB200Error(f"pe_png_bound: no PNG for a {w} x {h} frame")
     out, n = (C.c_uint8 * cap)(), C.c_size_t()
     if L.pe_encode_png_host(ctx, C.c_void_p(rgba8.data_ptr()), w, h, out, cap, C.byref(n)):
+        raise PortalB200Error(L.pe_last_error(ctx).decode(errors="replace"))
+    return bytes(memoryview(out)[:n.value])
+
+
+def encode_png16_device(ctx, rgba16) -> bytes:
+    """16-bit PNG file of a CUDA uint16 tensor [h, w, 4] (contiguous, host byte order) encoded on the device by
+    pe_encode_png_host_rgba16 on context `ctx`."""
+    if rgba16.dim() != 3 or rgba16.shape[2] != 4 or not rgba16.is_cuda or str(rgba16.dtype) != "torch.uint16" or not rgba16.is_contiguous():
+        raise ValueError("frame must be a contiguous CUDA uint16 tensor [h, w, 4]")
+    L = lib()
+    h, w = int(rgba16.shape[0]), int(rgba16.shape[1])
+    cap = L.pe_png_bound_rgba16(w, h)
+    if cap == 0:
+        raise PortalB200Error(f"pe_png_bound_rgba16: no PNG for a {w} x {h} frame")
+    out, n = (C.c_uint8 * cap)(), C.c_size_t()
+    if L.pe_encode_png_host_rgba16(ctx, C.c_void_p(rgba16.data_ptr()), w, h, out, cap, C.byref(n)):
         raise PortalB200Error(L.pe_last_error(ctx).decode(errors="replace"))
     return bytes(memoryview(out)[:n.value])

@@ -608,16 +608,47 @@ int ph_player_set_adaptive_aa(ph_player* pl, int on, int threshold) {
     return 0;
 }
 
-// The device half of ph_player_render_motion_blur_frame: the sub-frames and their gamma-2 average, left in scratch slot 0
-// (*out8); the sub-frames use slots 1 .. motion_blur_frames.
+// The frame as RGBA16 in scratch slot 0 (*out16): rendered as floats into slot 1, then quantised.
+static int render_player_rgba16(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, void** out16) {
+    if (upload_player_uniforms(pl, ctx, p)) return 1;
+    pe_target t = {p->width, p->height, p->height, 0, 1, 1, 1};
+    const size_t n = size_t(p->width) * size_t(p->height);
+    void* f32 = nullptr;
+    if (pe_scratch_buffer(ctx, 0, n * 8, out16) || pe_scratch_buffer(ctx, 1, n * 16, &f32) || render_player_device(pl, ctx, &t, 0, f32) ||
+        pe_quantize_rgba16(ctx, f32, *out16, n, nullptr))
+        return pfail(pl, std::string("render failed: ") + pe_last_error(ctx));
+    return 0;
+}
+
+int ph_player_render_frame_rgba16(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, uint16_t* out_host) {
+    if (!pl || !ctx || !p || !out_host) return 1;
+    void* dev = nullptr;
+    if (render_player_rgba16(pl, ctx, p, &dev)) return 1;
+    if (pe_memcpy_d2h(ctx, out_host, dev, size_t(p->width) * size_t(p->height) * 8, nullptr)) return pfail(pl, std::string("render failed: ") + pe_last_error(ctx));
+    return 0;
+}
+
+int ph_player_render_frame_png16(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, uint8_t* png, size_t capacity, size_t* len) {
+    if (!pl || !ctx || !p || !png || !len) return 1;
+    void* dev = nullptr;
+    if (render_player_rgba16(pl, ctx, p, &dev)) return 1;
+    if (pe_encode_png_host_rgba16(ctx, dev, p->width, p->height, png, capacity, len)) return pfail(pl, std::string("PNG encoding failed: ") + pe_last_error(ctx));
+    return 0;
+}
+
+// The device half of ph_player_render_motion_blur_frame*: the sub-frames and their gamma-2 average, left in scratch slot 0
+// (*out); the sub-frames use slots 1 .. motion_blur_frames.  `bits` is the sub-frames' format: 8 -- RGBA8, rendered so by
+// the render kernel; 16 -- RGBA16, each rendered as floats into slot motion_blur_frames + 1 and quantised from there.
 static int motion_blur_device(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index, int frame_count, int motion_blur_frames,
-                              double duration_seconds, void** out8) {
+                              double duration_seconds, int bits, void** out) {
     if (frame_count < 1 || motion_blur_frames < 1 || motion_blur_frames > 64 || frame_index < 0)
         return pfail(pl, "ph_player_render_motion_blur_frame: bad frame arguments");
-    const size_t n = size_t(p->width) * size_t(p->height);
+    const size_t n = size_t(p->width) * size_t(p->height), px_bytes = bits == 16 ? 8 : 4;
     std::vector<void*> sub(size_t(motion_blur_frames), nullptr);
-    int rc = pe_scratch_buffer(ctx, 0, n * 4, out8);
-    for (size_t j = 0; j < sub.size(); j++) rc |= pe_scratch_buffer(ctx, 1 + int(j), n * 4, &sub[j]);
+    void* f32 = nullptr;
+    int rc = pe_scratch_buffer(ctx, 0, n * px_bytes, out);
+    for (size_t j = 0; j < sub.size(); j++) rc |= pe_scratch_buffer(ctx, 1 + int(j), n * px_bytes, &sub[j]);
+    if (bits == 16) rc |= pe_scratch_buffer(ctx, 1 + motion_blur_frames, n * 16, &f32);
     if (rc) pl->err = std::string("device allocation failed: ") + pe_last_error(ctx);
     pe_target t = {p->width, p->height, p->height, 0, 1, 1, 1};
     const double exposure = 0.5;  // main.rs:1787
@@ -629,12 +660,14 @@ static int motion_blur_device(ph_player* pl, pe_ctx* ctx, const ph_frame_params*
         if (pl->hook && pl->hook(pl->hook_user)) { pl->err = "the update hook failed"; rc = 1; break; }   // ... whose tail swaps video frames
         if (upload_player_uniforms(pl, ctx, &q)) {
             rc = 1;
-        } else if (render_player_device(pl, ctx, &t, 1, sub[size_t(j)])) {
+        } else if (bits == 16 ? render_player_device(pl, ctx, &t, 0, f32) || pe_quantize_rgba16(ctx, f32, sub[size_t(j)], n, nullptr)
+                              : render_player_device(pl, ctx, &t, 1, sub[size_t(j)])) {
             pl->err = std::string("render failed: ") + pe_last_error(ctx);
             rc = 1;
         }
     }
-    if (!rc && pe_average_frames_rgba8(ctx, sub.data(), motion_blur_frames, *out8, n, nullptr)) {
+    if (!rc && (bits == 16 ? pe_average_frames_rgba16(ctx, sub.data(), motion_blur_frames, *out, n, nullptr)
+                           : pe_average_frames_rgba8(ctx, sub.data(), motion_blur_frames, *out, n, nullptr))) {
         pl->err = std::string("motion-blur average failed: ") + pe_last_error(ctx);
         rc = 1;
     }
@@ -645,7 +678,7 @@ int ph_player_render_motion_blur_frame(ph_player* pl, pe_ctx* ctx, const ph_fram
                                        int motion_blur_frames, double duration_seconds, uint8_t* out_host) {
     if (!pl || !ctx || !p || !out_host) return 1;
     void* out8 = nullptr;
-    if (motion_blur_device(pl, ctx, p, frame_index, frame_count, motion_blur_frames, duration_seconds, &out8)) return 1;
+    if (motion_blur_device(pl, ctx, p, frame_index, frame_count, motion_blur_frames, duration_seconds, 8, &out8)) return 1;
     if (pe_memcpy_d2h(ctx, out_host, out8, size_t(p->width) * size_t(p->height) * 4, nullptr)) return pfail(pl, std::string("motion-blur average failed: ") + pe_last_error(ctx));
     return 0;
 }
@@ -654,8 +687,26 @@ int ph_player_render_motion_blur_frame_png(ph_player* pl, pe_ctx* ctx, const ph_
                                            int motion_blur_frames, double duration_seconds, uint8_t* png, size_t capacity, size_t* len) {
     if (!pl || !ctx || !p || !png || !len) return 1;
     void* out8 = nullptr;
-    if (motion_blur_device(pl, ctx, p, frame_index, frame_count, motion_blur_frames, duration_seconds, &out8)) return 1;
+    if (motion_blur_device(pl, ctx, p, frame_index, frame_count, motion_blur_frames, duration_seconds, 8, &out8)) return 1;
     if (pe_encode_png_host(ctx, out8, p->width, p->height, png, capacity, len)) return pfail(pl, std::string("PNG encoding failed: ") + pe_last_error(ctx));
+    return 0;
+}
+
+int ph_player_render_motion_blur_frame_rgba16(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index, int frame_count,
+                                              int motion_blur_frames, double duration_seconds, uint16_t* out_host) {
+    if (!pl || !ctx || !p || !out_host) return 1;
+    void* out16 = nullptr;
+    if (motion_blur_device(pl, ctx, p, frame_index, frame_count, motion_blur_frames, duration_seconds, 16, &out16)) return 1;
+    if (pe_memcpy_d2h(ctx, out_host, out16, size_t(p->width) * size_t(p->height) * 8, nullptr)) return pfail(pl, std::string("motion-blur average failed: ") + pe_last_error(ctx));
+    return 0;
+}
+
+int ph_player_render_motion_blur_frame_png16(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index, int frame_count,
+                                             int motion_blur_frames, double duration_seconds, uint8_t* png, size_t capacity, size_t* len) {
+    if (!pl || !ctx || !p || !png || !len) return 1;
+    void* out16 = nullptr;
+    if (motion_blur_device(pl, ctx, p, frame_index, frame_count, motion_blur_frames, duration_seconds, 16, &out16)) return 1;
+    if (pe_encode_png_host_rgba16(ctx, out16, p->width, p->height, png, capacity, len)) return pfail(pl, std::string("PNG encoding failed: ") + pe_last_error(ctx));
     return 0;
 }
 

@@ -4,16 +4,21 @@
 //   portal_b200_render render-frame <scene.ron> [--width W] [--height H] [--render-depth D] [--aa-count N]
 //                      [--time T] [--stage NAME] [--animation NAME] [--camera NAME] [--device K]
 //                      [--texture name=file.png | name=file.rgba:WxH ...] [--assets DIR] [--output out.png|.ppm|.rgba]
-//                      [--adaptive-aa T]
+//                      [--adaptive-aa T] [--bit-depth 8|16]
 //   portal_b200_render render <scene.ron> [--animations a,b,... | --starts-with PREFIX] [--fps N] [--motion-blur-frames M] [--width W]
 //                      [--height H] [--render-depth D] [--aa-count N] [--stereo-image] [--no-skip-existing] [--out-dir DIR] [--max-frames K]
-//                      [--frame-format ppm|png|rgba] [--assets DIR] [--adaptive-aa T]
+//                      [--frame-format ppm|png|rgba] [--assets DIR] [--adaptive-aa T] [--bit-depth 8|16]
 //                      (`portal render`, main.rs:2808-2873 -> render_named_animations :1876-1930 ->
 //                       render_animation :1757-1830; frames are written as DIR/<animation>/frame_<i>.<format>, the
 //                       ffmpeg step is out of scope)
 //
 // --adaptive-aa T (not in the reference; off by default): every frame / sub-frame is traced with one sample, and with all
 // --aa-count samples only where that frame has an edge (a 3x3 unorm8 range above T, pe_render_adaptive).
+//
+// --bit-depth 16 (not in the reference; 8 by default): frames of 16 bits per channel for a 10-bit video encode.  Every frame /
+// sub-frame is rendered as floats and quantised to unorm16 (motion blur averages the RGBA16 sub-frames), then written as a
+// 16-bit PNG (encoded on the device: ph_player_render_frame_png16, pe_encode_png_rgba16), as raw little-endian RGBA16 for
+// .rgba, or as a P6 PPM with maxval 65535 (big-endian samples, alpha dropped).
 //
 // Output: the RGBA8 frame the reference hands to export_png (main.rs:2939-2943) as a PNG when the name ends in .png (encoded
 // on the device: ph_player_render_frame_png / ph_player_render_motion_blur_frame_png, pe_encode_png_rgba8), as raw RGBA8 for
@@ -69,6 +74,27 @@ static bool write_image(const std::string& output, const std::vector<uint8_t>& p
         out << "P6\n" << width << " " << height << "\n255\n";
         for (size_t i = 0; i < size_t(width) * size_t(height); i++) out.write(reinterpret_cast<const char*>(&px[4 * i]), 3);
     }
+    return bool(out);
+}
+
+// The same for an RGBA16 frame (`px` holds its uint16 samples in host byte order): .rgba is raw RGBA16, little-endian; .ppm is
+// P6 with maxval 65535, alpha dropped, samples big-endian (as the format defines)
+static bool write_image16(const std::string& output, const std::vector<uint8_t>& px, int width, int height) {
+    const uint16_t* s = reinterpret_cast<const uint16_t*>(px.data());
+    const size_t n = size_t(width) * size_t(height);
+    const bool rgba = ends_with(output, ".rgba");
+    std::vector<uint8_t> bytes;
+    bytes.reserve(n * (rgba ? 8 : 6));
+    for (size_t i = 0; i < n; i++)
+        for (int k = 0; k < (rgba ? 4 : 3); k++) {
+            const uint16_t v = s[4 * i + size_t(k)];
+            if (rgba) { bytes.push_back(uint8_t(v)); bytes.push_back(uint8_t(v >> 8)); }
+            else { bytes.push_back(uint8_t(v >> 8)); bytes.push_back(uint8_t(v)); }
+        }
+    std::ofstream out(output, std::ios::binary);
+    if (!out) return false;
+    if (!rgba) out << "P6\n" << width << " " << height << "\n65535\n";
+    out.write(reinterpret_cast<const char*>(bytes.data()), std::streamsize(bytes.size()));
     return bool(out);
 }
 
@@ -152,9 +178,9 @@ int main(int argc, char** argv) {
     const bool anim_cmd = argc >= 3 && std::strcmp(argv[1], "render") == 0;
     if (!frame_cmd && !anim_cmd) {
         std::fprintf(stderr, "usage: %s render-frame <scene.ron> [--width W] [--height H] [--render-depth D] [--aa-count N] [--time T] "
-                             "[--stage NAME] [--animation NAME] [--camera NAME] [--device K] [--texture name=file.png|name=file.rgba:WxH] [--assets DIR] [--output out.png|.ppm|.rgba] [--adaptive-aa T]\n"
+                             "[--stage NAME] [--animation NAME] [--camera NAME] [--device K] [--texture name=file.png|name=file.rgba:WxH] [--assets DIR] [--output out.png|.ppm|.rgba] [--adaptive-aa T] [--bit-depth 8|16]\n"
                              "       %s render <scene.ron> [a,b | --animations a,b | --starts-with PREFIX] [--fps N] [--motion-blur-frames M] [--width W] [--height H] "
-                             "[--render-depth D] [--aa-count N] [--stereo-image] [--no-skip-existing] [--out-dir DIR] [--max-frames K] [--adaptive-aa T]\n", argv[0], argv[0]);
+                             "[--render-depth D] [--aa-count N] [--stereo-image] [--no-skip-existing] [--out-dir DIR] [--max-frames K] [--frame-format ppm|png|rgba] [--adaptive-aa T] [--bit-depth 8|16]\n", argv[0], argv[0]);
         return 2;
     }
     std::string scene_path = argv[2], output = "frame.ppm", out_dir = "video";
@@ -162,7 +188,7 @@ int main(int argc, char** argv) {
     int width = frame_cmd ? 1920 : 3840, height = frame_cmd ? 1080 : 2160, depth = frame_cmd ? 100 : 150, aa = frame_cmd ? 1 : 4, device = 0;
     int fps = 60, motion_blur = 1, max_frames = -1;
     bool stereo = false, skip_existing = true, adaptive = false;
-    int adaptive_threshold = 0;
+    int adaptive_threshold = 0, bits = 8;
     double time = 0.0;
     std::vector<std::string> textures;
     std::string stage, animation, camera, animations, starts_with, assets, frame_ext = ".ppm";
@@ -199,6 +225,11 @@ int main(int argc, char** argv) {
             if (!*v || *end) { std::fprintf(stderr, "--adaptive-aa needs an integer threshold, got `%s`\n", v); return 2; }
             adaptive = true;
             adaptive_threshold = int(std::max(-1L, std::min(t, 255L)));
+        }
+        else if (a == "--bit-depth" || a == "--bit_depth") {
+            const std::string v = next();
+            if (v != "8" && v != "16") { std::fprintf(stderr, "--bit-depth must be 8 or 16, got `%s`\n", v.c_str()); return 2; }
+            bits = std::atoi(v.c_str());
         }
         else { std::fprintf(stderr, "unknown option %s\n", a.c_str()); return 2; }
     }
@@ -278,18 +309,24 @@ int main(int argc, char** argv) {
         ph_player_set_stereo(player, 1, 0.07, 0);
     }
     const bool png = frame_cmd ? ends_with(output, ".png") : frame_ext == ".png";       // Image::export_png (main.rs:2939-2943)
-    // one buffer for the frame: RGBA8 pixels, or a PNG file of at most pe_png_bound bytes
-    std::vector<uint8_t> px(png ? pe_png_bound(width, height) : size_t(width) * size_t(height) * 4);
+    // one buffer for the frame: RGBA8 / RGBA16 pixels, or a PNG file of at most pe_png_bound(_rgba16) bytes
+    const bool b16 = bits == 16;
+    std::vector<uint8_t> px(png ? (b16 ? pe_png_bound_rgba16(width, height) : pe_png_bound(width, height)) : size_t(width) * size_t(height) * (b16 ? 8 : 4));
     if (px.empty()) { std::fprintf(stderr, "no PNG for a %d x %d frame\n", width, height); return 1; }
     size_t png_len = 0;
+    uint16_t* px16 = reinterpret_cast<uint16_t*>(px.data());
+    auto write_frame = [&](const std::string& name) {
+        return png ? write_bytes(name, px, png_len) : b16 ? write_image16(name, px, width, height) : write_image(name, px, width, height);
+    };
     ph_frame_params p = {width, height, depth, aa, 0, 0, {0, 0, 0}, 0, 0, 0};
     if (frame_cmd) {
         if (ph_player_update(player, time) ||                                                          // main.rs:2928-2929
-            (png ? ph_player_render_frame_png(player, ctx, &p, px.data(), px.size(), &png_len) : ph_player_render_frame(player, ctx, &p, px.data(), 1))) {
+            (png ? (b16 ? ph_player_render_frame_png16 : ph_player_render_frame_png)(player, ctx, &p, px.data(), px.size(), &png_len)
+                 : b16 ? ph_player_render_frame_rgba16(player, ctx, &p, px16) : ph_player_render_frame(player, ctx, &p, px.data(), 1))) {
             std::fprintf(stderr, "%s\n", ph_player_last_error(player));
             return 1;
         }
-        if (!(png ? write_bytes(output, px, png_len) : write_image(output, px, width, height))) { std::fprintf(stderr, "cannot write %s\n", output.c_str()); return 1; }
+        if (!write_frame(output)) { std::fprintf(stderr, "cannot write %s\n", output.c_str()); return 1; }
         std::printf("Rendered `%s` to `%s`\n", scene_path.c_str(), output.c_str());
     } else {
         // --animations a,b: render_named_animations (main.rs:1876-1930); otherwise render_all_animations (:1932-1974): every
@@ -327,13 +364,15 @@ int main(int argc, char** argv) {
             const int todo = max_frames >= 0 && max_frames < count ? max_frames : count;
             for (int i = 0; i < todo; i++) {
                 if (skip_existing && file_exists(dir + "/frame_" + std::to_string(i) + frame_ext)) continue;   // resumes like main.rs:1789-1793
-                if (png ? ph_player_render_motion_blur_frame_png(player, ctx, &p, i, count, motion_blur, double(duration32), px.data(), px.size(), &png_len)
-                        : ph_player_render_motion_blur_frame(player, ctx, &p, i, count, motion_blur, double(duration32), px.data())) {
+                const double dur = double(duration32);
+                if (png ? (b16 ? ph_player_render_motion_blur_frame_png16 : ph_player_render_motion_blur_frame_png)(player, ctx, &p, i, count, motion_blur, dur, px.data(), px.size(), &png_len)
+                        : b16 ? ph_player_render_motion_blur_frame_rgba16(player, ctx, &p, i, count, motion_blur, dur, px16)
+                              : ph_player_render_motion_blur_frame(player, ctx, &p, i, count, motion_blur, dur, px.data())) {
                     std::fprintf(stderr, "%s\n", ph_player_last_error(player));
                     return 1;
                 }
                 const std::string name = dir + "/frame_" + std::to_string(i) + frame_ext;
-                if (!(png ? write_bytes(name, px, png_len) : write_image(name, px, width, height))) { std::fprintf(stderr, "cannot write %s\n", name.c_str()); return 1; }
+                if (!write_frame(name)) { std::fprintf(stderr, "cannot write %s\n", name.c_str()); return 1; }
                 std::printf("\r%d/%d done      ", i + 1, count);
                 std::fflush(stdout);
             }

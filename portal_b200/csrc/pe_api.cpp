@@ -1173,42 +1173,97 @@ int pe_quantize_rgba8(pe_ctx* c, const void* in, void* out, size_t n_pixels, voi
     return 0;
 }
 
-// ------------------------------------------------------------------------------ PNG encoding (pe_png.cu)
-size_t pe_png_bound(int width, int height) { return png_bound(width, height); }
-
-int pe_encode_png_rgba8(pe_ctx* c, const void* rgba8, int width, int height, void* png, size_t capacity, void* size_device, void* stream) {
+int pe_average_frames_rgba16(pe_ctx* c, const void* const* frames, int n_frames, void* out, size_t n_pixels, void* stream) {
     if (!c) return 1;
-    if (!rgba8 || !png || !size_device) return c->fail("pe_encode_png_rgba8: null argument");
-    if (width < 1 || height < 1) return c->fail("pe_encode_png_rgba8: width and height must be at least 1");
-    const size_t bound = png_bound(width, height);
-    if (!bound) return c->fail("pe_encode_png_rgba8: frame too large (its PNG could exceed 2^31 - 1 bytes)");
-    if (capacity < bound) return c->fail("pe_encode_png_rgba8: capacity " + std::to_string(capacity) + " is below pe_png_bound = " + std::to_string(bound));
-    if (uintptr_t(rgba8) & 3) return c->fail("pe_encode_png_rgba8: the frame must be 4-byte aligned");
+    if (!frames || !out || n_frames < 1 || n_frames > 64) return c->fail("pe_average_frames_rgba16: bad arguments (1 <= n_frames <= 64)");
+    bool aligned = (uintptr_t(out) & 7) == 0;
+    for (int i = 0; i < n_frames; i++) aligned = aligned && frames[i] && (uintptr_t(frames[i]) & 7) == 0;
+    if (!aligned) return c->fail("pe_average_frames_rgba16: the frames and the output must be 8-byte aligned");
     if (!bind_device(c)) return 1;
-    if (!cuda_ok(c, c->png_work.ensure(png_workspace_bytes(width, height)), "cudaMalloc(PNG work space)")) return 1;
-    if (!cuda_ok(c, (cudaError_t)launch_png_encode(rgba8, width, height, c->png_work.dev, png, size_device, stream_of(c, stream)), "pe_encode_png_rgba8"))
+    const cudaStream_t s = stream_of(c, stream);
+    if (!cuda_ok(c, (cudaError_t)launch_average_rgba16(frames, n_frames, out, n_pixels, c->sm_count, s), "average")) return 1;
+    c->launches++;
+    return 0;
+}
+
+int pe_quantize_rgba16(pe_ctx* c, const void* in, void* out, size_t n_pixels, void* stream) {
+    if (!c) return 1;
+    if (!in || !out) return c->fail("pe_quantize_rgba16: bad arguments");
+    if ((uintptr_t(in) & 15) || (uintptr_t(out) & 7)) return c->fail("pe_quantize_rgba16: the float frame must be 16-byte and the output 8-byte aligned");
+    if (!bind_device(c)) return 1;
+    const cudaStream_t s = stream_of(c, stream);
+    if (!cuda_ok(c, (cudaError_t)launch_quantize_rgba16(in, out, n_pixels, c->sm_count, s), "quantize")) return 1;
+    c->launches++;
+    return 0;
+}
+
+// ------------------------------------------------------------------------------ PNG encoding (pe_png.cu)
+size_t pe_png_bound(int width, int height) { return png_bound(width, height, 4); }
+size_t pe_png_bound_rgba16(int width, int height) { return png_bound(width, height, 8); }
+
+}  // extern "C"
+
+namespace {
+
+// pe_encode_png_rgba8 / _rgba16 (`bpp` 4 / 8 bytes per pixel; the frame must be aligned to one pixel word)
+int encode_png(pe_ctx* c, const char* name, int bpp, const void* rgba, int width, int height, void* png, size_t capacity, void* size_device,
+               void* stream) {
+    const std::string fn = name;
+    if (!rgba || !png || !size_device) return c->fail(fn + ": null argument");
+    if (width < 1 || height < 1) return c->fail(fn + ": width and height must be at least 1");
+    const size_t bound = png_bound(width, height, bpp);
+    if (!bound) return c->fail(fn + ": frame too large (its PNG could exceed 2^31 - 1 bytes)");
+    const char* bound_fn = bpp == 4 ? "pe_png_bound" : "pe_png_bound_rgba16";
+    if (capacity < bound) return c->fail(fn + ": capacity " + std::to_string(capacity) + " is below " + bound_fn + " = " + std::to_string(bound));
+    if (uintptr_t(rgba) & uintptr_t(bpp - 1)) return c->fail(fn + ": the frame must be " + std::to_string(bpp) + "-byte aligned");
+    if (!bind_device(c)) return 1;
+    if (!cuda_ok(c, c->png_work.ensure(png_workspace_bytes(width, height, bpp)), "cudaMalloc(PNG work space)")) return 1;
+    if (!cuda_ok(c, (cudaError_t)launch_png_encode(rgba, width, height, bpp, c->png_work.dev, png, size_device, stream_of(c, stream)), name))
         return 1;
     c->launches += 5;
     return 0;
 }
 
-int pe_encode_png_host(pe_ctx* c, const void* rgba8, int width, int height, uint8_t* png_host, size_t capacity, size_t* size_out) {
-    if (!c) return 1;
-    if (!rgba8 || !png_host || !size_out) return c->fail("pe_encode_png_host: null argument");
-    if (width < 1 || height < 1) return c->fail("pe_encode_png_host: width and height must be at least 1");
-    const size_t bound = png_bound(width, height);
-    if (!bound) return c->fail("pe_encode_png_host: frame too large (its PNG could exceed 2^31 - 1 bytes)");
-    if (capacity < bound) return c->fail("pe_encode_png_host: capacity " + std::to_string(capacity) + " is below pe_png_bound = " + std::to_string(bound));
+// pe_encode_png_host / _host_rgba16: the device form into the context's own file buffer, then read back
+int encode_png_host(pe_ctx* c, const char* name, const char* device_name, int bpp, const void* rgba, int width, int height, uint8_t* png_host,
+                    size_t capacity, size_t* size_out) {
+    const std::string fn = name;
+    if (!rgba || !png_host || !size_out) return c->fail(fn + ": null argument");
+    if (width < 1 || height < 1) return c->fail(fn + ": width and height must be at least 1");
+    const size_t bound = png_bound(width, height, bpp);
+    if (!bound) return c->fail(fn + ": frame too large (its PNG could exceed 2^31 - 1 bytes)");
+    const char* bound_fn = bpp == 4 ? "pe_png_bound" : "pe_png_bound_rgba16";
+    if (capacity < bound) return c->fail(fn + ": capacity " + std::to_string(capacity) + " is below " + bound_fn + " = " + std::to_string(bound));
     if (!bind_device(c)) return 1;
     if (!cuda_ok(c, c->png_file.ensure(bound), "cudaMalloc(PNG file)") || !cuda_ok(c, c->png_size.ensure(8), "cudaMalloc(PNG length)")) return 1;
-    if (pe_encode_png_rgba8(c, rgba8, width, height, c->png_file.dev, c->png_file.bytes, c->png_size.dev, nullptr)) return 1;
+    if (encode_png(c, device_name, bpp, rgba, width, height, c->png_file.dev, c->png_file.bytes, c->png_size.dev, nullptr)) return 1;
     uint64_t n = 0;
-    if (!cuda_ok(c, cudaMemcpyAsync(&n, c->png_size.dev, 8, cudaMemcpyDeviceToHost, c->stream), "pe_encode_png_host") ||
-        !cuda_ok(c, cudaStreamSynchronize(c->stream), "pe_encode_png_host") ||
-        !cuda_ok(c, cudaMemcpyAsync(png_host, c->png_file.dev, size_t(n), cudaMemcpyDeviceToHost, c->stream), "pe_encode_png_host") ||
-        !cuda_ok(c, cudaStreamSynchronize(c->stream), "pe_encode_png_host")) return 1;
+    if (!cuda_ok(c, cudaMemcpyAsync(&n, c->png_size.dev, 8, cudaMemcpyDeviceToHost, c->stream), name) ||
+        !cuda_ok(c, cudaStreamSynchronize(c->stream), name) ||
+        !cuda_ok(c, cudaMemcpyAsync(png_host, c->png_file.dev, size_t(n), cudaMemcpyDeviceToHost, c->stream), name) ||
+        !cuda_ok(c, cudaStreamSynchronize(c->stream), name)) return 1;
     *size_out = size_t(n);
     return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int pe_encode_png_rgba8(pe_ctx* c, const void* rgba8, int width, int height, void* png, size_t capacity, void* size_device, void* stream) {
+    return c ? encode_png(c, "pe_encode_png_rgba8", 4, rgba8, width, height, png, capacity, size_device, stream) : 1;
+}
+
+int pe_encode_png_host(pe_ctx* c, const void* rgba8, int width, int height, uint8_t* png_host, size_t capacity, size_t* size_out) {
+    return c ? encode_png_host(c, "pe_encode_png_host", "pe_encode_png_rgba8", 4, rgba8, width, height, png_host, capacity, size_out) : 1;
+}
+
+int pe_encode_png_rgba16(pe_ctx* c, const void* rgba16, int width, int height, void* png, size_t capacity, void* size_device, void* stream) {
+    return c ? encode_png(c, "pe_encode_png_rgba16", 8, rgba16, width, height, png, capacity, size_device, stream) : 1;
+}
+
+int pe_encode_png_host_rgba16(pe_ctx* c, const void* rgba16, int width, int height, uint8_t* png_host, size_t capacity, size_t* size_out) {
+    return c ? encode_png_host(c, "pe_encode_png_host_rgba16", "pe_encode_png_rgba16", 8, rgba16, width, height, png_host, capacity, size_out) : 1;
 }
 
 }  // extern "C"

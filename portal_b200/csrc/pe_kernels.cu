@@ -7,6 +7,8 @@
 //   pe_k_deinterleave       rank-major gathered strips -> row-major frame (SURVEY.md §8e)
 //   pe_k_average_rgba8      motion-blur average in gamma-2 space = average_images
 //                           (/root/reference/src/main.rs:640-722): square, integer mean, rounded sqrt
+//   pe_k_quantize_rgba16    float RGBA -> RGBA16 (unorm16, host byte order): what an RGBA16 target would store
+//   pe_k_average_rgba16     average_images at 16 bits per channel, in exact integers
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -166,6 +168,117 @@ __global__ void __launch_bounds__(256) pe_k_average_rgba8_px(FramePtrs frames, i
     }
 }
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+
+// ---- 16 bits per channel.  A pixel is four uint16 in host byte order: as a uint2, x = r | g << 16, y = b | a << 16.
+__device__ __forceinline__ unsigned quant16(float v) {
+    // as quant8, at 65535: clamp to [0,1] (NaN -> 0), an f32 product, round half to even
+    v = fminf(fmaxf(v, 0.0f), 1.0f);
+    return (unsigned)__float2int_rn(v * 65535.0f);
+}
+__device__ __forceinline__ uint2 pack16(float4 p) { return make_uint2(quant16(p.x) | (quant16(p.y) << 16), quant16(p.z) | (quant16(p.w) << 16)); }
+
+// float RGBA -> RGBA16.  A thread owns 4 consecutive pixels: four 16-byte loads, two 16-byte stores; PE_Q_UNROLL groups are
+// loaded before the first store (8 loads, 128 B in flight per thread).
+__global__ void __launch_bounds__(256) pe_k_quantize_rgba16(const float4* __restrict__ in, uint4* __restrict__ out, size_t n) {
+    const size_t n4 = n >> 2;
+    const size_t stride = size_t(gridDim.x) * blockDim.x;
+    size_t g = size_t(blockIdx.x) * blockDim.x + threadIdx.x;
+    for (; g + (PE_Q_UNROLL - 1) * stride < n4; g += PE_Q_UNROLL * stride) {
+        float4 p[PE_Q_UNROLL][4];
+#pragma unroll
+        for (int u = 0; u < PE_Q_UNROLL; u++)
+#pragma unroll
+            for (int k = 0; k < 4; k++) p[u][k] = ld_stream(in + 4 * (g + u * stride) + k);
+#pragma unroll
+        for (int u = 0; u < PE_Q_UNROLL; u++) {
+            const uint2 a = pack16(p[u][0]), b = pack16(p[u][1]), c = pack16(p[u][2]), d = pack16(p[u][3]);
+            st_stream(out + 2 * (g + u * stride), make_uint4(a.x, a.y, b.x, b.y));
+            st_stream(out + 2 * (g + u * stride) + 1, make_uint4(c.x, c.y, d.x, d.y));
+        }
+    }
+    for (; g < n4; g += stride) {
+        float4 p[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++) p[k] = ld_stream(in + 4 * g + k);
+        const uint2 a = pack16(p[0]), b = pack16(p[1]), c = pack16(p[2]), d = pack16(p[3]);
+        st_stream(out + 2 * g, make_uint4(a.x, a.y, b.x, b.y));
+        st_stream(out + 2 * g + 1, make_uint4(c.x, c.y, d.x, d.y));
+    }
+    const size_t i = (n4 << 2) + size_t(blockIdx.x) * blockDim.x + threadIdx.x;   // ragged tail: at most 3 pixels
+    if (i < n) reinterpret_cast<uint2*>(out)[i] = pack16(in[i]);
+}
+// Scalar form for an output that is 8- but not 16-byte aligned: one pixel per thread.
+__global__ void __launch_bounds__(256) pe_k_quantize_rgba16_px(const float4* __restrict__ in, uint2* __restrict__ out, size_t n) {
+    const size_t stride = size_t(gridDim.x) * blockDim.x;
+    for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) out[i] = pack16(in[i]);
+}
+
+// The 16-bit motion-blur channel: sum = sum_j q_j^2 over n frames (< 64 * 65535^2 < 2^39), m = floor(sum / n),
+// out = floor(sqrt(m) + 1/2), all exact.
+// floor(sum / n) for n >= 2 is __umul64hi(sum, magic) with magic = ceil(2^64 / n) = (2^64 - 1) / n + 1: the product exceeds
+// sum / n by sum * e / (n 2^64) with e = magic * n - 2^64 < n, less than 2^39 * 64 / 2^64 / n, far below the 1/n the
+// fractional part of sum / n leaves before the next integer.
+// m <= 65535^2 < 2^32; k = floor(sqrt(m)) from the f32 square root is off by at most one (the relative error of the float
+// conversion and of sqrtf is ~2^-24, ~0.004 at k = 65535) and is corrected with exact 64-bit squares.  Then
+// sqrt(m) + 1/2 >= k + 1  <=>  m >= k^2 + k + 1/4  <=>  m - k^2 > k.
+__device__ __forceinline__ unsigned round_sqrt_mean16(unsigned long long sum, unsigned long long magic, unsigned nn) {
+    const unsigned m = unsigned(nn == 1u ? sum : __umul64hi(sum, magic));
+    unsigned k = __float2uint_rz(sqrtf(__uint2float_rn(m)));
+    if (uint64_t(k) * k > m) k--;
+    else if (uint64_t(k + 1) * (k + 1) <= m) k++;
+    return k + (m - k * k > k ? 1u : 0u);
+}
+__device__ __forceinline__ void acc_sq16(uint2 w, unsigned long long (&s)[3]) {
+    const unsigned r = w.x & 0xffffu, g = w.x >> 16, b = w.y & 0xffffu;
+    s[0] += (unsigned long long)r * r;
+    s[1] += (unsigned long long)g * g;
+    s[2] += (unsigned long long)b * b;
+}
+__device__ __forceinline__ uint2 mean16(const unsigned long long (&s)[3], unsigned long long magic, unsigned nn) {
+    return make_uint2(round_sqrt_mean16(s[0], magic, nn) | (round_sqrt_mean16(s[1], magic, nn) << 16),
+                      round_sqrt_mean16(s[2], magic, nn) | 0xffff0000u);
+}
+
+// Motion-blur mean at 16 bits, the shape of pe_k_average_rgba8: a thread owns 2 consecutive pixels (one 16-byte load per
+// sub-frame, one 16-byte store); the loads of 4 sub-frames are issued together.
+__global__ void __launch_bounds__(256) pe_k_average_rgba16(FramePtrs frames, int n_frames, unsigned long long magic, uint4* __restrict__ out, size_t n) {
+    const size_t n2 = n >> 1;
+    const size_t stride = size_t(gridDim.x) * blockDim.x;
+    const unsigned nn = (unsigned)n_frames;
+    for (size_t g = size_t(blockIdx.x) * blockDim.x + threadIdx.x; g < n2; g += stride) {
+        unsigned long long s0[3] = {0, 0, 0}, s1[3] = {0, 0, 0};
+        int f = 0;
+        for (; f + 4 <= n_frames; f += 4) {
+            uint4 v[4];
+#pragma unroll
+            for (int k = 0; k < 4; k++) v[k] = ld_stream(reinterpret_cast<const uint4*>(frames.p[f + k]) + g);
+#pragma unroll
+            for (int k = 0; k < 4; k++) { acc_sq16(make_uint2(v[k].x, v[k].y), s0); acc_sq16(make_uint2(v[k].z, v[k].w), s1); }
+        }
+        for (; f < n_frames; f++) {
+            const uint4 v = ld_stream(reinterpret_cast<const uint4*>(frames.p[f]) + g);
+            acc_sq16(make_uint2(v.x, v.y), s0);
+            acc_sq16(make_uint2(v.z, v.w), s1);
+        }
+        const uint2 a = mean16(s0, magic, nn), b = mean16(s1, magic, nn);
+        st_stream(out + g, make_uint4(a.x, a.y, b.x, b.y));
+    }
+    const size_t i = (n2 << 1) + size_t(blockIdx.x) * blockDim.x + threadIdx.x;   // ragged tail: at most 1 pixel
+    if (i < n) {
+        unsigned long long s[3] = {0, 0, 0};
+        for (int f = 0; f < n_frames; f++) acc_sq16(reinterpret_cast<const uint2*>(frames.p[f])[i], s);
+        reinterpret_cast<uint2*>(out)[i] = mean16(s, magic, nn);
+    }
+}
+// Scalar form for buffers that are 8- but not 16-byte aligned: one pixel per thread.
+__global__ void __launch_bounds__(256) pe_k_average_rgba16_px(FramePtrs frames, int n_frames, unsigned long long magic, uint2* __restrict__ out, size_t n) {
+    const size_t stride = size_t(gridDim.x) * blockDim.x;
+    for (size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {
+        unsigned long long s[3] = {0, 0, 0};
+        for (int f = 0; f < n_frames; f++) acc_sq16(reinterpret_cast<const uint2*>(frames.p[f])[i], s);
+        out[i] = mean16(s, magic, unsigned(n_frames));
+    }
+}
 
 // Cross-GPU signal: after everything earlier in the stream (the render kernel's remote stores
 // included) one thread publishes `value` to up to 8 flag words, which may live in peer memory.
@@ -346,6 +459,24 @@ int launch_average_rgba8(const void* const* frames, int n_frames, void* out, siz
     const unsigned magic = n_frames > 1 ? unsigned(((1ull << 32) + unsigned(n_frames) - 1) / unsigned(n_frames)) : 0u;
     if (vec) pe_k_average_rgba8<<<grid_for((n + 3) / 4, sms), 256, 0, s>>>(fp, n_frames, magic, (uchar4*)out, n);
     else pe_k_average_rgba8_px<<<grid_for(n, sms), 256, 0, s>>>(fp, n_frames, (unsigned*)out, n);
+    return (int)cudaGetLastError();
+}
+
+int launch_quantize_rgba16(const void* in, void* out, size_t n, int sms, cudaStream_t s) {
+    if (aligned16(out)) pe_k_quantize_rgba16<<<grid_for((n + 3) / 4, sms), 256, 0, s>>>((const float4*)in, (uint4*)out, n);
+    else pe_k_quantize_rgba16_px<<<grid_for(n, sms), 256, 0, s>>>((const float4*)in, (uint2*)out, n);
+    return (int)cudaGetLastError();
+}
+
+int launch_average_rgba16(const void* const* frames, int n_frames, void* out, size_t n, int sms, cudaStream_t s) {
+    if (n_frames < 1 || n_frames > PE_MAX_AVG_FRAMES) return (int)cudaErrorInvalidValue;
+    FramePtrs fp;
+    for (int i = 0; i < n_frames; i++) fp.p[i] = (const uchar4*)frames[i];
+    bool vec = aligned16(out);
+    for (int i = 0; i < n_frames; i++) vec = vec && aligned16(frames[i]);
+    const unsigned long long magic = n_frames > 1 ? ~0ull / unsigned(n_frames) + 1ull : 0ull;
+    if (vec) pe_k_average_rgba16<<<grid_for((n + 1) / 2, sms), 256, 0, s>>>(fp, n_frames, magic, (uint4*)out, n);
+    else pe_k_average_rgba16_px<<<grid_for(n, sms), 256, 0, s>>>(fp, n_frames, magic, (uint2*)out, n);
     return (int)cudaGetLastError();
 }
 

@@ -10,6 +10,9 @@ int launch_deinterleave(const void* gathered, void* frame, int width, int height
                         int strips_per_rank, int sms, cudaStream_t s);
 int launch_signal(void* const* ptrs, int n, unsigned int value, cudaStream_t s);
 int launch_average_rgba8(const void* const* frames, int n_frames, void* out, size_t n_pixels, int sms, cudaStream_t s);
+// 16 bits per channel (host byte order): `rgba16` / `out` / the frames 8-byte aligned, `rgba_f32` 16-byte aligned
+int launch_quantize_rgba16(const void* rgba_f32, void* rgba16, size_t n_pixels, int sms, cudaStream_t s);
+int launch_average_rgba16(const void* const* frames, int n_frames, void* out, size_t n_pixels, int sms, cudaStream_t s);
 // *count += number of 16-byte words in which a and b differ (bitwise); both 16-byte aligned
 int launch_count_diff(const void* a, const void* b, size_t n_words16, unsigned* count, int sms, cudaStream_t s);
 // The rows of a render target (pe_target) the edge mask walks: local rows [0, local_rows) are those that can hold frame rows.
@@ -27,11 +30,12 @@ int launch_refine_list(const void* frame, bool rgba8, const RefineTarget& t, con
 // PNG encoding on the device (pe_png.cu; the encoding is tests/host_harness/png_spec.cpp): the filtered stream is deflated in
 // segments of kPngSegment bytes, the zlib stream is cut into IDAT chunks of kPngChunk bytes.
 constexpr size_t kPngSegment = 16384, kPngChunk = 8192;
+// `bpp`: bytes per pixel, 4 (RGBA8) or 8 (RGBA16 in host byte order, a 16-bit PNG).
 // Upper bound of the file for a width x height frame; 0 when the size is invalid or the bound does not fit an int32.
-size_t png_bound(int width, int height);
+size_t png_bound(int width, int height, int bpp);
 // Bytes of device work space launch_png_encode needs for a width x height frame (16-byte aligned base).
-size_t png_workspace_bytes(int width, int height);
-// Enqueue the five kernels: RGBA8 frame -> PNG file at `png` (capacity >= png_bound), its length in *(uint64*)size_out.
-int launch_png_encode(const void* rgba8, int width, int height, void* work, void* png, void* size_out, cudaStream_t s);
+size_t png_workspace_bytes(int width, int height, int bpp);
+// Enqueue the five kernels: frame -> PNG file at `png` (capacity >= png_bound), its length in *(uint64*)size_out.
+int launch_png_encode(const void* rgba, int width, int height, int bpp, void* work, void* png, void* size_out, cudaStream_t s);
 
 }  // namespace pe_host

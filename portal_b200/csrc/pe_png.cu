@@ -1,8 +1,10 @@
-// PNG encoder on the device (pe_encode_png_rgba8).  The encoding is restated sequentially in tests/host_harness/png_spec.cpp
-// and described in DESIGN.md section 5.2; these kernels produce its bytes exactly:
+// PNG encoder on the device (pe_encode_png_rgba8, pe_encode_png_rgba16).  The encoding is restated sequentially in
+// tests/host_harness/png_spec.cpp (8 bits) and png16_spec.cpp (16 bits) and described in DESIGN.md sections 5.2 and 5.3; these
+// kernels produce its bytes exactly.  Only the filter kernel and the IHDR depend on the bit depth; the rest works on bytes:
 //
 //   pe_k_png_filter    one warp per row: the five candidate filters' costs (sum of min(v, 256 - v)) by warp reductions,
-//                      the smallest (lowest type on a tie) written as type byte + filtered row into the filtered stream F
+//                      the smallest (lowest type on a tie) written as type byte + filtered row into the filtered stream F;
+//                      4-byte pixels (RGBA8) or 8-byte pixels (RGBA16, samples swapped to big-endian)
 //   pe_k_png_deflate   one CTA per kPngSegment bytes of F: the segment and the 32 KiB before it in shared memory, hash chains
 //                      of that window built by one warp (__match_any_sync resolves the positions of one step), then the
 //                      greedy parse by the same warp -- the chain candidates of a token compared 32 bytes per step -- into a
@@ -48,17 +50,25 @@ __device__ __forceinline__ unsigned filtered(int ft, int x, int a, int b, int c)
     return unsigned(x - pred) & 0xFFu;
 }
 
+// A pixel of BPP bytes: RGBA8 (4) or RGBA16 (8, host byte order), loaded as one word.  Byte k of the pixel in the file is
+// byte k of the word for RGBA8; for RGBA16 the samples are big-endian in the file, so it is byte k ^ 1.
+template <int BPP> struct PngPixel;
+template <> struct PngPixel<4> { using T = uint32_t; static constexpr int kSwap = 0; };
+template <> struct PngPixel<8> { using T = unsigned long long; static constexpr int kSwap = 1; };
+
+template <int BPP>
 __global__ void __launch_bounds__(256) pe_k_png_filter(const uint8_t* __restrict__ rgba, uint8_t* __restrict__ out, int width, int height) {
+    using T = typename PngPixel<BPP>::T;
     const int y = int(blockIdx.x) * 8 + int(threadIdx.x >> 5), lane = int(threadIdx.x & 31);
     if (y >= height) return;
-    const size_t rb = size_t(width) * 4;
-    const uint32_t* cur = reinterpret_cast<const uint32_t*>(rgba + size_t(y) * rb);
-    const uint32_t* up = y ? cur - width : nullptr;
+    const size_t rb = size_t(width) * BPP;
+    const T* cur = reinterpret_cast<const T*>(rgba + size_t(y) * rb);
+    const T* up = y ? cur - width : nullptr;
     uint32_t cost[5] = {0, 0, 0, 0, 0};
     for (int px = lane; px < width; px += kWarp) {
-        const uint32_t x = cur[px], a = px ? cur[px - 1] : 0u, b = up ? up[px] : 0u, c = (up && px) ? up[px - 1] : 0u;
-        for (int k = 0; k < 4; k++) {
-            const int s = 8 * k, xv = int((x >> s) & 0xFF), av = int((a >> s) & 0xFF), bv = int((b >> s) & 0xFF), cv = int((c >> s) & 0xFF);
+        const T x = cur[px], a = px ? cur[px - 1] : T(0), b = up ? up[px] : T(0), c = (up && px) ? up[px - 1] : T(0);
+        for (int k = 0; k < BPP; k++) {
+            const int s = 8 * (k ^ PngPixel<BPP>::kSwap), xv = int((x >> s) & 0xFF), av = int((a >> s) & 0xFF), bv = int((b >> s) & 0xFF), cv = int((c >> s) & 0xFF);
 #pragma unroll
             for (int ft = 0; ft < 5; ft++) {
                 const unsigned v = filtered(ft, xv, av, bv, cv);
@@ -77,10 +87,10 @@ __global__ void __launch_bounds__(256) pe_k_png_filter(const uint8_t* __restrict
     uint8_t* dst = out + size_t(y) * (rb + 1);
     if (lane == 0) dst[0] = uint8_t(best);
     for (int px = lane; px < width; px += kWarp) {
-        const uint32_t x = cur[px], a = px ? cur[px - 1] : 0u, b = up ? up[px] : 0u, c = (up && px) ? up[px - 1] : 0u;
-        for (int k = 0; k < 4; k++) {
-            const int s = 8 * k;
-            dst[1 + 4 * size_t(px) + k] = uint8_t(filtered(best, int((x >> s) & 0xFF), int((a >> s) & 0xFF), int((b >> s) & 0xFF), int((c >> s) & 0xFF)));
+        const T x = cur[px], a = px ? cur[px - 1] : T(0), b = up ? up[px] : T(0), c = (up && px) ? up[px - 1] : T(0);
+        for (int k = 0; k < BPP; k++) {
+            const int s = 8 * (k ^ PngPixel<BPP>::kSwap);
+            dst[1 + BPP * size_t(px) + k] = uint8_t(filtered(best, int((x >> s) & 0xFF), int((a >> s) & 0xFF), int((b >> s) & 0xFF), int((c >> s) & 0xFF)));
         }
     }
 }
@@ -344,9 +354,9 @@ struct Layout {
     size_t n_total, n_seg, filtered, staging, meta, offs, zlen, total;
 };
 
-Layout layout(int width, int height) {
+Layout layout(int width, int height, int bpp) {
     Layout L;
-    L.n_total = size_t(height) * (size_t(width) * 4 + 1);
+    L.n_total = size_t(height) * (size_t(width) * size_t(bpp) + 1);
     L.n_seg = (L.n_total + kPngSegment - 1) / kPngSegment;
     auto up = [](size_t v) { return (v + 255) & ~size_t(255); };
     L.filtered = 0;
@@ -362,18 +372,19 @@ Layout layout(int width, int height) {
 
 namespace pe_host {
 
-size_t png_bound(int width, int height) {
+size_t png_bound(int width, int height, int bpp) {
     if (width < 1 || height < 1) return 0;
-    const size_t n_total = size_t(height) * (size_t(width) * 4 + 1), n_seg = (n_total + kPngSegment - 1) / kPngSegment;
+    const size_t n_total = size_t(height) * (size_t(width) * size_t(bpp) + 1), n_seg = (n_total + kPngSegment - 1) / kPngSegment;
     const size_t z = 2 + n_total + 5 * n_seg + 4;                  // every segment is at most its stored form
     const size_t bound = 33 + z + 12 * ((z + kPngChunk - 1) / kPngChunk) + 12;
     return bound > size_t(INT32_MAX) ? 0 : bound;
 }
 
-size_t png_workspace_bytes(int width, int height) { return layout(width, height).total; }
+size_t png_workspace_bytes(int width, int height, int bpp) { return layout(width, height, bpp).total; }
 
-int launch_png_encode(const void* rgba8, int width, int height, void* work, void* png, void* size_out, cudaStream_t s) {
-    const Layout L = layout(width, height);
+int launch_png_encode(const void* rgba, int width, int height, int bpp, void* work, void* png, void* size_out, cudaStream_t s) {
+    if (bpp != 4 && bpp != 8) return int(cudaErrorInvalidValue);
+    const Layout L = layout(width, height, bpp);
     uint8_t* w = static_cast<uint8_t*>(work);
     uint8_t* filtered = w + L.filtered;
     uint8_t* staging = w + L.staging;
@@ -390,7 +401,7 @@ int launch_png_encode(const void* rgba8, int width, int height, void* work, void
         ihdr[8 + k] = uint8_t(uint32_t(width) >> (24 - 8 * k));
         ihdr[12 + k] = uint8_t(uint32_t(height) >> (24 - 8 * k));
     }
-    ihdr[16] = 8;                                                  // bit depth
+    ihdr[16] = uint8_t(2 * bpp);                                   // bit depth: 8 or 16
     ihdr[17] = 6;                                                  // RGBA
     ihdr[18] = ihdr[19] = ihdr[20] = 0;
     const uint32_t crc = host_crc32(ihdr + 4, 17);
@@ -398,12 +409,12 @@ int launch_png_encode(const void* rgba8, int width, int height, void* work, void
 
     cudaError_t e = cudaFuncSetAttribute(pe_k_png_deflate, cudaFuncAttributeMaxDynamicSharedMemorySize, int(kDeflateSmem));
     if (e != cudaSuccess) return int(e);
-    pe_k_png_filter<<<unsigned((height + 7) / 8), 256, 0, s>>>(static_cast<const uint8_t*>(rgba8), filtered, width, height);
+    (bpp == 4 ? pe_k_png_filter<4> : pe_k_png_filter<8>)<<<unsigned((height + 7) / 8), 256, 0, s>>>(static_cast<const uint8_t*>(rgba), filtered, width, height);
     pe_k_png_deflate<<<unsigned(L.n_seg), kDeflateThreads, kDeflateSmem, s>>>(filtered, L.n_total, staging, meta);
     pe_k_png_scan<<<1, 1024, 0, s>>>(meta, int(L.n_seg), L.n_total, hdr, offs, zlen, static_cast<uint8_t*>(png),
                                      static_cast<unsigned long long*>(size_out));
     pe_k_png_gather<<<unsigned(L.n_seg), 256, 0, s>>>(staging, meta, offs, static_cast<uint8_t*>(png));
-    const size_t max_chunks = (png_bound(width, height) + kPngChunk - 1) / kPngChunk;
+    const size_t max_chunks = (png_bound(width, height, bpp) + kPngChunk - 1) / kPngChunk;
     pe_k_png_chunks<<<unsigned((max_chunks + 127) / 128), 128, 0, s>>>(zlen, static_cast<uint8_t*>(png));
     return int(cudaGetLastError());
 }

@@ -260,6 +260,22 @@ class HostPlayer:
                                                                  motion_blur_frames, float(duration_seconds), out.ctypes.data))
         return out
 
+    def render_frame_rgba16(self, width, height, depth, aa_count=1, aa_start=0) -> np.ndarray:
+        """The frame of render_frame as unorm16 (uint16 [h, w, 4]): the float frame quantised by pe_quantize_rgba16."""
+        p = PhFrameParams(width, height, depth, aa_count, aa_start, 0)
+        out = np.empty((height, width, 4), dtype=np.uint16)
+        self._check(self._lib.ph_player_render_frame_rgba16(self._p, self.renderer._ctx, C.byref(p), out.ctypes.data))
+        return out
+
+    def render_motion_blur_frame_rgba16(self, width, height, depth, frame_index, frame_count, motion_blur_frames, duration_seconds,
+                                        aa_count=1) -> np.ndarray:
+        """render_motion_blur_frame with RGBA16 sub-frames and average (uint16 [h, w, 4])."""
+        p = PhFrameParams(width, height, depth, aa_count, 0, 0)
+        out = np.empty((height, width, 4), dtype=np.uint16)
+        self._check(self._lib.ph_player_render_motion_blur_frame_rgba16(self._p, self.renderer._ctx, C.byref(p), frame_index, frame_count,
+                                                                        motion_blur_frames, float(duration_seconds), out.ctypes.data))
+        return out
+
 
 class HostRenderer:
     """SceneRenderer::new + render_frame over the C API only (no scene IR involved)."""
