@@ -350,6 +350,23 @@ PE_API int pe_encode_png_rgba16(pe_ctx* ctx, const void* rgba16_device, int widt
 PE_API int pe_encode_png_host_rgba16(pe_ctx* ctx, const void* rgba16_device, int width, int height, uint8_t* png_host,
                                      size_t capacity, size_t* size_out);
 
+/* ---- Y'CbCr 4:2:0 at 10 bits (the yuv420p10le the reference's ffmpeg `zscale` step makes from its frames, on the device) ----
+ * DESIGN.md section 5.4, restated in tests/helpers/yuv_spec.py: BT.709 matrix, full range, no change of transfer; exact
+ * rationals rounded once, round(x) = floor(x + 1/2).  Y = round(1023 (2126 R + 7152 G + 722 B) / (10000 M)) at every pixel
+ * (M = 255 or 65535, alpha ignored); Cb, Cr on a ceil(W/2) x ceil(H/2) grid sited as H.265 chroma_sample_loc 0 (co-sited with
+ * luma column 2i, midway between rows 2j and 2j + 1): taps (1, 2, 1) on columns 2i-1 .. 2i+1 times (1, 3, 3, 1) on rows
+ * 2j-1 .. 2j+2, edge-replicated, weights summing to 32; Cb = clamp(round(512 + 1023 Sb / (32 * 18556 M)), 0, 1023) with
+ * Sb = sum w (-2126 R - 7152 G + 9278 B), Cr likewise with 7874 R - 7152 G - 722 B and 15748.  Output: the Y plane (W * H),
+ * then Cb and Cr (ceil(W/2) * ceil(H/2) each), row-major uint16 in host byte order with values in the low 10 bits. */
+/* Bytes of the planes, 2 (W H + 2 ceil(W/2) ceil(H/2)); 0 when width or height is below 1 or the frame has more than
+ * 2^31 - 1 pixels. */
+PE_API size_t pe_yuv420p10_bytes(int width, int height);
+/* The planes of a row-major RGBA8 (`bits` 8, 4-byte aligned) or RGBA16 (`bits` 16, host byte order, 8-byte aligned) frame in
+ * device memory into yuv_device (2-byte aligned, pe_yuv420p10_bytes long).  One kernel launch, asynchronous on `stream` (NULL:
+ * the context's stream); no work space, no scratch slot.  Bad arguments are refused before any launch.  The frame is only read. */
+PE_API int pe_rgba_to_yuv420p10(pe_ctx* ctx, const void* rgba_device, int bits, int width, int height, void* yuv_device,
+                                void* stream);
+
 #ifdef __cplusplus
 }
 #endif

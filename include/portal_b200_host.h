@@ -209,6 +209,18 @@ PE_API int ph_player_render_motion_blur_frame_rgba16(ph_player* pl, pe_ctx* ctx,
 PE_API int ph_player_render_motion_blur_frame_png16(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index,
                                                     int frame_count, int motion_blur_frames, double duration_seconds,
                                                     uint8_t* png, size_t capacity, size_t* len);
+/* Y'CbCr 4:2:0 10-bit twins (DESIGN.md section 5.4): the frame exactly as the RGBA8 twin (`bits` 8: ph_player_render_frame with
+ * rgba8 = 1, ph_player_render_motion_blur_frame) or the RGBA16 twin (`bits` 16) renders it -- adaptive anti-aliasing, stereo and
+ * the update hook included -- converted on the device by pe_rgba_to_yuv420p10; only the planes are read back, into `out_host`
+ * (pe_yuv420p10_bytes(width, height) bytes: Y, then Cb, then Cr).  Scratch slots: the frame is staged in slot 0 as in the
+ * twins (a single RGBA8 frame is always staged there; single RGBA16 frames render their floats into slot 1; motion blur with M
+ * sub-frames keeps them in slots 1 .. M, and at 16 bits renders their floats into slot M + 1).  The planes go into the first
+ * slot after those: 1 (single frame, 8 bits), 2 (single frame, 16 bits), M + 1 (motion blur, 8 bits), M + 2 (motion blur,
+ * 16 bits). */
+PE_API int ph_player_render_frame_yuv420p10(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int bits, uint16_t* out_host);
+PE_API int ph_player_render_motion_blur_frame_yuv420p10(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index,
+                                                        int frame_count, int motion_blur_frames, double duration_seconds, int bits,
+                                                        uint16_t* out_host);
 
 /* ---- image files either side of the path ------------------------------------------------------------------------
  * Textures reach the reference as PNG files (Texture2D::from_file_with_format, src/main.rs:1066-1085) and frames leave it as

@@ -118,6 +118,8 @@ def lib() -> C.CDLL:
         "pe_png_bound_rgba16": (C.c_size_t, [i32, i32]),
         "pe_encode_png_rgba16": (i32, [vp, vp, i32, i32, vp, C.c_size_t, vp, vp]),
         "pe_encode_png_host_rgba16": (i32, [vp, vp, i32, i32, vp, C.c_size_t, C.POINTER(C.c_size_t)]),
+        "pe_yuv420p10_bytes": (C.c_size_t, [i32, i32]),
+        "pe_rgba_to_yuv420p10": (i32, [vp, vp, i32, i32, i32, vp, vp]),
         "pe_shard_target": (i32, [i32, i32, i32, i32, i32, i32, C.POINTER(PeTarget)]),
         "pe_sharder_create": (i32, [vp, cp, i32, i32, i32, i32, i32, i32, i32, C.POINTER(vp)]),
         "pe_sharder_destroy": (None, [vp]),
@@ -193,6 +195,8 @@ def lib() -> C.CDLL:
         "ph_player_render_motion_blur_frame_rgba16": (i32, [vp, vp, C.POINTER(PhFrameParams), i32, i32, i32, C.c_double, vp]),
         "ph_player_render_motion_blur_frame_png16": (i32, [vp, vp, C.POINTER(PhFrameParams), i32, i32, i32, C.c_double, vp, C.c_size_t,
                                                            C.POINTER(C.c_size_t)]),
+        "ph_player_render_frame_yuv420p10": (i32, [vp, vp, C.POINTER(PhFrameParams), i32, vp]),
+        "ph_player_render_motion_blur_frame_yuv420p10": (i32, [vp, vp, C.POINTER(PhFrameParams), i32, i32, i32, C.c_double, i32, vp]),
     })
     for name, (res, args) in sig.items():
         fn = getattr(L, name)
@@ -242,3 +246,36 @@ def encode_png16_device(ctx, rgba16) -> bytes:
     if L.pe_encode_png_host_rgba16(ctx, C.c_void_p(rgba16.data_ptr()), w, h, out, cap, C.byref(n)):
         raise PortalB200Error(L.pe_last_error(ctx).decode(errors="replace"))
     return bytes(memoryview(out)[:n.value])
+
+
+def yuv420p10_planes(buf, width: int, height: int):
+    """Split the planes pe_rgba_to_yuv420p10 writes (a uint16 array of pe_yuv420p10_bytes / 2 values) into Y [h, w],
+    Cb and Cr [ceil(h/2), ceil(w/2)]."""
+    cw, ch = (width + 1) // 2, (height + 1) // 2
+    n = width * height
+    return (buf[:n].reshape(height, width), buf[n:n + cw * ch].reshape(ch, cw), buf[n + cw * ch:n + 2 * cw * ch].reshape(ch, cw))
+
+
+def yuv420p10_device(ctx, rgba, bits: int):
+    """Y'CbCr 4:2:0 10-bit planes (DESIGN.md section 5.4) of a CUDA uint8 (`bits` 8) or uint16 (`bits` 16) tensor [h, w, 4]
+    (contiguous), converted on the device by pe_rgba_to_yuv420p10 on context `ctx`, ordered after the work already queued on
+    the current torch stream.  Returns (Y, Cb, Cr) as numpy uint16 arrays."""
+    import numpy as np
+    import torch
+    want = {8: torch.uint8, 16: torch.uint16}.get(bits)
+    if want is None:
+        raise ValueError("bits must be 8 or 16")
+    if rgba.dim() != 3 or rgba.shape[2] != 4 or not rgba.is_cuda or rgba.dtype != want or not rgba.is_contiguous():
+        raise ValueError(f"frame must be a contiguous CUDA {want} tensor [h, w, 4]")
+    L = lib()
+    h, w = int(rgba.shape[0]), int(rgba.shape[1])
+    nbytes = L.pe_yuv420p10_bytes(w, h)
+    if nbytes == 0:
+        raise PortalB200Error(f"pe_yuv420p10_bytes: no planes for a {w} x {h} frame")
+    out = torch.empty(nbytes // 2, dtype=torch.int16, device=rgba.device)
+    stream = C.c_void_p(torch.cuda.current_stream(rgba.device).cuda_stream)
+    host = np.empty(nbytes // 2, np.uint16)
+    if (L.pe_rgba_to_yuv420p10(ctx, C.c_void_p(rgba.data_ptr()), bits, w, h, C.c_void_p(out.data_ptr()), stream)
+            or L.pe_memcpy_d2h(ctx, host.ctypes.data, C.c_void_p(out.data_ptr()), nbytes, stream)):
+        raise PortalB200Error(L.pe_last_error(ctx).decode(errors="replace"))
+    return yuv420p10_planes(host, w, h)

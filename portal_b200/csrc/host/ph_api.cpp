@@ -590,13 +590,19 @@ int ph_player_render_frame(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p,
     return 0;
 }
 
-int ph_player_render_frame_png(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, uint8_t* png, size_t capacity, size_t* len) {
-    if (!pl || !ctx || !p || !png || !len) return 1;
+// The frame as RGBA8 in scratch slot 0 (*out8).
+static int render_player_rgba8(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, void** out8) {
     if (upload_player_uniforms(pl, ctx, p)) return 1;
     pe_target t = {p->width, p->height, p->height, 0, 1, 1, 1};
-    void* dev = nullptr;
-    if (pe_scratch_buffer(ctx, 0, size_t(p->width) * size_t(p->height) * 4, &dev) || render_player_device(pl, ctx, &t, 1, dev))
+    if (pe_scratch_buffer(ctx, 0, size_t(p->width) * size_t(p->height) * 4, out8) || render_player_device(pl, ctx, &t, 1, *out8))
         return pfail(pl, std::string("render failed: ") + pe_last_error(ctx));
+    return 0;
+}
+
+int ph_player_render_frame_png(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, uint8_t* png, size_t capacity, size_t* len) {
+    if (!pl || !ctx || !p || !png || !len) return 1;
+    void* dev = nullptr;
+    if (render_player_rgba8(pl, ctx, p, &dev)) return 1;
     if (pe_encode_png_host(ctx, dev, p->width, p->height, png, capacity, len)) return pfail(pl, std::string("PNG encoding failed: ") + pe_last_error(ctx));
     return 0;
 }
@@ -708,6 +714,33 @@ int ph_player_render_motion_blur_frame_png16(ph_player* pl, pe_ctx* ctx, const p
     if (motion_blur_device(pl, ctx, p, frame_index, frame_count, motion_blur_frames, duration_seconds, 16, &out16)) return 1;
     if (pe_encode_png_host_rgba16(ctx, out16, p->width, p->height, png, capacity, len)) return pfail(pl, std::string("PNG encoding failed: ") + pe_last_error(ctx));
     return 0;
+}
+
+// A frame already on the device (RGBA8 or RGBA16 per `bits`) -> its Y'CbCr 4:2:0 planes in scratch slot `slot` -> out_host.
+static int read_back_yuv420p10(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int bits, const void* frame, int slot, uint16_t* out_host) {
+    const size_t bytes = pe_yuv420p10_bytes(p->width, p->height);
+    void* yuv = nullptr;
+    if (!bytes || pe_scratch_buffer(ctx, slot, bytes, &yuv) || pe_rgba_to_yuv420p10(ctx, frame, bits, p->width, p->height, yuv, nullptr) ||
+        pe_memcpy_d2h(ctx, out_host, yuv, bytes, nullptr))
+        return pfail(pl, std::string("Y'CbCr conversion failed: ") + (bytes ? pe_last_error(ctx) : "invalid frame size"));
+    return 0;
+}
+
+int ph_player_render_frame_yuv420p10(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int bits, uint16_t* out_host) {
+    if (!pl || !ctx || !p || !out_host) return 1;
+    if (bits != 8 && bits != 16) return pfail(pl, "ph_player_render_frame_yuv420p10: bits must be 8 or 16");
+    void* dev = nullptr;
+    if (bits == 16 ? render_player_rgba16(pl, ctx, p, &dev) : render_player_rgba8(pl, ctx, p, &dev)) return 1;
+    return read_back_yuv420p10(pl, ctx, p, bits, dev, bits == 16 ? 2 : 1, out_host);
+}
+
+int ph_player_render_motion_blur_frame_yuv420p10(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index, int frame_count,
+                                                 int motion_blur_frames, double duration_seconds, int bits, uint16_t* out_host) {
+    if (!pl || !ctx || !p || !out_host) return 1;
+    if (bits != 8 && bits != 16) return pfail(pl, "ph_player_render_motion_blur_frame_yuv420p10: bits must be 8 or 16");
+    void* dev = nullptr;
+    if (motion_blur_device(pl, ctx, p, frame_index, frame_count, motion_blur_frames, duration_seconds, bits, &dev)) return 1;
+    return read_back_yuv420p10(pl, ctx, p, bits, dev, motion_blur_frames + (bits == 16 ? 2 : 1), out_host);
 }
 
 // ---- image files (ph_png.cpp)

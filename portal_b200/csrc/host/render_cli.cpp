@@ -4,13 +4,13 @@
 //   portal_b200_render render-frame <scene.ron> [--width W] [--height H] [--render-depth D] [--aa-count N]
 //                      [--time T] [--stage NAME] [--animation NAME] [--camera NAME] [--device K]
 //                      [--texture name=file.png | name=file.rgba:WxH ...] [--assets DIR] [--output out.png|.ppm|.rgba]
-//                      [--adaptive-aa T] [--bit-depth 8|16]
+//                      [--adaptive-aa T] [--bit-depth 8|16]                              (also --output out.y4m)
 //   portal_b200_render render <scene.ron> [--animations a,b,... | --starts-with PREFIX] [--fps N] [--motion-blur-frames M] [--width W]
 //                      [--height H] [--render-depth D] [--aa-count N] [--stereo-image] [--no-skip-existing] [--out-dir DIR] [--max-frames K]
-//                      [--frame-format ppm|png|rgba] [--assets DIR] [--adaptive-aa T] [--bit-depth 8|16]
+//                      [--frame-format ppm|png|rgba|y4m] [--assets DIR] [--adaptive-aa T] [--bit-depth 8|16]
 //                      (`portal render`, main.rs:2808-2873 -> render_named_animations :1876-1930 ->
-//                       render_animation :1757-1830; frames are written as DIR/<animation>/frame_<i>.<format>, the
-//                       ffmpeg step is out of scope)
+//                       render_animation :1757-1830; frames are written as DIR/<animation>/frame_<i>.<format>, or as one
+//                       Y4M stream DIR/<animation>.y4m; the HEVC encode itself is out of scope)
 //
 // --adaptive-aa T (not in the reference; off by default): every frame / sub-frame is traced with one sample, and with all
 // --aa-count samples only where that frame has an edge (a 3x3 unorm8 range above T, pe_render_adaptive).
@@ -19,6 +19,14 @@
 // sub-frame is rendered as floats and quantised to unorm16 (motion blur averages the RGBA16 sub-frames), then written as a
 // 16-bit PNG (encoded on the device: ph_player_render_frame_png16, pe_encode_png_rgba16), as raw little-endian RGBA16 for
 // .rgba, or as a P6 PPM with maxval 65535 (big-endian samples, alpha dropped).
+//
+// --frame-format y4m / --output *.y4m (not in the reference, whose ffmpeg step does this conversion): the frames the other
+// formats would write (RGBA8, or RGBA16 with --bit-depth 16) converted on the device to Y'CbCr 4:2:0 at 10 bits, BT.709, full
+// range (ph_player_render_*_yuv420p10, pe_rgba_to_yuv420p10; DESIGN.md section 5.4), written as a YUV4MPEG2 stream of
+// yuv420p10le frames -- the raw input ffmpeg and x265 read from a file or a pipe.  `render` writes one stream per animation,
+// DIR/<animation>.y4m at --fps, and skips an animation whose stream exists (as the reference skips an existing .mov,
+// main.rs:1771-1779); --out-dir - writes the stream of the one selected animation to stdout, with every status line on
+// stderr.  render-frame writes a one-frame stream at 25 fps.
 //
 // Output: the RGBA8 frame the reference hands to export_png (main.rs:2939-2943) as a PNG when the name ends in .png (encoded
 // on the device: ph_player_render_frame_png / ph_player_render_motion_blur_frame_png, pe_encode_png_rgba8), as raw RGBA8 for
@@ -55,6 +63,17 @@ static std::string slurp(const std::string& path, bool& ok) {
 static bool ends_with(const std::string& s, const char* suffix) {
     const size_t n = std::strlen(suffix);
     return s.size() >= n && s.compare(s.size() - n, n, suffix) == 0;
+}
+
+// YUV4MPEG2 (the raw input ffmpeg and x265 read): the stream header with the tags ffmpeg's own muxer writes for full-range
+// yuv420p10le, then per frame "FRAME\n" and the Y, Cb, Cr planes as little-endian uint16.  Y4M cannot carry the matrix
+// (BT.709): the encode command states it (README.md, DESIGN.md section 5.4).
+static_assert(__BYTE_ORDER__ == __ORDER_LITTLE_ENDIAN__, "the planes are written as read back, in host byte order");
+static bool write_y4m_header(FILE* f, int width, int height, int fps) {
+    return std::fprintf(f, "YUV4MPEG2 W%d H%d F%d:1 Ip A1:1 C420p10 XYSCSS=420P10 XCOLORRANGE=FULL\n", width, height, fps) > 0;
+}
+static bool write_y4m_frame(FILE* f, const std::vector<uint8_t>& planes) {
+    return std::fputs("FRAME\n", f) >= 0 && std::fwrite(planes.data(), 1, planes.size(), f) == planes.size();
 }
 
 static bool write_bytes(const std::string& output, const std::vector<uint8_t>& bytes, size_t n) {
@@ -178,9 +197,9 @@ int main(int argc, char** argv) {
     const bool anim_cmd = argc >= 3 && std::strcmp(argv[1], "render") == 0;
     if (!frame_cmd && !anim_cmd) {
         std::fprintf(stderr, "usage: %s render-frame <scene.ron> [--width W] [--height H] [--render-depth D] [--aa-count N] [--time T] "
-                             "[--stage NAME] [--animation NAME] [--camera NAME] [--device K] [--texture name=file.png|name=file.rgba:WxH] [--assets DIR] [--output out.png|.ppm|.rgba] [--adaptive-aa T] [--bit-depth 8|16]\n"
+                             "[--stage NAME] [--animation NAME] [--camera NAME] [--device K] [--texture name=file.png|name=file.rgba:WxH] [--assets DIR] [--output out.png|.ppm|.rgba|.y4m] [--adaptive-aa T] [--bit-depth 8|16]\n"
                              "       %s render <scene.ron> [a,b | --animations a,b | --starts-with PREFIX] [--fps N] [--motion-blur-frames M] [--width W] [--height H] "
-                             "[--render-depth D] [--aa-count N] [--stereo-image] [--no-skip-existing] [--out-dir DIR] [--max-frames K] [--frame-format ppm|png|rgba] [--adaptive-aa T] [--bit-depth 8|16]\n", argv[0], argv[0]);
+                             "[--render-depth D] [--aa-count N] [--stereo-image] [--no-skip-existing] [--out-dir DIR] [--max-frames K] [--frame-format ppm|png|rgba|y4m] [--adaptive-aa T] [--bit-depth 8|16]\n", argv[0], argv[0]);
         return 2;
     }
     std::string scene_path = argv[2], output = "frame.ppm", out_dir = "video";
@@ -217,7 +236,7 @@ int main(int argc, char** argv) {
         else if (a == "--output") output = next();
         else if (a == "--texture") textures.push_back(next());
         else if (a == "--assets") assets = next();
-        else if (a == "--frame-format") frame_ext = std::string(".") + next();          // render: ppm (default) | png | rgba
+        else if (a == "--frame-format") frame_ext = std::string(".") + next();          // render: ppm (default) | png | rgba | y4m
         else if (a == "--adaptive-aa" || a == "--adaptive_aa") {
             const char* v = next();
             char* end = nullptr;
@@ -239,6 +258,30 @@ int main(int argc, char** argv) {
     char err[2048] = {0};
     ph_scene* scene = ph_scene_load_ron(text.data(), text.size(), err, sizeof err);
     if (!scene) { std::fprintf(stderr, "Failed to parse scene `%s`: %s\n", scene_path.c_str(), err); return 1; }
+    // render: --animations a,b -> render_named_animations (main.rs:1876-1930); otherwise render_all_animations (:1932-1974): every
+    // animation in file order is initialised and updated once, and rendered unless --starts-with filters it out
+    std::vector<std::string> names;
+    const bool all = animations.empty();
+    size_t selected = 0;
+    if (anim_cmd) {
+        if (all) {
+            for (int a = 0; a < ph_scene_animation_count(scene); a++) {
+                const char* nm = nullptr;
+                if (ph_scene_animation(scene, a, &nm, nullptr) == 0) names.push_back(nm);
+            }
+        } else {
+            std::stringstream ss(animations);
+            for (std::string item; std::getline(ss, item, ',');) if (!item.empty()) names.push_back(item);
+        }
+        for (const std::string& nm : names) selected += !all || starts_with.empty() || nm.compare(0, starts_with.size(), starts_with) == 0;
+    }
+    const bool y4m = frame_cmd ? ends_with(output, ".y4m") : frame_ext == ".y4m";
+    const bool to_stdout = anim_cmd && y4m && out_dir == "-";
+    if (to_stdout && selected != 1) {
+        std::fprintf(stderr, "--out-dir - writes one Y4M stream to stdout: select exactly one animation (%zu selected)\n", selected);
+        return 2;
+    }
+    FILE* status = to_stdout ? stderr : stdout;     // stdout carries the stream
     pe_ctx* ctx = pe_create(device);
     if (!ctx) { std::fprintf(stderr, "pe_create: %s\n", pe_last_error(nullptr)); return 1; }
     ph_player* player = ph_player_new(scene);
@@ -309,10 +352,11 @@ int main(int argc, char** argv) {
         ph_player_set_stereo(player, 1, 0.07, 0);
     }
     const bool png = frame_cmd ? ends_with(output, ".png") : frame_ext == ".png";       // Image::export_png (main.rs:2939-2943)
-    // one buffer for the frame: RGBA8 / RGBA16 pixels, or a PNG file of at most pe_png_bound(_rgba16) bytes
+    // one buffer for the frame: RGBA8 / RGBA16 pixels, a PNG file of at most pe_png_bound(_rgba16) bytes, or Y'CbCr planes
     const bool b16 = bits == 16;
-    std::vector<uint8_t> px(png ? (b16 ? pe_png_bound_rgba16(width, height) : pe_png_bound(width, height)) : size_t(width) * size_t(height) * (b16 ? 8 : 4));
-    if (px.empty()) { std::fprintf(stderr, "no PNG for a %d x %d frame\n", width, height); return 1; }
+    std::vector<uint8_t> px(png ? (b16 ? pe_png_bound_rgba16(width, height) : pe_png_bound(width, height))
+                            : y4m ? pe_yuv420p10_bytes(width, height) : size_t(width) * size_t(height) * (b16 ? 8 : 4));
+    if (px.empty()) { std::fprintf(stderr, "no %s for a %d x %d frame\n", y4m ? "Y4M stream" : "PNG", width, height); return 1; }
     size_t png_len = 0;
     uint16_t* px16 = reinterpret_cast<uint16_t*>(px.data());
     auto write_frame = [&](const std::string& name) {
@@ -322,26 +366,23 @@ int main(int argc, char** argv) {
     if (frame_cmd) {
         if (ph_player_update(player, time) ||                                                          // main.rs:2928-2929
             (png ? (b16 ? ph_player_render_frame_png16 : ph_player_render_frame_png)(player, ctx, &p, px.data(), px.size(), &png_len)
+                 : y4m ? ph_player_render_frame_yuv420p10(player, ctx, &p, bits, px16)
                  : b16 ? ph_player_render_frame_rgba16(player, ctx, &p, px16) : ph_player_render_frame(player, ctx, &p, px.data(), 1))) {
             std::fprintf(stderr, "%s\n", ph_player_last_error(player));
             return 1;
         }
-        if (!write_frame(output)) { std::fprintf(stderr, "cannot write %s\n", output.c_str()); return 1; }
-        std::printf("Rendered `%s` to `%s`\n", scene_path.c_str(), output.c_str());
-    } else {
-        // --animations a,b: render_named_animations (main.rs:1876-1930); otherwise render_all_animations (:1932-1974): every
-        // animation in file order is initialised and updated once, and rendered unless --starts-with filters it out
-        std::vector<std::string> names;
-        const bool all = animations.empty();
-        if (all) {
-            for (int a = 0; a < ph_scene_animation_count(scene); a++) {
-                const char* nm = nullptr;
-                if (ph_scene_animation(scene, a, &nm, nullptr) == 0) names.push_back(nm);
+        bool written = false;
+        if (y4m) {
+            if (FILE* f = std::fopen(output.c_str(), "wb")) {
+                written = write_y4m_header(f, width, height, 25) && write_y4m_frame(f, px);
+                written = std::fclose(f) == 0 && written;
             }
         } else {
-            std::stringstream ss(animations);
-            for (std::string item; std::getline(ss, item, ',');) if (!item.empty()) names.push_back(item);
+            written = write_frame(output);
         }
+        if (!written) { std::fprintf(stderr, "cannot write %s\n", output.c_str()); return 1; }
+        std::printf("Rendered `%s` to `%s`\n", scene_path.c_str(), output.c_str());
+    } else {
         for (size_t k = 0; k < names.size(); k++) {
             if (ph_player_init_animation(player, names[k].c_str())) {
                 std::fprintf(stderr, "Scene `%s` has no animation named `%s`\n", scene_path.c_str(), names[k].c_str());
@@ -355,13 +396,41 @@ int main(int argc, char** argv) {
                 if (ph_scene_animation(scene, a, &nm, &d) == 0 && names[k] == nm) duration = d;
             }
             if (all && !starts_with.empty() && names[k].compare(0, starts_with.size(), starts_with) != 0) continue;
-            std::printf("Rendering animation %s, %zu/%zu\n", names[k].c_str(), k + 1, names.size());
-            const std::string dir = out_dir + "/" + names[k];
-            if (!make_dirs(dir)) { std::fprintf(stderr, "cannot create %s\n", dir.c_str()); return 1; }
+            std::fprintf(status, "Rendering animation %s, %zu/%zu\n", names[k].c_str(), k + 1, names.size());
             const float duration32 = float(duration);                                          // render_animation takes f32
             int count = int(duration32 * float(fps));                                           // main.rs:1785
             if (count < 1) count = 1;
             const int todo = max_frames >= 0 && max_frames < count ? max_frames : count;
+            if (y4m) {
+                // one stream per animation, written under a temporary name and renamed when complete, so that an interrupted
+                // run leaves no stream for skip-existing to take as done
+                const std::string stream = out_dir + "/" + names[k] + ".y4m", part = stream + ".part";
+                if (!to_stdout && skip_existing && file_exists(stream)) {               // main.rs:1771-1779
+                    std::fprintf(status, "Skip `%s`, because it's already exists\n", names[k].c_str());
+                    continue;
+                }
+                if (!to_stdout && !make_dirs(out_dir)) { std::fprintf(stderr, "cannot create %s\n", out_dir.c_str()); return 1; }
+                FILE* f = to_stdout ? stdout : std::fopen(part.c_str(), "wb");
+                bool ok_stream = f && write_y4m_header(f, width, height, fps);
+                for (int i = 0; i < todo && ok_stream; i++) {
+                    if (ph_player_render_motion_blur_frame_yuv420p10(player, ctx, &p, i, count, motion_blur, double(duration32), bits, px16)) {
+                        std::fprintf(stderr, "%s\n", ph_player_last_error(player));
+                        return 1;
+                    }
+                    ok_stream = write_y4m_frame(f, px);
+                    std::fprintf(status, "\r%d/%d done      ", i + 1, count);
+                    std::fflush(status);
+                }
+                if (f) ok_stream = (to_stdout ? std::fflush(f) : std::fclose(f)) == 0 && ok_stream;
+                if (!ok_stream || (!to_stdout && std::rename(part.c_str(), stream.c_str()) != 0)) {
+                    std::fprintf(stderr, "cannot write %s\n", to_stdout ? "the stream to stdout" : stream.c_str());
+                    return 1;
+                }
+                std::fprintf(status, "\n");
+                continue;
+            }
+            const std::string dir = out_dir + "/" + names[k];
+            if (!make_dirs(dir)) { std::fprintf(stderr, "cannot create %s\n", dir.c_str()); return 1; }
             for (int i = 0; i < todo; i++) {
                 if (skip_existing && file_exists(dir + "/frame_" + std::to_string(i) + frame_ext)) continue;   // resumes like main.rs:1789-1793
                 const double dur = double(duration32);

@@ -1266,4 +1266,22 @@ int pe_encode_png_host_rgba16(pe_ctx* c, const void* rgba16, int width, int heig
     return c ? encode_png_host(c, "pe_encode_png_host_rgba16", "pe_encode_png_rgba16", 8, rgba16, width, height, png_host, capacity, size_out) : 1;
 }
 
+// ------------------------------------------------------------------------------ Y'CbCr 4:2:0, 10 bits (pe_yuv.cu)
+size_t pe_yuv420p10_bytes(int width, int height) { return yuv420p10_bytes(width, height); }
+
+int pe_rgba_to_yuv420p10(pe_ctx* c, const void* rgba, int bits, int width, int height, void* yuv, void* stream) {
+    if (!c) return 1;
+    if (!rgba || !yuv) return c->fail("pe_rgba_to_yuv420p10: null argument");
+    if (bits != 8 && bits != 16) return c->fail("pe_rgba_to_yuv420p10: bits must be 8 or 16, got " + std::to_string(bits));
+    if (!yuv420p10_bytes(width, height))
+        return c->fail("pe_rgba_to_yuv420p10: invalid size " + std::to_string(width) + " x " + std::to_string(height) + " (1 <= width, height; at most 2^31 - 1 pixels)");
+    const uintptr_t word = bits == 16 ? 7 : 3;
+    if ((uintptr_t(rgba) & word) || (uintptr_t(yuv) & 1))
+        return c->fail("pe_rgba_to_yuv420p10: the frame must be " + std::to_string(word + 1) + "-byte and the planes 2-byte aligned");
+    if (!bind_device(c)) return 1;
+    if (!cuda_ok(c, (cudaError_t)launch_rgba_to_yuv420p10(rgba, bits, width, height, yuv, stream_of(c, stream)), "pe_rgba_to_yuv420p10")) return 1;
+    c->launches++;
+    return 0;
+}
+
 }  // extern "C"

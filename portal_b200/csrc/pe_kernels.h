@@ -38,4 +38,11 @@ size_t png_workspace_bytes(int width, int height, int bpp);
 // Enqueue the five kernels: frame -> PNG file at `png` (capacity >= png_bound), its length in *(uint64*)size_out.
 int launch_png_encode(const void* rgba, int width, int height, int bpp, void* work, void* png, void* size_out, cudaStream_t s);
 
+// RGB -> Y'CbCr 4:2:0 at 10 bits (pe_yuv.cu; DESIGN.md section 5.4).  Bytes of the Y, Cb, Cr planes of a width x height frame,
+// 0 when the size is invalid or the frame has more than 2^31 - 1 pixels.
+size_t yuv420p10_bytes(int width, int height);
+// One kernel launch: RGBA8 (`bits` 8, 4-byte aligned) or RGBA16 (`bits` 16, 8-byte aligned) frame -> the planes at `yuv`
+// (2-byte aligned, yuv420p10_bytes long).
+int launch_rgba_to_yuv420p10(const void* rgba, int bits, int width, int height, void* yuv, cudaStream_t s);
+
 }  // namespace pe_host

@@ -276,6 +276,24 @@ class HostPlayer:
                                                                         motion_blur_frames, float(duration_seconds), out.ctypes.data))
         return out
 
+    def render_frame_yuv420p10(self, width, height, depth, bits=8, aa_count=1, aa_start=0):
+        """The frame of render_frame (rgba8=True; `bits` 8) or of render_frame_rgba16 (`bits` 16) as Y'CbCr 4:2:0 at 10 bits,
+        converted on the device (DESIGN.md section 5.4): (Y, Cb, Cr), numpy uint16 arrays."""
+        p = PhFrameParams(width, height, depth, aa_count, aa_start, 0)
+        out = np.empty(self._lib.pe_yuv420p10_bytes(width, height) // 2, dtype=np.uint16)
+        self._check(self._lib.ph_player_render_frame_yuv420p10(self._p, self.renderer._ctx, C.byref(p), int(bits), out.ctypes.data))
+        return capi.yuv420p10_planes(out, width, height)
+
+    def render_motion_blur_frame_yuv420p10(self, width, height, depth, frame_index, frame_count, motion_blur_frames, duration_seconds,
+                                           bits=8, aa_count=1):
+        """render_motion_blur_frame (`bits` 8) or render_motion_blur_frame_rgba16 (`bits` 16) as Y'CbCr 4:2:0 planes."""
+        p = PhFrameParams(width, height, depth, aa_count, 0, 0)
+        out = np.empty(self._lib.pe_yuv420p10_bytes(width, height) // 2, dtype=np.uint16)
+        self._check(self._lib.ph_player_render_motion_blur_frame_yuv420p10(self._p, self.renderer._ctx, C.byref(p), frame_index, frame_count,
+                                                                           motion_blur_frames, float(duration_seconds), int(bits),
+                                                                           out.ctypes.data))
+        return capi.yuv420p10_planes(out, width, height)
+
 
 class HostRenderer:
     """SceneRenderer::new + render_frame over the C API only (no scene IR involved)."""
