@@ -367,6 +367,41 @@ PE_API size_t pe_yuv420p10_bytes(int width, int height);
 PE_API int pe_rgba_to_yuv420p10(pe_ctx* ctx, const void* rgba_device, int bits, int width, int height, void* yuv_device,
                                 void* stream);
 
+/* ---- Y'CbCr 4:2:0 to RGBA8 (video textures from raw 4:2:0 clips, on the device) ----
+ * DESIGN.md section 5.5, restated in tests/helpers/yuv_in_spec.py.  Input: the Y plane (W * H samples), then Cb and Cr
+ * (ceil(W/2) * ceil(H/2) each), row-major; samples are uint8 at 8 bits, or uint16 in host byte order at 10 bits (a word above
+ * 1023 counts as 1023).  Output: RGBA8, row 0 first (as a PNG of the same picture), alpha 255.  Full range: y = Y / (2^b - 1),
+ * c = (C - 2^(b-1)) / (2^b - 1); limited: y = (Y - 16 s) / (219 s), c = (C - 128 s) / (224 s), s = 2^(b-8).  Chroma at each
+ * luma pixel is bilinear at the siting with edges replicated: rows 2j, 2j + 1 take (3 C_j + C_{j-1}) / 4, (3 C_j + C_{j+1}) / 4;
+ * left siting (MPEG-2 / H.265 chroma_sample_loc 0) takes C_i at column 2i and (C_i + C_{i+1}) / 2 at 2i + 1; centre siting
+ * (JPEG, loc 1) takes (3 C_i + C_{i-1}) / 4 and (3 C_i + C_{i+1}) / 4.  R = y + 2 (1 - Kr) cr, B = y + 2 (1 - Kb) cb,
+ * G = (y - Kr R - Kb B) / Kg; each channel is clamp(round(255 x), 0, 255), round(x) = floor(x + 1/2), in exact rationals. */
+#define PE_YUV_BT709 0           /* Kr 0.2126, Kb 0.0722 */
+#define PE_YUV_BT601 1           /* Kr 0.299, Kb 0.114 */
+#define PE_YUV_SITING_LEFT 0     /* co-sited with luma column 2i, midway between rows 2j and 2j + 1 */
+#define PE_YUV_SITING_CENTER 1   /* midway in both directions */
+typedef struct pe_yuv_format {
+    int bits;         /* 8 or 10 */
+    int matrix;       /* PE_YUV_BT709 or PE_YUV_BT601 */
+    int full_range;   /* 1 full, 0 limited */
+    int siting;       /* PE_YUV_SITING_LEFT or PE_YUV_SITING_CENTER */
+} pe_yuv_format;
+/* Bytes of the planes, (W H + 2 ceil(W/2) ceil(H/2)) times 1 (`bits` 8) or 2 (`bits` 10); 0 when `bits` is neither, width or
+ * height is below 1 or the frame has more than 2^31 - 1 pixels. */
+PE_API size_t pe_yuv420_bytes(int width, int height, int bits);
+/* The planes at yuv_device (aligned to one sample, pe_yuv420_bytes long) -> RGBA8 at rgba8_device (4-byte aligned, 4 W H bytes).
+ * One kernel launch, asynchronous on `stream` (NULL: the context's stream); no work space, no scratch slot.  Bad arguments
+ * are refused before any launch.  The planes are only read. */
+PE_API int pe_yuv420_to_rgba8(pe_ctx* ctx, const void* yuv_device, const pe_yuv_format* format, int width, int height,
+                              void* rgba8_device, void* stream);
+/* The Y'CbCr twin of pe_set_texture: the planes at yuv_host (pe_yuv420_bytes long; page-locked memory from pe_host_malloc
+ * makes the copy faster) are copied into a device buffer the context owns (grown on demand) and converted on the device into
+ * the texture's image.  As pe_set_texture, it waits for the device before touching an image a queued render may read, never
+ * leaves the sampler pointing at freed memory, and the image is in place when the call returns.  An image of the same size
+ * is converted in place; another size replaces it.  Returns 2 for an unknown texture name. */
+PE_API int pe_set_texture_yuv420(pe_ctx* ctx, const char* name, const void* yuv_host, const pe_yuv_format* format, int width,
+                                 int height);
+
 #ifdef __cplusplus
 }
 #endif

@@ -236,6 +236,23 @@ PE_API void ph_png_free(uint8_t* p);
  * written (0 = the path has no file name). */
 PE_API int ph_video_frames_dir(const char* video_path, char* out, size_t out_len);
 
+/* ---- Y4M clips: raw 4:2:0 frames for pe_set_texture_yuv420 (DESIGN.md section 5.5) ------------------------------
+ * A YUV4MPEG2 stream as `ffmpeg -i clip.mp4 -pix_fmt yuv420p clip.y4m` (or yuv420p10le) writes it.  The colour-space tag gives
+ * the format: C420jpeg, bare C420 or none -> 8 bits, centre siting; C420mpeg2 -> 8 bits, left; C420p10 -> 10 bits, left.
+ * XCOLORRANGE=FULL is full range; LIMITED or no tag is limited.  The matrix (PE_YUV_BT709 / PE_YUV_BT601) is not in the
+ * stream and is the caller's.  Anything else (4:2:2, 4:4:4, mono, C420paldv, other depths) is refused with a message in
+ * `err`.  The frames are indexed once at open by walking the FRAME lines (which may carry parameters), with 64-bit offsets;
+ * a trailing partial frame is not counted and its length is reported by ph_y4m_info.  Frame k is read with one pread, as
+ * the planes pe_set_texture_yuv420 takes (pe_yuv420_bytes long). */
+typedef struct ph_y4m ph_y4m;
+PE_API ph_y4m* ph_y4m_open(const char* path, int matrix, char* err, size_t err_len);
+/* Any output pointer may be NULL. */
+PE_API int ph_y4m_info(const ph_y4m* r, int32_t* width, int32_t* height, int64_t* frame_count, pe_yuv_format* format,
+                       int64_t* partial_bytes);
+PE_API int ph_y4m_read_frame(ph_y4m* r, int64_t k, void* out, size_t len);
+PE_API const char* ph_y4m_last_error(const ph_y4m* r);
+PE_API void ph_y4m_close(ph_y4m* r);
+
 #ifdef __cplusplus
 }
 #endif

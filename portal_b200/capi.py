@@ -31,6 +31,24 @@ class PhFrameParams(C.Structure):
                 ("beta", C.c_double), ("r", C.c_double)]
 
 
+PE_YUV_BT709, PE_YUV_BT601 = 0, 1
+PE_YUV_SITING_LEFT, PE_YUV_SITING_CENTER = 0, 1
+MATRICES = {"bt709": PE_YUV_BT709, "bt601": PE_YUV_BT601}
+
+
+class PeYuvFormat(C.Structure):
+    """pe_yuv_format: bits 8 | 10, matrix PE_YUV_BT709 | PE_YUV_BT601, full_range 0 | 1, siting PE_YUV_SITING_LEFT | CENTER."""
+    _fields_ = [("bits", C.c_int), ("matrix", C.c_int), ("full_range", C.c_int), ("siting", C.c_int)]
+
+    def astuple(self):
+        return (self.bits, self.matrix, self.full_range, self.siting)
+
+
+def yuv_format(fmt) -> PeYuvFormat:
+    """A PeYuvFormat from itself or from a (bits, matrix, full_range, siting) tuple."""
+    return fmt if isinstance(fmt, PeYuvFormat) else PeYuvFormat(*[int(v) for v in fmt])
+
+
 class PortalB200Error(RuntimeError):
     pass
 
@@ -120,6 +138,9 @@ def lib() -> C.CDLL:
         "pe_encode_png_host_rgba16": (i32, [vp, vp, i32, i32, vp, C.c_size_t, C.POINTER(C.c_size_t)]),
         "pe_yuv420p10_bytes": (C.c_size_t, [i32, i32]),
         "pe_rgba_to_yuv420p10": (i32, [vp, vp, i32, i32, i32, vp, vp]),
+        "pe_yuv420_bytes": (C.c_size_t, [i32, i32, i32]),
+        "pe_yuv420_to_rgba8": (i32, [vp, vp, C.POINTER(PeYuvFormat), i32, i32, vp, vp]),
+        "pe_set_texture_yuv420": (i32, [vp, cp, vp, C.POINTER(PeYuvFormat), i32, i32]),
         "pe_shard_target": (i32, [i32, i32, i32, i32, i32, i32, C.POINTER(PeTarget)]),
         "pe_sharder_create": (i32, [vp, cp, i32, i32, i32, i32, i32, i32, i32, C.POINTER(vp)]),
         "pe_sharder_destroy": (None, [vp]),
@@ -196,6 +217,12 @@ def lib() -> C.CDLL:
         "ph_player_render_motion_blur_frame_png16": (i32, [vp, vp, C.POINTER(PhFrameParams), i32, i32, i32, C.c_double, vp, C.c_size_t,
                                                            C.POINTER(C.c_size_t)]),
         "ph_player_render_frame_yuv420p10": (i32, [vp, vp, C.POINTER(PhFrameParams), i32, vp]),
+        "ph_y4m_open": (vp, [cp, i32, cp, C.c_size_t]),
+        "ph_y4m_info": (i32, [vp, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(PeYuvFormat),
+                              C.POINTER(C.c_int64)]),
+        "ph_y4m_read_frame": (i32, [vp, C.c_int64, vp, C.c_size_t]),
+        "ph_y4m_last_error": (cp, [vp]),
+        "ph_y4m_close": (None, [vp]),
         "ph_player_render_motion_blur_frame_yuv420p10": (i32, [vp, vp, C.POINTER(PhFrameParams), i32, i32, i32, C.c_double, i32, vp]),
     })
     for name, (res, args) in sig.items():
@@ -279,3 +306,23 @@ def yuv420p10_device(ctx, rgba, bits: int):
             or L.pe_memcpy_d2h(ctx, host.ctypes.data, C.c_void_p(out.data_ptr()), nbytes, stream)):
         raise PortalB200Error(L.pe_last_error(ctx).decode(errors="replace"))
     return yuv420p10_planes(host, w, h)
+
+
+def yuv420_to_rgba8_device(ctx, yuv, fmt, width: int, height: int):
+    """RGBA8 [h, w, 4] (a CUDA uint8 tensor) of the Y'CbCr 4:2:0 planes in the contiguous CUDA tensor `yuv` (uint8 at 8 bits,
+    uint16 / int16 at 10; pe_yuv420_bytes long), converted on the device by pe_yuv420_to_rgba8 (DESIGN.md section 5.5) on
+    context `ctx`, ordered after the work already queued on the current torch stream.  `fmt`: PeYuvFormat or
+    (bits, matrix, full_range, siting)."""
+    import torch
+    f = yuv_format(fmt)
+    L = lib()
+    nbytes = L.pe_yuv420_bytes(width, height, f.bits)
+    if nbytes == 0:
+        raise PortalB200Error(f"pe_yuv420_bytes: no planes for a {width} x {height} frame at {f.bits} bits")
+    if not yuv.is_cuda or not yuv.is_contiguous() or yuv.numel() * yuv.element_size() < nbytes:
+        raise ValueError(f"planes must be a contiguous CUDA tensor of at least {nbytes} bytes")
+    out = torch.empty((height, width, 4), dtype=torch.uint8, device=yuv.device)
+    stream = C.c_void_p(torch.cuda.current_stream(yuv.device).cuda_stream)
+    if L.pe_yuv420_to_rgba8(ctx, C.c_void_p(yuv.data_ptr()), C.byref(f), width, height, C.c_void_p(out.data_ptr()), stream):
+        raise PortalB200Error(L.pe_last_error(ctx).decode(errors="replace"))
+    return out

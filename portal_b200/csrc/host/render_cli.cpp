@@ -5,9 +5,11 @@
 //                      [--time T] [--stage NAME] [--animation NAME] [--camera NAME] [--device K]
 //                      [--texture name=file.png | name=file.rgba:WxH ...] [--assets DIR] [--output out.png|.ppm|.rgba]
 //                      [--adaptive-aa T] [--bit-depth 8|16]                              (also --output out.y4m)
+//                      [--video name=clip.y4m ...] [--video-matrix bt709|bt601]
 //   portal_b200_render render <scene.ron> [--animations a,b,... | --starts-with PREFIX] [--fps N] [--motion-blur-frames M] [--width W]
 //                      [--height H] [--render-depth D] [--aa-count N] [--stereo-image] [--no-skip-existing] [--out-dir DIR] [--max-frames K]
 //                      [--frame-format ppm|png|rgba|y4m] [--assets DIR] [--adaptive-aa T] [--bit-depth 8|16]
+//                      [--video name=clip.y4m ...] [--video-matrix bt709|bt601]
 //                      (`portal render`, main.rs:2808-2873 -> render_named_animations :1876-1930 ->
 //                       render_animation :1757-1830; frames are written as DIR/<animation>/frame_<i>.<format>, or as one
 //                       Y4M stream DIR/<animation>.y4m; the HEVC encode itself is out of scope)
@@ -35,6 +37,13 @@
 // (main.rs:1066-1085) -- a file that cannot be read is reported and the sampler stays unbound, as there; --texture overrides one
 // by name (PNG, or raw RGBA8 with :WxH).  Videos: the frames of video_png/<stem>/*.png, sorted, the one the video's uniform
 // selects swapped in after every update (VideoRuntime, main.rs:771-930).
+//
+// Y4M clips (not in the reference, which decodes a PNG per frame change): a video's frames may instead come from a YUV4MPEG2
+// stream of raw 4:2:0 frames (`ffmpeg -i clip.mp4 -pix_fmt yuv420p clip.y4m`), read with one pread per frame change and
+// converted to the RGBA8 image on the device (ph_y4m_*, pe_set_texture_yuv420; DESIGN.md section 5.5).  Each video's source,
+// in order: --video name=clip.y4m (a clip that cannot be opened, or a name that is not a video of the scene, exits 1 before
+// anything is rendered); the PNG frames of video_png/<stem>/, exactly as above; <assets>/video_y4m/<stem>.y4m.  The matrix is
+// not in the stream: --video-matrix, BT.709 by default.  A status line names each video's source and format.
 #include <dirent.h>
 #include <sys/stat.h>
 #include <sys/types.h>
@@ -132,11 +141,18 @@ static bool set_texture_from_png(pe_ctx* ctx, const std::string& name, const std
     return true;
 }
 
-// VideoRuntime (main.rs:771-930): the sorted PNG frames of one video and the frame last uploaded
+// VideoRuntime (main.rs:771-930): the sorted PNG frames of one video, or its Y4M clip and a page-locked buffer for one of
+// its frames, and the frame last uploaded
 struct VideoRuntime {
     int video = 0;
     std::string name;
     std::vector<std::string> frames;
+    ph_y4m* clip = nullptr;
+    int64_t clip_frames = 0;
+    int32_t clip_w = 0, clip_h = 0;
+    pe_yuv_format format = {8, PE_YUV_BT709, 0, PE_YUV_SITING_LEFT};
+    void* planes = nullptr;
+    size_t planes_bytes = 0;
     long last = -1;
 };
 struct VideoState {
@@ -167,13 +183,46 @@ static int update_videos(void* user) {
     VideoState& st = *static_cast<VideoState*>(user);
     for (VideoRuntime& v : st.videos) {
         uint64_t idx = 0;
-        if (ph_scene_video_frame(st.scene, v.video, v.frames.size(), &idx)) continue;
+        if (ph_scene_video_frame(st.scene, v.video, v.clip ? uint64_t(v.clip_frames) : v.frames.size(), &idx)) continue;
         if (long(idx) == v.last) continue;                     // avoid a reload when the frame did not change
-        std::string why;
-        if (!set_texture_from_png(st.ctx, v.name, v.frames[size_t(idx)], why)) continue;   // IO errors are ignored there too: the texture just does not update
+        if (v.clip) {
+            if (ph_y4m_read_frame(v.clip, int64_t(idx), v.planes, v.planes_bytes) ||
+                pe_set_texture_yuv420(st.ctx, v.name.c_str(), v.planes, &v.format, v.clip_w, v.clip_h)) continue;   // as below
+        } else {
+            std::string why;
+            if (!set_texture_from_png(st.ctx, v.name, v.frames[size_t(idx)], why)) continue;   // IO errors are ignored there too: the texture just does not update
+        }
         v.last = long(idx);
     }
     return 0;
+}
+
+// "<path>: WxH, N frames, 8-bit 4:2:0, BT.709, limited range, left siting" for the status line
+static std::string clip_description(const std::string& path, const VideoRuntime& v) {
+    return path + ": " + std::to_string(v.clip_w) + "x" + std::to_string(v.clip_h) + ", " + std::to_string(v.clip_frames) + " frames, " +
+           std::to_string(v.format.bits) + "-bit 4:2:0, " + (v.format.matrix == PE_YUV_BT601 ? "BT.601, " : "BT.709, ") +
+           (v.format.full_range ? "full range, " : "limited range, ") + (v.format.siting == PE_YUV_SITING_CENTER ? "centre siting" : "left siting");
+}
+
+// Opens a Y4M clip for video `v`; false with a message in `why` when it cannot be used.
+static bool open_clip(VideoRuntime& v, const std::string& path, int matrix, std::string& why) {
+    char err[1024] = {0};
+    v.clip = ph_y4m_open(path.c_str(), matrix, err, sizeof err);
+    if (!v.clip) { why = err; return false; }
+    int64_t partial = 0;
+    ph_y4m_info(v.clip, &v.clip_w, &v.clip_h, &v.clip_frames, &v.format, &partial);
+    if (v.clip_frames < 1) { why = path + ": no complete frame"; ph_y4m_close(v.clip); v.clip = nullptr; return false; }
+    if (partial) std::fprintf(stderr, "%s: a trailing partial frame of %lld bytes is ignored\n", path.c_str(), (long long)partial);
+    v.planes_bytes = pe_yuv420_bytes(v.clip_w, v.clip_h, v.format.bits);
+    return true;
+}
+
+// The file of `--video name=file` for `name`
+static std::string videos_path_of(const std::vector<std::string>& videos, const std::string& name) {
+    std::string path;
+    for (const std::string& g : videos)
+        if (g.compare(0, name.size() + 1, name + "=") == 0) path = g.substr(name.size() + 1);
+    return path;
 }
 
 static bool file_exists(const std::string& path) {
@@ -197,9 +246,9 @@ int main(int argc, char** argv) {
     const bool anim_cmd = argc >= 3 && std::strcmp(argv[1], "render") == 0;
     if (!frame_cmd && !anim_cmd) {
         std::fprintf(stderr, "usage: %s render-frame <scene.ron> [--width W] [--height H] [--render-depth D] [--aa-count N] [--time T] "
-                             "[--stage NAME] [--animation NAME] [--camera NAME] [--device K] [--texture name=file.png|name=file.rgba:WxH] [--assets DIR] [--output out.png|.ppm|.rgba|.y4m] [--adaptive-aa T] [--bit-depth 8|16]\n"
+                             "[--stage NAME] [--animation NAME] [--camera NAME] [--device K] [--texture name=file.png|name=file.rgba:WxH] [--assets DIR] [--output out.png|.ppm|.rgba|.y4m] [--adaptive-aa T] [--bit-depth 8|16] [--video name=clip.y4m] [--video-matrix bt709|bt601]\n"
                              "       %s render <scene.ron> [a,b | --animations a,b | --starts-with PREFIX] [--fps N] [--motion-blur-frames M] [--width W] [--height H] "
-                             "[--render-depth D] [--aa-count N] [--stereo-image] [--no-skip-existing] [--out-dir DIR] [--max-frames K] [--frame-format ppm|png|rgba|y4m] [--adaptive-aa T] [--bit-depth 8|16]\n", argv[0], argv[0]);
+                             "[--render-depth D] [--aa-count N] [--stereo-image] [--no-skip-existing] [--out-dir DIR] [--max-frames K] [--frame-format ppm|png|rgba|y4m] [--adaptive-aa T] [--bit-depth 8|16] [--video name=clip.y4m] [--video-matrix bt709|bt601]\n", argv[0], argv[0]);
         return 2;
     }
     std::string scene_path = argv[2], output = "frame.ppm", out_dir = "video";
@@ -209,7 +258,8 @@ int main(int argc, char** argv) {
     bool stereo = false, skip_existing = true, adaptive = false;
     int adaptive_threshold = 0, bits = 8;
     double time = 0.0;
-    std::vector<std::string> textures;
+    std::vector<std::string> textures, videos;
+    int video_matrix = PE_YUV_BT709;
     std::string stage, animation, camera, animations, starts_with, assets, frame_ext = ".ppm";
     int first_option = 3;
     if (anim_cmd && argc > 3 && std::strncmp(argv[3], "--", 2) != 0) animations = argv[first_option++];   // `render <scene> [animations]`
@@ -235,6 +285,12 @@ int main(int argc, char** argv) {
         else if (a == "--no-skip-existing" || a == "--no_skip_existing") skip_existing = false;
         else if (a == "--output") output = next();
         else if (a == "--texture") textures.push_back(next());
+        else if (a == "--video") videos.push_back(next());
+        else if (a == "--video-matrix" || a == "--video_matrix") {
+            const std::string v = next();
+            if (v != "bt709" && v != "bt601") { std::fprintf(stderr, "--video-matrix must be bt709 or bt601, got `%s`\n", v.c_str()); return 2; }
+            video_matrix = v == "bt601" ? PE_YUV_BT601 : PE_YUV_BT709;
+        }
         else if (a == "--assets") assets = next();
         else if (a == "--frame-format") frame_ext = std::string(".") + next();          // render: ppm (default) | png | rgba | y4m
         else if (a == "--adaptive-aa" || a == "--adaptive_aa") {
@@ -282,6 +338,21 @@ int main(int argc, char** argv) {
         return 2;
     }
     FILE* status = to_stdout ? stderr : stdout;     // stdout carries the stream
+    // --video name=clip.y4m: every clip is opened (and refused) before a context exists
+    std::map<std::string, VideoRuntime> given_clips;
+    for (const std::string& g : videos) {
+        const size_t eq = g.find('=');
+        const std::string name = eq == std::string::npos ? std::string() : g.substr(0, eq), path = eq == std::string::npos ? g : g.substr(eq + 1);
+        bool known = false;
+        for (int k = 0;; k++) {
+            const char *nm = nullptr, *vp = nullptr, *un = nullptr;
+            if (ph_scene_video(scene, k, &nm, &vp, &un)) break;
+            known = known || name == nm;
+        }
+        if (!known) { std::fprintf(stderr, "--video %s: the scene has no video named `%s`\n", g.c_str(), name.c_str()); return 1; }
+        std::string why;
+        if (!open_clip(given_clips[name], path, video_matrix, why)) { std::fprintf(stderr, "--video %s: %s\n", g.c_str(), why.c_str()); return 1; }
+    }
     pe_ctx* ctx = pe_create(device);
     if (!ctx) { std::fprintf(stderr, "pe_create: %s\n", pe_last_error(nullptr)); return 1; }
     ph_player* player = ph_player_new(scene);
@@ -341,11 +412,31 @@ int main(int argc, char** argv) {
         if (ph_scene_video(scene, k, &name, &path, &uniform)) break;
         if (!path[0] || !uniform[0]) continue;
         VideoRuntime v;
+        std::string source;
+        auto it = given_clips.find(name);
+        if (it != given_clips.end()) {                                   // --video
+            v = it->second;
+            given_clips.erase(it);
+            source = clip_description(videos_path_of(videos, name), v);
+        } else if (!(v.frames = video_frame_files(assets, path)).empty()) {   // video_png/<stem>/
+            source = std::to_string(v.frames.size()) + " PNG frames in " + v.frames[0].substr(0, v.frames[0].rfind('/'));
+        } else {                                                         // <assets>/video_y4m/<stem>.y4m
+            char rel[1024];
+            const int n = ph_video_frames_dir(path, rel, sizeof rel);
+            const std::string stem = n > 0 ? std::string(rel).substr(std::string(rel).find('/') + 1) : std::string();
+            const std::string clip = (assets.empty() ? std::string() : assets + "/") + "video_y4m/" + stem + ".y4m";
+            std::string why;
+            if (stem.empty() || !file_exists(clip)) continue;
+            if (!open_clip(v, clip, video_matrix, why)) { std::fprintf(stderr, "video `%s`: %s (the sampler is not updated)\n", name, why.c_str()); continue; }
+            source = clip_description(clip, v);
+        }
         v.video = k;
         v.name = name;
-        v.frames = video_frame_files(assets, path);
-        if (!v.frames.empty()) video_state.videos.push_back(v);
+        if (v.clip && pe_host_malloc(ctx, v.planes_bytes, &v.planes)) { std::fprintf(stderr, "%s\n", pe_last_error(ctx)); return 1; }
+        std::fprintf(status, "video `%s`: %s\n", name, source.c_str());
+        video_state.videos.push_back(v);
     }
+    for (auto& kv : given_clips) ph_y4m_close(kv.second.clip);       // a video without a path or a uniform plays nothing
     if (!video_state.videos.empty()) ph_player_set_update_hook(player, update_videos, &video_state);
     if (stereo) {                   // `render --stereo-image`: side-by-side eyes, doubled width (main.rs:2809-2816, 2842)
         width *= 2;
@@ -447,6 +538,10 @@ int main(int argc, char** argv) {
             }
             std::printf("\n");
         }
+    }
+    for (VideoRuntime& v : video_state.videos) {
+        if (v.planes) pe_host_free(ctx, v.planes);
+        ph_y4m_close(v.clip);
     }
     ph_player_free(player);
     pe_destroy(ctx);

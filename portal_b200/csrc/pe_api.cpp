@@ -1284,4 +1284,78 @@ int pe_rgba_to_yuv420p10(pe_ctx* c, const void* rgba, int bits, int width, int h
     return 0;
 }
 
+// ------------------------------------------------------------------------------ Y'CbCr 4:2:0 -> RGBA8 (pe_yuv.cu)
+size_t pe_yuv420_bytes(int width, int height, int bits) { return yuv420_bytes(width, height, bits); }
+
+}  // extern "C"
+
+namespace {
+
+// The format and the size of a conversion, checked before anything is copied or launched.
+bool check_yuv420(pe_ctx* c, const std::string& fn, const pe_yuv_format* f, int width, int height) {
+    if (!f) return !c->fail(fn + ": null format");
+    if (f->bits != 8 && f->bits != 10) return !c->fail(fn + ": bits must be 8 or 10, got " + std::to_string(f->bits));
+    if (f->matrix != PE_YUV_BT709 && f->matrix != PE_YUV_BT601) return !c->fail(fn + ": matrix must be PE_YUV_BT709 or PE_YUV_BT601");
+    if (f->full_range != 0 && f->full_range != 1) return !c->fail(fn + ": full_range must be 0 or 1");
+    if (f->siting != PE_YUV_SITING_LEFT && f->siting != PE_YUV_SITING_CENTER)
+        return !c->fail(fn + ": siting must be PE_YUV_SITING_LEFT or PE_YUV_SITING_CENTER");
+    if (!yuv420_bytes(width, height, f->bits))
+        return !c->fail(fn + ": invalid size " + std::to_string(width) + " x " + std::to_string(height) + " (1 <= width, height; at most 2^31 - 1 pixels)");
+    return true;
+}
+
+int yuv420_launch(pe_ctx* c, const void* yuv, const pe_yuv_format* f, int width, int height, void* rgba, cudaStream_t s, const char* fn) {
+    if (!cuda_ok(c, (cudaError_t)launch_yuv420_to_rgba8(yuv, f->bits, f->matrix, f->full_range, f->siting, width, height, rgba, s), fn)) return 1;
+    c->launches++;
+    return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int pe_yuv420_to_rgba8(pe_ctx* c, const void* yuv, const pe_yuv_format* format, int width, int height, void* rgba8, void* stream) {
+    if (!c) return 1;
+    const std::string fn = "pe_yuv420_to_rgba8";
+    if (!yuv || !rgba8) return c->fail(fn + ": null argument");
+    if (!check_yuv420(c, fn, format, width, height)) return 1;
+    if ((uintptr_t(yuv) & uintptr_t(format->bits == 10 ? 1 : 0)) || (uintptr_t(rgba8) & 3))
+        return c->fail(fn + ": the planes must be " + std::string(format->bits == 10 ? "2" : "1") + "-byte and the image 4-byte aligned");
+    if (!bind_device(c)) return 1;
+    return yuv420_launch(c, yuv, format, width, height, rgba8, stream_of(c, stream), "pe_yuv420_to_rgba8");
+}
+
+int pe_set_texture_yuv420(pe_ctx* c, const char* name, const void* yuv_host, const pe_yuv_format* format, int width, int height) {
+    if (!c) return 1;
+    const std::string fn = "pe_set_texture_yuv420";
+    if (!name || !yuv_host) return c->fail(fn + ": null argument");
+    if (!check_yuv420(c, fn, format, width, height)) return 1;
+    ensure_layout(c);
+    auto it = c->layout.tex_slot.find(name);
+    if (it == c->layout.tex_slot.end()) return c->fail(std::string("unknown texture `") + name + "`", 2);
+    if (!bind_device(c)) return 1;
+    DeviceBuffer& t = c->textures[name];
+    const size_t bytes = size_t(width) * size_t(height) * 4, planes = yuv420_bytes(width, height, format->bits);
+    uint8_t* rec = c->cblock.data() + c->layout.off_tex + size_t(it->second) * 16;
+    // As pe_set_texture: a render queued on any stream may still read the image, so wait for the device before touching it.
+    // If that wait fails the old image stays allocated and bound.
+    if (t.dev && !cuda_ok(c, cudaDeviceSynchronize(), "pe_set_texture_yuv420: waiting for queued renders")) return 1;
+    if (t.bytes != bytes) {            // another size: free the old image; until the new one is in place the sampler is unbound
+        t.release();
+        std::memset(rec, 0, 16);
+        if (!cuda_ok(c, t.ensure(bytes), "cudaMalloc(texture)")) return 1;
+    }
+    if (!cuda_ok(c, c->yuv_upload.ensure(planes), "cudaMalloc(texture planes)") ||
+        !cuda_ok(c, cudaMemcpyAsync(c->yuv_upload.dev, yuv_host, planes, cudaMemcpyHostToDevice, c->stream), "cudaMemcpy(texture planes)") ||
+        yuv420_launch(c, c->yuv_upload.dev, format, width, height, t.dev, c->stream, "pe_set_texture_yuv420") ||
+        !cuda_ok(c, cudaStreamSynchronize(c->stream), "pe_set_texture_yuv420")) {
+        std::memset(rec, 0, 16);       // the image may be half written: unbind it, keep the memory (it is freed with the context)
+        return 1;
+    }
+    std::memcpy(rec, &t.dev, 8);
+    std::memcpy(rec + 8, &width, 4);
+    std::memcpy(rec + 12, &height, 4);
+    return 0;
+}
+
 }  // extern "C"

@@ -106,6 +106,8 @@ struct pe_ctx {
     // pe_encode_png_rgba8's work space: filtered stream, per-segment deflate output, segment sizes / offsets / checksums; and
     // pe_encode_png_host's device copy of the file and its length
     pe_host::DeviceBuffer png_work, png_file, png_size;
+    // pe_set_texture_yuv420's device copy of the Y'CbCr planes it converts
+    pe_host::DeviceBuffer yuv_upload;
     // adaptive de-specialisation: a slot whose value differed between renders more than kMaxRespecialisations times is read
     // from the constant block from then on (bounds NVRTC compiles when an animation drives an int or a matrix structure)
     std::vector<int> last_ints, int_changes;

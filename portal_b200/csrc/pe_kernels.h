@@ -45,4 +45,11 @@ size_t yuv420p10_bytes(int width, int height);
 // (2-byte aligned, yuv420p10_bytes long).
 int launch_rgba_to_yuv420p10(const void* rgba, int bits, int width, int height, void* yuv, cudaStream_t s);
 
+// Y'CbCr 4:2:0 -> RGBA8 (pe_yuv.cu; DESIGN.md section 5.5).  Bytes of the planes at `bits` 8 (uint8 samples) or 10 (uint16), 0
+// when the size or the depth is invalid or the frame has more than 2^31 - 1 pixels.
+size_t yuv420_bytes(int width, int height, int bits);
+// One kernel launch: the planes at `yuv` (aligned to one sample) -> RGBA8 at `rgba` (4-byte aligned).  `matrix` 0 BT.709, 1
+// BT.601; `siting` 0 left, 1 centre; the caller has validated the format.
+int launch_yuv420_to_rgba8(const void* yuv, int bits, int matrix, int full_range, int siting, int width, int height, void* rgba, cudaStream_t s);
+
 }  // namespace pe_host

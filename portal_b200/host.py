@@ -375,10 +375,70 @@ class HostRenderer:
                                                                 motion_blur_frames, float(duration_seconds), out.ctypes.data))
         return out
 
+    def set_texture_yuv420(self, name: str, planes, fmt, width: int, height: int):
+        """pe_set_texture_yuv420: the Y'CbCr 4:2:0 planes (bytes or a numpy buffer of pe_yuv420_bytes, e.g. one
+        Y4MClip.read_frame) converted on the device (DESIGN.md section 5.5) into the image of texture `name`.  `fmt`:
+        capi.PeYuvFormat or (bits, matrix, full_range, siting)."""
+        f = capi.yuv_format(fmt)
+        buf = np.frombuffer(planes, np.uint8) if isinstance(planes, (bytes, bytearray)) else np.ascontiguousarray(planes).view(np.uint8)
+        if buf.nbytes < self._lib.pe_yuv420_bytes(width, height, f.bits):
+            raise ValueError("the planes are shorter than pe_yuv420_bytes")
+        self._pe(self._lib.pe_set_texture_yuv420(self._ctx, b(name), buf.ctypes.data, C.byref(f), width, height))
+
     def close(self):
         if getattr(self, "_ctx", None):
             self._lib.pe_destroy(self._ctx)
             self._ctx = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class Y4MClip:
+    """A YUV4MPEG2 clip read one frame at a time (ph_y4m_*, include/portal_b200_host.h): width, height, frame_count, format
+    (capi.PeYuvFormat; the matrix is the caller's, "bt709" or "bt601") and partial_bytes (a trailing partial frame, not
+    counted)."""
+
+    def __init__(self, path: str, matrix: str = "bt709"):
+        self._lib = capi.lib()
+        if matrix not in capi.MATRICES:
+            raise ValueError("matrix must be bt709 or bt601")
+        err = C.create_string_buffer(1024)
+        self._r = self._lib.ph_y4m_open(path.encode() if isinstance(path, str) else bytes(path), capi.MATRICES[matrix], err, len(err))
+        if not self._r:
+            raise PortalB200Error(err.value.decode(errors="replace"))
+        w, h, n, part = C.c_int32(), C.c_int32(), C.c_int64(), C.c_int64()
+        self.format = capi.PeYuvFormat()
+        self._lib.ph_y4m_info(self._r, C.byref(w), C.byref(h), C.byref(n), C.byref(self.format), C.byref(part))
+        self.width, self.height, self.frame_count, self.partial_bytes = w.value, h.value, n.value, part.value
+        self.frame_bytes = self._lib.pe_yuv420_bytes(self.width, self.height, self.format.bits)
+
+    def read_frame(self, k: int) -> np.ndarray:
+        """The planes of frame k as pe_set_texture_yuv420 takes them: a uint8 array of frame_bytes."""
+        out = np.empty(self.frame_bytes, np.uint8)
+        if self._lib.ph_y4m_read_frame(self._r, int(k), out.ctypes.data, out.nbytes):
+            raise PortalB200Error(self._lib.ph_y4m_last_error(self._r).decode(errors="replace"))
+        return out
+
+    def planes(self, k: int):
+        """(Y [h, w], Cb, Cr [ceil(h/2), ceil(w/2)]) of frame k: uint8 at 8 bits, uint16 at 10."""
+        v = self.read_frame(k).view(np.uint8 if self.format.bits == 8 else np.uint16)
+        n, cw, ch = self.width * self.height, (self.width + 1) // 2, (self.height + 1) // 2
+        return v[:n].reshape(self.height, self.width), v[n:n + cw * ch].reshape(ch, cw), v[n + cw * ch:].reshape(ch, cw)
+
+    def close(self):
+        if getattr(self, "_r", None):
+            self._lib.ph_y4m_close(self._r)
+            self._r = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
 
     def __del__(self):
         try:
