@@ -223,7 +223,10 @@ PE_API uint64_t pe_launch_count(pe_ctx* ctx);
 /* ---- multi-GPU helpers -------------------------------------------------------------------- */
 
 /* De-interleave strips gathered rank-major ([rank][local strip][row][x], every rank padded to
- * `strips_per_rank` strips) into a row-major frame.  Device pointers; async on `stream`. */
+ * `strips_per_rank` strips) into a row-major frame.  Device pointers; async on `stream`.  Both buffers hold float RGBA
+ * pixels and must be 16-byte aligned.  Global strip g is local strip g / n_ranks of rank g % n_ranks, so
+ * strips_per_rank >= ceil(ceil(height / strip_rows) / n_ranks) (larger values are padding); anything else is refused
+ * before any launch. */
 PE_API int pe_deinterleave_strips(pe_ctx* ctx, const void* gathered_device, void* frame_device, int width, int height,
                            int strip_rows, int n_ranks, int strips_per_rank, void* stream);
 /* Device memory owned by the context (cudaMalloc, so its base address can be exported over IPC). */
@@ -301,10 +304,14 @@ PE_API int pe_sharder_release_frame(pe_sharder* s, uint64_t frame_no);
 
 /* ---- frame post-processing (the offline `render` caller, src/main.rs:640-722) -------------- */
 
-/* Motion-blur average of n RGBA8 frames in gamma-2 space (average_images). Device pointers. */
+/* Motion-blur average of 1 <= n <= 64 RGBA8 frames in gamma-2 space (average_images).  Device pointers, none null; frames
+ * and output 4-byte aligned (16-byte aligned buffers take the vector kernel).  Asynchronous on `stream`.  Bad arguments
+ * are refused before any launch. */
 PE_API int pe_average_frames_rgba8(pe_ctx* ctx, const void* const* frames_device, int n_frames, void* out_device,
                             size_t n_pixels, void* stream);
-/* float RGBA -> RGBA8, the render target's quantisation. Device pointers. */
+/* float RGBA -> RGBA8, the render target's quantisation: round_half_even(f32(clamp(v, 0, 1) * 255)), NaN -> 0.
+ * `rgba_f32_device` 16-byte aligned, `rgba8_device` 4-byte aligned (a 16-byte aligned output takes the vector kernel), else
+ * refused before any launch.  Device pointers; asynchronous on `stream`. */
 PE_API int pe_quantize_rgba8(pe_ctx* ctx, const void* rgba_f32_device, void* rgba8_device, size_t n_pixels, void* stream);
 /* Bit comparison of two device buffers (16-byte aligned, `bytes` a multiple of 16): *words_out = how many 16-byte words
  * (= float RGBA pixels) differ.  Synchronous.  pe_autotune's guard uses it -- a candidate variant is only eligible when its

@@ -966,8 +966,15 @@ uint64_t pe_launch_count(pe_ctx* c) { return c ? c->launches : 0; }
 int pe_deinterleave_strips(pe_ctx* c, const void* gathered, void* frame, int width, int height, int strip_rows, int n_ranks,
                            int strips_per_rank, void* stream) {
     if (!c) return 1;
-    if (!gathered || !frame || width <= 0 || height <= 0 || strip_rows <= 0 || n_ranks <= 0 || strips_per_rank <= 0)
+    if (!gathered || !frame || width <= 0 || height <= 0 || strip_rows <= 0 || n_ranks <= 0)
         return c->fail("pe_deinterleave_strips: bad arguments");
+    if ((uintptr_t(gathered) & 15) || (uintptr_t(frame) & 15))
+        return c->fail("pe_deinterleave_strips: the gathered strips and the frame must be 16-byte aligned");
+    // global strip g is read from local strip g / n_ranks of rank g % n_ranks: every rank must hold ceil(strips / n_ranks)
+    const long long strips = (height + (long long)strip_rows - 1) / strip_rows, need = (strips + n_ranks - 1) / n_ranks;
+    if (strips_per_rank < need)
+        return c->fail("pe_deinterleave_strips: strips_per_rank " + std::to_string(strips_per_rank) +
+                       " is below ceil(ceil(height / strip_rows) / n_ranks) = " + std::to_string(need));
     if (!bind_device(c)) return 1;
     const cudaStream_t s = stream_of(c, stream);
     if (!cuda_ok(c, (cudaError_t)launch_deinterleave(gathered, frame, width, height, strip_rows, n_ranks, strips_per_rank,
@@ -1155,7 +1162,12 @@ int pe_ipc_close(pe_ctx* c, void* p) {
 // ------------------------------------------------------------------------------ post-processing
 int pe_average_frames_rgba8(pe_ctx* c, const void* const* frames, int n_frames, void* out, size_t n_pixels, void* stream) {
     if (!c) return 1;
-    if (!frames || !out || n_frames < 1) return c->fail("pe_average_frames_rgba8: bad arguments");
+    if (!frames || !out || n_frames < 1 || n_frames > 64) return c->fail("pe_average_frames_rgba8: bad arguments (1 <= n_frames <= 64)");
+    for (int i = 0; i < n_frames; i++)
+        if (!frames[i]) return c->fail("pe_average_frames_rgba8: frame " + std::to_string(i) + " is null");
+    bool aligned = (uintptr_t(out) & 3) == 0;
+    for (int i = 0; i < n_frames; i++) aligned = aligned && (uintptr_t(frames[i]) & 3) == 0;
+    if (!aligned) return c->fail("pe_average_frames_rgba8: the frames and the output must be 4-byte aligned");
     if (!bind_device(c)) return 1;
     const cudaStream_t s = stream_of(c, stream);
     if (!cuda_ok(c, (cudaError_t)launch_average_rgba8(frames, n_frames, out, n_pixels, c->sm_count, s), "average")) return 1;
@@ -1166,6 +1178,7 @@ int pe_average_frames_rgba8(pe_ctx* c, const void* const* frames, int n_frames, 
 int pe_quantize_rgba8(pe_ctx* c, const void* in, void* out, size_t n_pixels, void* stream) {
     if (!c) return 1;
     if (!in || !out) return c->fail("pe_quantize_rgba8: bad arguments");
+    if ((uintptr_t(in) & 15) || (uintptr_t(out) & 3)) return c->fail("pe_quantize_rgba8: the float frame must be 16-byte and the output 4-byte aligned");
     if (!bind_device(c)) return 1;
     const cudaStream_t s = stream_of(c, stream);
     if (!cuda_ok(c, (cudaError_t)launch_quantize_rgba8(in, out, n_pixels, c->sm_count, s), "quantize")) return 1;

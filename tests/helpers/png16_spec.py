@@ -44,11 +44,15 @@ def quantize16(frame: np.ndarray) -> np.ndarray:
     return np.rint(np.clip(f, np.float32(0.0), np.float32(1.0)) * np.float32(65535.0)).astype(np.uint16)
 
 
-def average16_channel(qs) -> int:
-    """One channel of the 16-bit motion-blur average, in Python integers: floor(sqrt(floor(sum q^2 / n)) + 1/2)."""
-    m = sum(q * q for q in qs) // len(qs)
+def round_sqrt16(m: int) -> int:
+    """floor(sqrt(m) + 1/2) of an integer m >= 0, in Python integers: sqrt(m) + 1/2 >= k + 1 <=> m - k^2 > k, k = isqrt(m)."""
     k = math.isqrt(m)
     return k + 1 if m - k * k > k else k
+
+
+def average16_channel(qs) -> int:
+    """One channel of the 16-bit motion-blur average, in Python integers: floor(sqrt(floor(sum q^2 / n)) + 1/2)."""
+    return round_sqrt16(sum(q * q for q in qs) // len(qs))
 
 
 def average16(frames) -> np.ndarray:
