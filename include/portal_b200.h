@@ -43,7 +43,7 @@ typedef struct pe_ctx pe_ctx;
 PE_API pe_ctx* pe_create(int device);
 PE_API void pe_destroy(pe_ctx* ctx);
 /* Message of the last failed call on this context (never NULL). With ctx == NULL: why the last
- * pe_create failed. */
+ * pe_create of the calling thread failed. */
 PE_API const char* pe_last_error(pe_ctx* ctx);
 /* ABI version of this header: major * 100 + minor. */
 PE_API int pe_abi_version(void);

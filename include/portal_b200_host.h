@@ -178,6 +178,15 @@ PE_API int ph_player_render_frame(ph_player* pl, pe_ctx* ctx, const ph_frame_par
 PE_API int ph_player_render_motion_blur_frame(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index,
                                               int frame_count, int motion_blur_frames, double duration_seconds,
                                               uint8_t* out_host_rgba8);
+/* The player state of ph_player_render_motion_blur_frame* without the frame: exactly the same sub-frame updates -- the same
+ * times t_j * duration_seconds, in the same order, with the same probes through the attached context or probe function --
+ * and the same refusal of bad arguments, but no update hook, no uniform upload and no render.  A caller that deals the
+ * frames of one animation out to several players (`portal_b200_render render --devices`) advances every player through the
+ * frames it does not render, so that each one's camera, teleport matrix and subspace flag at frame i are the sequential
+ * ones.  Skipping the hook is safe when, as in the render CLI's video hook, what the hook binds is derived from the scene's
+ * current state alone: the next update that does call it binds the right frame. */
+PE_API int ph_player_advance_motion_blur_frame(ph_player* pl, int frame_index, int frame_count, int motion_blur_frames,
+                                               double duration_seconds);
 /* Adaptive anti-aliasing for the player's frames (off by default): when on, ph_player_render_frame and every sub-frame of
  * ph_player_render_motion_blur_frame (before the unchanged gamma-2 average) are rendered by pe_render_adaptive with
  * `threshold` -- one sample everywhere, all aa_count samples where the one-sample frame has an edge.  ph_player_render_frame

@@ -207,6 +207,7 @@ def lib() -> C.CDLL:
         "ph_scene_camera_name": (i32, [vp, i32, C.POINTER(cp)]),
         "ph_player_render_frame": (i32, [vp, vp, C.POINTER(PhFrameParams), vp, i32]),
         "ph_player_render_motion_blur_frame": (i32, [vp, vp, C.POINTER(PhFrameParams), i32, i32, i32, C.c_double, vp]),
+        "ph_player_advance_motion_blur_frame": (i32, [vp, i32, i32, i32, C.c_double]),
         "ph_player_set_adaptive_aa": (i32, [vp, i32, i32]),
         "ph_player_render_frame_png": (i32, [vp, vp, C.POINTER(PhFrameParams), vp, C.c_size_t, C.POINTER(C.c_size_t)]),
         "ph_player_render_motion_blur_frame_png": (i32, [vp, vp, C.POINTER(PhFrameParams), i32, i32, i32, C.c_double, vp, C.c_size_t,

@@ -642,13 +642,29 @@ int ph_player_render_frame_png16(ph_player* pl, pe_ctx* ctx, const ph_frame_para
     return 0;
 }
 
+// The sub-frame update times of one output frame of render_animation (main.rs:1786-1797): sub-frame j at t * duration_seconds,
+// t = frame_index / frame_count + j / motion_blur_frames / frame_count * exposure, exposure 0.5.  The render and the advance
+// paths both check their arguments and take their times here, so that they cannot drift apart.
+static int motion_blur_times(ph_player* pl, const char* fn, int frame_index, int frame_count, int motion_blur_frames, double duration_seconds,
+                             std::vector<double>& times) {
+    if (frame_count < 1 || motion_blur_frames < 1 || motion_blur_frames > 64 || frame_index < 0)
+        return pfail(pl, std::string(fn) + ": bad frame arguments");
+    const double exposure = 0.5;
+    times.resize(size_t(motion_blur_frames));
+    for (int j = 0; j < motion_blur_frames; j++) {
+        const double tt = double(frame_index) / double(frame_count) + double(j) / double(motion_blur_frames) / double(frame_count) * exposure;
+        times[size_t(j)] = tt * duration_seconds;
+    }
+    return 0;
+}
+
 // The device half of ph_player_render_motion_blur_frame*: the sub-frames and their gamma-2 average, left in scratch slot 0
 // (*out); the sub-frames use slots 1 .. motion_blur_frames.  `bits` is the sub-frames' format: 8 -- RGBA8, rendered so by
 // the render kernel; 16 -- RGBA16, each rendered as floats into slot motion_blur_frames + 1 and quantised from there.
 static int motion_blur_device(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index, int frame_count, int motion_blur_frames,
                               double duration_seconds, int bits, void** out) {
-    if (frame_count < 1 || motion_blur_frames < 1 || motion_blur_frames > 64 || frame_index < 0)
-        return pfail(pl, "ph_player_render_motion_blur_frame: bad frame arguments");
+    std::vector<double> times;
+    if (motion_blur_times(pl, "ph_player_render_motion_blur_frame", frame_index, frame_count, motion_blur_frames, duration_seconds, times)) return 1;
     const size_t n = size_t(p->width) * size_t(p->height), px_bytes = bits == 16 ? 8 : 4;
     std::vector<void*> sub(size_t(motion_blur_frames), nullptr);
     void* f32 = nullptr;
@@ -657,12 +673,14 @@ static int motion_blur_device(ph_player* pl, pe_ctx* ctx, const ph_frame_params*
     if (bits == 16) rc |= pe_scratch_buffer(ctx, 1 + motion_blur_frames, n * 16, &f32);
     if (rc) pl->err = std::string("device allocation failed: ") + pe_last_error(ctx);
     pe_target t = {p->width, p->height, p->height, 0, 1, 1, 1};
-    const double exposure = 0.5;  // main.rs:1787
     for (int j = 0; j < motion_blur_frames && !rc; j++) {
-        const double tt = double(frame_index) / double(frame_count) + double(j) / double(motion_blur_frames) / double(frame_count) * exposure;
         ph_frame_params q = *p;
         q.aa_start = j;  // main.rs:1797
-        if (!pl->player.update(tt * duration_seconds)) { pl->err = pl->player.error; rc = 1; break; }   // self.update(memory, t * duration)
+        if (!pl->player.update(times[size_t(j)])) {   // self.update(memory, t * duration)
+            pl->err = pl->player.error;
+            rc = 1;
+            break;
+        }
         if (pl->hook && pl->hook(pl->hook_user)) { pl->err = "the update hook failed"; rc = 1; break; }   // ... whose tail swaps video frames
         if (upload_player_uniforms(pl, ctx, &q)) {
             rc = 1;
@@ -678,6 +696,15 @@ static int motion_blur_device(ph_player* pl, pe_ctx* ctx, const ph_frame_params*
         rc = 1;
     }
     return rc ? 1 : 0;
+}
+
+int ph_player_advance_motion_blur_frame(ph_player* pl, int frame_index, int frame_count, int motion_blur_frames, double duration_seconds) {
+    if (!pl) return 1;
+    std::vector<double> times;
+    if (motion_blur_times(pl, "ph_player_advance_motion_blur_frame", frame_index, frame_count, motion_blur_frames, duration_seconds, times)) return 1;
+    for (double t : times)
+        if (!pl->player.update(t)) return pfail(pl, pl->player.error);
+    return 0;
 }
 
 int ph_player_render_motion_blur_frame(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index, int frame_count,

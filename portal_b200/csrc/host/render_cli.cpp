@@ -44,6 +44,16 @@
 // in order: --video name=clip.y4m (a clip that cannot be opened, or a name that is not a video of the scene, exits 1 before
 // anything is rendered); the PNG frames of video_png/<stem>/, exactly as above; <assets>/video_y4m/<stem>.y4m.  The matrix is
 // not in the stream: --video-matrix, BT.709 by default.  A status line names each video's source and format.
+//
+// --devices LIST (`render`; not in the reference): frame-parallel rendering with one worker thread per entry, e.g. 0,1,2,3 for
+// four GPUs or 0,0 for two workers sharing GPU 0 (one renders while the other reads back and writes).  Every output byte is
+// the one a single worker (--device K, the default) writes; DESIGN.md section 8.1.  Each worker has its own context, scene,
+// player, clip handles and pinned buffers, and runs the whole loop: frame i of an animation is rendered by worker i mod N and
+// replayed by every other one (ph_player_advance_motion_blur_frame), so that camera teleportation through portals -- state that
+// carries from frame to frame -- is the sequential one everywhere.  Skip-existing decides from one snapshot of the output taken
+// before the workers start.  Frame files are written by their worker; a Y4M stream by the main thread, in frame order, with at
+// most two frames per worker in flight.  Status lines come in frame order, as from one worker.  The first failure stops every
+// worker at its next frame boundary, exits 1 and renames no stream.  render-frame takes one entry.
 #include <dirent.h>
 #include <sys/stat.h>
 #include <sys/types.h>
@@ -53,10 +63,14 @@
 #include <cstdlib>
 #include <cstring>
 #include <algorithm>
+#include <condition_variable>
 #include <fstream>
 #include <map>
+#include <mutex>
+#include <set>
 #include <sstream>
 #include <string>
+#include <thread>
 #include <vector>
 
 #include "../../../include/portal_b200_host.h"
@@ -126,18 +140,33 @@ static bool write_image16(const std::string& output, const std::vector<uint8_t>&
     return bool(out);
 }
 
-// One PNG file -> the sampler `name` (Texture2D::from_file_with_format + material.set_texture, main.rs:1072-1078)
-static bool set_texture_from_png(pe_ctx* ctx, const std::string& name, const std::string& path, std::string& why) {
+// A PNG file decoded to RGBA8; `why` is non-empty when the file cannot be used
+struct DecodedPng {
+    std::vector<uint8_t> px;
+    int32_t w = 0, h = 0;
+    std::string why;
+};
+static DecodedPng decode_png(const std::string& path) {
+    DecodedPng d;
     bool ok = false;
     const std::string bytes = slurp(path, ok);
-    if (!ok) { why = "cannot read " + path; return false; }
     uint8_t* px = nullptr;
-    int32_t w = 0, h = 0;
     char err[256] = {0};
-    if (ph_png_decode(reinterpret_cast<const uint8_t*>(bytes.data()), bytes.size(), &px, &w, &h, err, sizeof err)) { why = path + ": " + err; return false; }
-    const int rc = pe_set_texture(ctx, name.c_str(), px, w, h);
+    if (!ok) d.why = "cannot read " + path;
+    else if (ph_png_decode(reinterpret_cast<const uint8_t*>(bytes.data()), bytes.size(), &px, &d.w, &d.h, err, sizeof err)) d.why = path + ": " + err;
+    else d.px.assign(px, px + size_t(d.w) * size_t(d.h) * 4);
     ph_png_free(px);
-    if (rc) { why = pe_last_error(ctx); return false; }
+    return d;
+}
+// The scene's textures are decoded once, their pixels shared by every worker's context
+static const DecodedPng& decode_png_once(std::map<std::string, DecodedPng>& cache, const std::string& path) {
+    auto it = cache.find(path);
+    return it != cache.end() ? it->second : cache.emplace(path, decode_png(path)).first->second;
+}
+// A decoded PNG -> the sampler `name` (Texture2D::from_file_with_format + material.set_texture, main.rs:1072-1078)
+static bool set_texture_decoded(pe_ctx* ctx, const std::string& name, const DecodedPng& d, std::string& why) {
+    if (!d.why.empty()) { why = d.why; return false; }
+    if (pe_set_texture(ctx, name.c_str(), d.px.data(), d.w, d.h)) { why = pe_last_error(ctx); return false; }
     return true;
 }
 
@@ -190,7 +219,7 @@ static int update_videos(void* user) {
                 pe_set_texture_yuv420(st.ctx, v.name.c_str(), v.planes, &v.format, v.clip_w, v.clip_h)) continue;   // as below
         } else {
             std::string why;
-            if (!set_texture_from_png(st.ctx, v.name, v.frames[size_t(idx)], why)) continue;   // IO errors are ignored there too: the texture just does not update
+            if (!set_texture_decoded(st.ctx, v.name, decode_png(v.frames[size_t(idx)]), why)) continue;   // IO errors are ignored there too: the texture just does not update
         }
         v.last = long(idx);
     }
@@ -204,15 +233,16 @@ static std::string clip_description(const std::string& path, const VideoRuntime&
            (v.format.full_range ? "full range, " : "limited range, ") + (v.format.siting == PE_YUV_SITING_CENTER ? "centre siting" : "left siting");
 }
 
-// Opens a Y4M clip for video `v`; false with a message in `why` when it cannot be used.
-static bool open_clip(VideoRuntime& v, const std::string& path, int matrix, std::string& why) {
+// Opens a Y4M clip for video `v`; false with a message in `why` when it cannot be used.  `quiet`: a clip opened again for
+// another worker, whose trailing partial frame was reported already.
+static bool open_clip(VideoRuntime& v, const std::string& path, int matrix, std::string& why, bool quiet = false) {
     char err[1024] = {0};
     v.clip = ph_y4m_open(path.c_str(), matrix, err, sizeof err);
     if (!v.clip) { why = err; return false; }
     int64_t partial = 0;
     ph_y4m_info(v.clip, &v.clip_w, &v.clip_h, &v.clip_frames, &v.format, &partial);
     if (v.clip_frames < 1) { why = path + ": no complete frame"; ph_y4m_close(v.clip); v.clip = nullptr; return false; }
-    if (partial) std::fprintf(stderr, "%s: a trailing partial frame of %lld bytes is ignored\n", path.c_str(), (long long)partial);
+    if (partial && !quiet) std::fprintf(stderr, "%s: a trailing partial frame of %lld bytes is ignored\n", path.c_str(), (long long)partial);
     v.planes_bytes = pe_yuv420_bytes(v.clip_w, v.clip_h, v.format.bits);
     return true;
 }
@@ -241,6 +271,96 @@ static bool make_dirs(const std::string& path) {
     return ::stat(path.c_str(), &st) == 0 && S_ISDIR(st.st_mode);
 }
 
+// --devices 0,1,... -> the device of each worker; false with a message when an entry is empty, negative or not an integer
+static bool parse_devices(const std::string& list, std::vector<int>& devices, std::string& why) {
+    devices.clear();
+    if (list.empty()) { why = "needs at least one device index"; return false; }
+    size_t start = 0;
+    for (;;) {
+        const size_t comma = list.find(',', start);
+        const std::string e = list.substr(start, comma == std::string::npos ? std::string::npos : comma - start);
+        if (e.empty()) { why = "`" + list + "` has an empty entry"; return false; }
+        if (e[0] == '-') { why = "`" + list + "`: device `" + e + "` is negative"; return false; }
+        if (e.size() > 9 || e.find_first_not_of("0123456789") != std::string::npos) {
+            why = "`" + list + "`: device `" + e + "` is not an integer";
+            return false;
+        }
+        devices.push_back(std::atoi(e.c_str()));
+        if (comma == std::string::npos) return true;
+        start = comma + 1;
+    }
+}
+
+// One worker: a context, a scene parsed from the scene text, a player and the video runtimes, all its own
+struct Worker {
+    pe_ctx* ctx = nullptr;
+    ph_scene* scene = nullptr;
+    ph_player* player = nullptr;
+    VideoState video_state;                           // the player's update hook points here: workers never move
+    std::vector<uint8_t> px;                          // the frame: RGBA8 / RGBA16 pixels or a PNG file
+    size_t png_len = 0;
+    std::vector<std::vector<uint8_t>> free_planes;   // `render` to Y4M: the plane buffers the main thread does not hold
+};
+
+// What `render` does with one entry of the animation list, decided before any worker starts
+struct AnimationPlan {
+    bool rendered = false;           // false: --starts-with filters it out (it is still initialised and updated once)
+    double duration = 0.0;           // the f32 duration render_animation takes
+    int count = 1, todo = 0;         // frames of the animation, frames to render (--max-frames)
+    bool skip_stream = false;        // Y4M: the stream exists
+    std::vector<char> skip_frame;    // frame files: frame i exists
+};
+
+// The workers' link to the main thread: frames done, in any order, and the first failure
+struct Shared {
+    std::mutex m;
+    std::condition_variable cv;
+    bool stop = false;
+    std::string error;
+    // (animation, frame) -> the frame's Y4M planes (empty for the other formats); frame -1: the animation has begun
+    std::map<std::pair<size_t, int>, std::vector<uint8_t>> done;
+
+    void fail(const std::string& why) {
+        std::lock_guard<std::mutex> lk(m);
+        if (!stop) { stop = true; error = why; }
+        cv.notify_all();
+    }
+    bool stopped() {
+        std::lock_guard<std::mutex> lk(m);
+        return stop;
+    }
+    void post(size_t k, int i, std::vector<uint8_t> planes) {
+        std::lock_guard<std::mutex> lk(m);
+        done[{k, i}] = std::move(planes);
+        cv.notify_all();
+    }
+    // The main thread: waits for (k, i).  What was posted before a failure is still handed out, in order, so that a single
+    // worker's output up to its failure is exactly the sequential loop's.  False: a failure, and (k, i) will not come.
+    bool take(size_t k, int i, std::vector<uint8_t>& planes) {
+        std::unique_lock<std::mutex> lk(m);
+        cv.wait(lk, [&] { return stop || done.count({k, i}) != 0; });
+        auto it = done.find({k, i});
+        if (it == done.end()) return false;
+        planes = std::move(it->second);
+        done.erase(it);
+        return true;
+    }
+    // A worker: one of its plane buffers, once the main thread has written the frame it held; false on a failure
+    bool take_buffer(Worker& w, std::vector<uint8_t>& planes) {
+        std::unique_lock<std::mutex> lk(m);
+        cv.wait(lk, [&] { return stop || !w.free_planes.empty(); });
+        if (stop) return false;
+        planes = std::move(w.free_planes.back());
+        w.free_planes.pop_back();
+        return true;
+    }
+    void give_back(Worker& w, std::vector<uint8_t>& planes) {
+        std::lock_guard<std::mutex> lk(m);
+        w.free_planes.push_back(std::move(planes));
+        cv.notify_all();
+    }
+};
+
 int main(int argc, char** argv) {
     const bool frame_cmd = argc >= 3 && std::strcmp(argv[1], "render-frame") == 0;
     const bool anim_cmd = argc >= 3 && std::strcmp(argv[1], "render") == 0;
@@ -248,19 +368,19 @@ int main(int argc, char** argv) {
         std::fprintf(stderr, "usage: %s render-frame <scene.ron> [--width W] [--height H] [--render-depth D] [--aa-count N] [--time T] "
                              "[--stage NAME] [--animation NAME] [--camera NAME] [--device K] [--texture name=file.png|name=file.rgba:WxH] [--assets DIR] [--output out.png|.ppm|.rgba|.y4m] [--adaptive-aa T] [--bit-depth 8|16] [--video name=clip.y4m] [--video-matrix bt709|bt601]\n"
                              "       %s render <scene.ron> [a,b | --animations a,b | --starts-with PREFIX] [--fps N] [--motion-blur-frames M] [--width W] [--height H] "
-                             "[--render-depth D] [--aa-count N] [--stereo-image] [--no-skip-existing] [--out-dir DIR] [--max-frames K] [--frame-format ppm|png|rgba|y4m] [--adaptive-aa T] [--bit-depth 8|16] [--video name=clip.y4m] [--video-matrix bt709|bt601]\n", argv[0], argv[0]);
+                             "[--render-depth D] [--aa-count N] [--stereo-image] [--no-skip-existing] [--out-dir DIR] [--max-frames K] [--frame-format ppm|png|rgba|y4m] [--adaptive-aa T] [--bit-depth 8|16] [--video name=clip.y4m] [--video-matrix bt709|bt601] [--device K | --devices K,K,...]\n", argv[0], argv[0]);
         return 2;
     }
     std::string scene_path = argv[2], output = "frame.ppm", out_dir = "video";
     // defaults of RenderFrameCliOptions (main.rs:2744-2754) / RenderCliOptions (main.rs:2764-2803)
     int width = frame_cmd ? 1920 : 3840, height = frame_cmd ? 1080 : 2160, depth = frame_cmd ? 100 : 150, aa = frame_cmd ? 1 : 4, device = 0;
     int fps = 60, motion_blur = 1, max_frames = -1;
-    bool stereo = false, skip_existing = true, adaptive = false;
+    bool stereo = false, skip_existing = true, adaptive = false, device_given = false, devices_given = false;
     int adaptive_threshold = 0, bits = 8;
     double time = 0.0;
     std::vector<std::string> textures, videos;
     int video_matrix = PE_YUV_BT709;
-    std::string stage, animation, camera, animations, starts_with, assets, frame_ext = ".ppm";
+    std::string stage, animation, camera, animations, starts_with, assets, frame_ext = ".ppm", devices_list;
     int first_option = 3;
     if (anim_cmd && argc > 3 && std::strncmp(argv[3], "--", 2) != 0) animations = argv[first_option++];   // `render <scene> [animations]`
     for (int i = first_option; i < argc; i++) {
@@ -271,7 +391,8 @@ int main(int argc, char** argv) {
         else if (a == "--render-depth" || a == "--render_depth") depth = std::atoi(next());
         else if (a == "--aa-count" || a == "--aa_count") aa = std::atoi(next());
         else if (a == "--time") time = std::atof(next());
-        else if (a == "--device") device = std::atoi(next());
+        else if (a == "--device") { device = std::atoi(next()); device_given = true; }
+        else if (a == "--devices") { devices_list = next(); devices_given = true; }
         else if (a == "--stage") stage = next();
         else if (a == "--animation") animation = next();
         else if (a == "--camera") camera = next();
@@ -307,6 +428,16 @@ int main(int argc, char** argv) {
             bits = std::atoi(v.c_str());
         }
         else { std::fprintf(stderr, "unknown option %s\n", a.c_str()); return 2; }
+    }
+    std::vector<int> devices = {device};         // one worker per entry
+    if (devices_given) {
+        std::string why;
+        if (device_given) { std::fprintf(stderr, "--devices and --device exclude each other\n"); return 2; }
+        if (!parse_devices(devices_list, devices, why)) { std::fprintf(stderr, "--devices %s\n", why.c_str()); return 2; }
+        if (frame_cmd && devices.size() > 1) {
+            std::fprintf(stderr, "render-frame renders one frame on one device: --devices takes one entry here, got `%s`\n", devices_list.c_str());
+            return 2;
+        }
     }
     bool ok = false;
     std::string text = slurp(scene_path, ok);
@@ -353,198 +484,304 @@ int main(int argc, char** argv) {
         std::string why;
         if (!open_clip(given_clips[name], path, video_matrix, why)) { std::fprintf(stderr, "--video %s: %s\n", g.c_str(), why.c_str()); return 1; }
     }
-    pe_ctx* ctx = pe_create(device);
-    if (!ctx) { std::fprintf(stderr, "pe_create: %s\n", pe_last_error(nullptr)); return 1; }
-    ph_player* player = ph_player_new(scene);
-    if (adaptive) ph_player_set_adaptive_aa(player, 1, adaptive_threshold);
-    if (frame_cmd) {  // main.rs:2900-2926
-        if (!stage.empty() && ph_player_init_stage(player, stage.c_str())) {
-            std::fprintf(stderr, "Scene `%s` has no stage named `%s`\n", scene_path.c_str(), stage.c_str());
-            return 1;
-        }
-        if (!animation.empty() && ph_player_init_animation(player, animation.c_str())) {
-            std::fprintf(stderr, "Scene `%s` has no animation named `%s`\n", scene_path.c_str(), animation.c_str());
-            return 1;
-        }
-        if (!camera.empty() && ph_player_select_camera(player, camera.c_str())) {
-            std::fprintf(stderr, "Scene `%s` has no camera named `%s`\n", scene_path.c_str(), camera.c_str());
-            return 1;
-        }
+    std::vector<Worker> workers(devices.size());
+    for (size_t w = 0; w < workers.size(); w++) {    // every device is opened before any work
+        workers[w].ctx = pe_create(devices[w]);
+        if (!workers[w].ctx) { std::fprintf(stderr, "pe_create: %s\n", pe_last_error(nullptr)); return 1; }
+        workers[w].scene = w == 0 ? scene : ph_scene_load_ron(text.data(), text.size(), err, sizeof err);
     }
-    if (ph_scene_build_program(scene, ctx) || ph_scene_upload_uniforms(scene, ctx)) {
-        std::fprintf(stderr, "%s\n", ph_scene_last_error(scene));
-        return 1;
-    }
-    std::map<std::string, bool> given;
-    for (const std::string& t : textures) {  // name=file.png | name=file.rgba:WxH
-        size_t eq = t.find('='), colon = t.rfind(':'), x = t.rfind('x');
-        if (eq != std::string::npos && ends_with(t, ".png")) {
-            std::string why;
-            if (!set_texture_from_png(ctx, t.substr(0, eq), t.substr(eq + 1), why)) { std::fprintf(stderr, "texture %s: %s\n", t.c_str(), why.c_str()); return 1; }
+    // Everything up to the first frame, for one worker.  Only the first reports what it finds (textures, videos): the others
+    // find the same.
+    std::map<std::string, DecodedPng> decoded;
+    std::set<std::string> given_video_names;
+    for (auto& kv : given_clips) given_video_names.insert(kv.first);
+    auto set_up = [&](Worker& wk, bool first) -> int {
+        pe_ctx* ctx = wk.ctx;
+        ph_scene* sc = wk.scene;
+        ph_player* player = wk.player = ph_player_new(sc);
+        if (adaptive) ph_player_set_adaptive_aa(player, 1, adaptive_threshold);
+        if (frame_cmd) {  // main.rs:2900-2926
+            if (!stage.empty() && ph_player_init_stage(player, stage.c_str())) {
+                std::fprintf(stderr, "Scene `%s` has no stage named `%s`\n", scene_path.c_str(), stage.c_str());
+                return 1;
+            }
+            if (!animation.empty() && ph_player_init_animation(player, animation.c_str())) {
+                std::fprintf(stderr, "Scene `%s` has no animation named `%s`\n", scene_path.c_str(), animation.c_str());
+                return 1;
+            }
+            if (!camera.empty() && ph_player_select_camera(player, camera.c_str())) {
+                std::fprintf(stderr, "Scene `%s` has no camera named `%s`\n", scene_path.c_str(), camera.c_str());
+                return 1;
+            }
+        }
+        if (ph_scene_build_program(sc, ctx) || ph_scene_upload_uniforms(sc, ctx)) {
+            std::fprintf(stderr, "%s\n", ph_scene_last_error(sc));
+            return 1;
+        }
+        std::map<std::string, bool> given;
+        for (const std::string& t : textures) {  // name=file.png | name=file.rgba:WxH
+            size_t eq = t.find('='), colon = t.rfind(':'), x = t.rfind('x');
+            if (eq != std::string::npos && ends_with(t, ".png")) {
+                std::string why;
+                if (!set_texture_decoded(ctx, t.substr(0, eq), decode_png_once(decoded, t.substr(eq + 1)), why)) { std::fprintf(stderr, "texture %s: %s\n", t.c_str(), why.c_str()); return 1; }
+                given[t.substr(0, eq)] = true;
+                continue;
+            }
+            if (eq == std::string::npos || colon == std::string::npos || x == std::string::npos || x < colon) { std::fprintf(stderr, "bad --texture %s\n", t.c_str()); return 2; }
             given[t.substr(0, eq)] = true;
-            continue;
+            int tw = std::atoi(t.substr(colon + 1, x - colon - 1).c_str()), th = std::atoi(t.substr(x + 1).c_str());
+            bool tok = false;
+            std::string bytes = slurp(t.substr(eq + 1, colon - eq - 1), tok);
+            if (!tok || bytes.size() != size_t(tw) * size_t(th) * 4) { std::fprintf(stderr, "texture %s: cannot read / wrong size\n", t.c_str()); return 1; }
+            if (pe_set_texture(ctx, t.substr(0, eq).c_str(), reinterpret_cast<const uint8_t*>(bytes.data()), tw, th)) { std::fprintf(stderr, "%s\n", pe_last_error(ctx)); return 1; }
         }
-        if (eq == std::string::npos || colon == std::string::npos || x == std::string::npos || x < colon) { std::fprintf(stderr, "bad --texture %s\n", t.c_str()); return 2; }
-        given[t.substr(0, eq)] = true;
-        int tw = std::atoi(t.substr(colon + 1, x - colon - 1).c_str()), th = std::atoi(t.substr(x + 1).c_str());
-        bool tok = false;
-        std::string bytes = slurp(t.substr(eq + 1, colon - eq - 1), tok);
-        if (!tok || bytes.size() != size_t(tw) * size_t(th) * 4) { std::fprintf(stderr, "texture %s: cannot read / wrong size\n", t.c_str()); return 1; }
-        if (pe_set_texture(ctx, t.substr(0, eq).c_str(), reinterpret_cast<const uint8_t*>(bytes.data()), tw, th)) { std::fprintf(stderr, "%s\n", pe_last_error(ctx)); return 1; }
-    }
-    // reload_textures (main.rs:1066-1085): every texture of the scene from its stored path; a failure is reported, the render goes on
-    for (int k = 0;; k++) {
-        const char *name = nullptr, *path = nullptr;
-        if (ph_scene_texture(scene, k, &name, &path)) break;
-        if (given.count(name)) continue;
-        const std::string file = assets.empty() || (path[0] == '/') ? std::string(path) : assets + "/" + path;
-        std::string why;
-        if (!set_texture_from_png(ctx, name, file, why)) std::fprintf(stderr, "texture `%s`: %s (the sampler stays unbound)\n", name, why.c_str());
-    }
-    if (pe_scene_compile(ctx)) { std::fprintf(stderr, "%s\n", pe_last_error(ctx)); return 1; }
-    ph_player_attach(player, ctx);  // camera teleportation goes through pe_probe_ray
-    // VideoRuntime::from_scene (main.rs:820-858): videos that have a path, a uniform and frames on disk
-    VideoState video_state;
-    video_state.scene = scene;
-    video_state.ctx = ctx;
-    for (int k = 0;; k++) {
-        const char *name = nullptr, *path = nullptr, *uniform = nullptr;
-        if (ph_scene_video(scene, k, &name, &path, &uniform)) break;
-        if (!path[0] || !uniform[0]) continue;
-        VideoRuntime v;
-        std::string source;
-        auto it = given_clips.find(name);
-        if (it != given_clips.end()) {                                   // --video
-            v = it->second;
-            given_clips.erase(it);
-            source = clip_description(videos_path_of(videos, name), v);
-        } else if (!(v.frames = video_frame_files(assets, path)).empty()) {   // video_png/<stem>/
-            source = std::to_string(v.frames.size()) + " PNG frames in " + v.frames[0].substr(0, v.frames[0].rfind('/'));
-        } else {                                                         // <assets>/video_y4m/<stem>.y4m
-            char rel[1024];
-            const int n = ph_video_frames_dir(path, rel, sizeof rel);
-            const std::string stem = n > 0 ? std::string(rel).substr(std::string(rel).find('/') + 1) : std::string();
-            const std::string clip = (assets.empty() ? std::string() : assets + "/") + "video_y4m/" + stem + ".y4m";
+        // reload_textures (main.rs:1066-1085): every texture of the scene from its stored path; a failure is reported, the render goes on
+        for (int k = 0;; k++) {
+            const char *name = nullptr, *path = nullptr;
+            if (ph_scene_texture(sc, k, &name, &path)) break;
+            if (given.count(name)) continue;
+            const std::string file = assets.empty() || (path[0] == '/') ? std::string(path) : assets + "/" + path;
             std::string why;
-            if (stem.empty() || !file_exists(clip)) continue;
-            if (!open_clip(v, clip, video_matrix, why)) { std::fprintf(stderr, "video `%s`: %s (the sampler is not updated)\n", name, why.c_str()); continue; }
-            source = clip_description(clip, v);
+            if (!set_texture_decoded(ctx, name, decode_png_once(decoded, file), why) && first)
+                std::fprintf(stderr, "texture `%s`: %s (the sampler stays unbound)\n", name, why.c_str());
         }
-        v.video = k;
-        v.name = name;
-        if (v.clip && pe_host_malloc(ctx, v.planes_bytes, &v.planes)) { std::fprintf(stderr, "%s\n", pe_last_error(ctx)); return 1; }
-        std::fprintf(status, "video `%s`: %s\n", name, source.c_str());
-        video_state.videos.push_back(v);
+        if (pe_scene_compile(ctx)) { std::fprintf(stderr, "%s\n", pe_last_error(ctx)); return 1; }
+        ph_player_attach(player, ctx);  // camera teleportation goes through pe_probe_ray
+        // VideoRuntime::from_scene (main.rs:820-858): videos that have a path, a uniform and frames on disk
+        VideoState& video_state = wk.video_state;
+        video_state.scene = sc;
+        video_state.ctx = ctx;
+        for (int k = 0;; k++) {
+            const char *name = nullptr, *path = nullptr, *uniform = nullptr;
+            if (ph_scene_video(sc, k, &name, &path, &uniform)) break;
+            if (!path[0] || !uniform[0]) continue;
+            VideoRuntime v;
+            std::string source;
+            auto it = given_clips.find(name);
+            if (given_video_names.count(name)) {                             // --video
+                const std::string given_path = videos_path_of(videos, name);
+                std::string why;
+                if (first && it != given_clips.end()) {
+                    v = it->second;
+                    given_clips.erase(it);
+                } else if (!open_clip(v, given_path, video_matrix, why, true)) {  // each worker reads with a handle of its own
+                    std::fprintf(stderr, "--video %s=%s: %s\n", name, given_path.c_str(), why.c_str());
+                    return 1;
+                }
+                source = clip_description(given_path, v);
+            } else if (!(v.frames = video_frame_files(assets, path)).empty()) {   // video_png/<stem>/
+                source = std::to_string(v.frames.size()) + " PNG frames in " + v.frames[0].substr(0, v.frames[0].rfind('/'));
+            } else {                                                         // <assets>/video_y4m/<stem>.y4m
+                char rel[1024];
+                const int n = ph_video_frames_dir(path, rel, sizeof rel);
+                const std::string stem = n > 0 ? std::string(rel).substr(std::string(rel).find('/') + 1) : std::string();
+                const std::string clip = (assets.empty() ? std::string() : assets + "/") + "video_y4m/" + stem + ".y4m";
+                std::string why;
+                if (stem.empty() || !file_exists(clip)) continue;
+                if (!open_clip(v, clip, video_matrix, why, !first)) {
+                    if (first) std::fprintf(stderr, "video `%s`: %s (the sampler is not updated)\n", name, why.c_str());
+                    continue;
+                }
+                source = clip_description(clip, v);
+            }
+            v.video = k;
+            v.name = name;
+            if (v.clip && pe_host_malloc(ctx, v.planes_bytes, &v.planes)) { std::fprintf(stderr, "%s\n", pe_last_error(ctx)); return 1; }
+            if (first) std::fprintf(status, "video `%s`: %s\n", name, source.c_str());
+            video_state.videos.push_back(v);
+        }
+        if (first)
+            for (auto& kv : given_clips) ph_y4m_close(kv.second.clip);   // a video without a path or a uniform plays nothing
+        if (!video_state.videos.empty()) ph_player_set_update_hook(player, update_videos, &video_state);
+        if (stereo) ph_player_set_stereo(player, 1, 0.07, 0);         // `render --stereo-image` (main.rs:2809-2816, 2842)
+        return 0;
+    };
+    for (size_t w = 0; w < workers.size(); w++) {
+        if (!workers[w].scene) { std::fprintf(stderr, "Failed to parse scene `%s`: %s\n", scene_path.c_str(), err); return 1; }
+        if (const int rc = set_up(workers[w], w == 0)) return rc;
     }
-    for (auto& kv : given_clips) ph_y4m_close(kv.second.clip);       // a video without a path or a uniform plays nothing
-    if (!video_state.videos.empty()) ph_player_set_update_hook(player, update_videos, &video_state);
-    if (stereo) {                   // `render --stereo-image`: side-by-side eyes, doubled width (main.rs:2809-2816, 2842)
-        width *= 2;
-        ph_player_set_stereo(player, 1, 0.07, 0);
-    }
+    if (stereo) width *= 2;         // side-by-side eyes, doubled width
     const bool png = frame_cmd ? ends_with(output, ".png") : frame_ext == ".png";       // Image::export_png (main.rs:2939-2943)
-    // one buffer for the frame: RGBA8 / RGBA16 pixels, a PNG file of at most pe_png_bound(_rgba16) bytes, or Y'CbCr planes
+    // one buffer per worker for the frame: RGBA8 / RGBA16 pixels, a PNG file of at most pe_png_bound(_rgba16) bytes, or Y'CbCr
+    // planes (`render` to Y4M: two, which travel to the main thread and back)
     const bool b16 = bits == 16;
-    std::vector<uint8_t> px(png ? (b16 ? pe_png_bound_rgba16(width, height) : pe_png_bound(width, height))
-                            : y4m ? pe_yuv420p10_bytes(width, height) : size_t(width) * size_t(height) * (b16 ? 8 : 4));
-    if (px.empty()) { std::fprintf(stderr, "no %s for a %d x %d frame\n", y4m ? "Y4M stream" : "PNG", width, height); return 1; }
-    size_t png_len = 0;
-    uint16_t* px16 = reinterpret_cast<uint16_t*>(px.data());
-    auto write_frame = [&](const std::string& name) {
-        return png ? write_bytes(name, px, png_len) : b16 ? write_image16(name, px, width, height) : write_image(name, px, width, height);
+    const size_t frame_bytes = png ? (b16 ? pe_png_bound_rgba16(width, height) : pe_png_bound(width, height))
+                                   : y4m ? pe_yuv420p10_bytes(width, height) : size_t(width) * size_t(height) * (b16 ? 8 : 4);
+    if (!frame_bytes) { std::fprintf(stderr, "no %s for a %d x %d frame\n", y4m ? "Y4M stream" : "PNG", width, height); return 1; }
+    for (Worker& wk : workers) {
+        if (anim_cmd && y4m) wk.free_planes.assign(2, std::vector<uint8_t>(frame_bytes));
+        else wk.px.resize(frame_bytes);
+    }
+    auto write_frame = [&](Worker& wk, const std::string& name) {
+        return png ? write_bytes(name, wk.px, wk.png_len) : b16 ? write_image16(name, wk.px, width, height) : write_image(name, wk.px, width, height);
     };
     ph_frame_params p = {width, height, depth, aa, 0, 0, {0, 0, 0}, 0, 0, 0};
+    int exit_code = 0;
     if (frame_cmd) {
-        if (ph_player_update(player, time) ||                                                          // main.rs:2928-2929
-            (png ? (b16 ? ph_player_render_frame_png16 : ph_player_render_frame_png)(player, ctx, &p, px.data(), px.size(), &png_len)
-                 : y4m ? ph_player_render_frame_yuv420p10(player, ctx, &p, bits, px16)
-                 : b16 ? ph_player_render_frame_rgba16(player, ctx, &p, px16) : ph_player_render_frame(player, ctx, &p, px.data(), 1))) {
-            std::fprintf(stderr, "%s\n", ph_player_last_error(player));
+        Worker& wk = workers[0];
+        uint16_t* px16 = reinterpret_cast<uint16_t*>(wk.px.data());
+        if (ph_player_update(wk.player, time) ||                                                          // main.rs:2928-2929
+            (png ? (b16 ? ph_player_render_frame_png16 : ph_player_render_frame_png)(wk.player, wk.ctx, &p, wk.px.data(), wk.px.size(), &wk.png_len)
+                 : y4m ? ph_player_render_frame_yuv420p10(wk.player, wk.ctx, &p, bits, px16)
+                 : b16 ? ph_player_render_frame_rgba16(wk.player, wk.ctx, &p, px16) : ph_player_render_frame(wk.player, wk.ctx, &p, wk.px.data(), 1))) {
+            std::fprintf(stderr, "%s\n", ph_player_last_error(wk.player));
             return 1;
         }
         bool written = false;
         if (y4m) {
             if (FILE* f = std::fopen(output.c_str(), "wb")) {
-                written = write_y4m_header(f, width, height, 25) && write_y4m_frame(f, px);
+                written = write_y4m_header(f, width, height, 25) && write_y4m_frame(f, wk.px);
                 written = std::fclose(f) == 0 && written;
             }
         } else {
-            written = write_frame(output);
+            written = write_frame(wk, output);
         }
         if (!written) { std::fprintf(stderr, "cannot write %s\n", output.c_str()); return 1; }
         std::printf("Rendered `%s` to `%s`\n", scene_path.c_str(), output.c_str());
     } else {
+        // The plan: every skip decision from one snapshot of the output, taken now, plus what the animations before each one
+        // will write (a name listed twice), so that the decisions are the sequential loop's and no worker's write can change
+        // another's
+        std::vector<AnimationPlan> plan(names.size());
+        std::set<std::string> to_write;
         for (size_t k = 0; k < names.size(); k++) {
-            if (ph_player_init_animation(player, names[k].c_str())) {
-                std::fprintf(stderr, "Scene `%s` has no animation named `%s`\n", scene_path.c_str(), names[k].c_str());
-                return 1;
-            }
-            if (ph_player_update(player, 0.0)) { std::fprintf(stderr, "%s\n", ph_player_last_error(player)); return 1; }
-            double duration = 0.0;
-            for (int a = 0; a < ph_scene_animation_count(scene); a++) {
+            AnimationPlan& a = plan[k];
+            for (int i = 0; i < ph_scene_animation_count(scene); i++) {
                 const char* nm = nullptr;
                 double d = 0.0;
-                if (ph_scene_animation(scene, a, &nm, &d) == 0 && names[k] == nm) duration = d;
+                if (ph_scene_animation(scene, i, &nm, &d) == 0 && names[k] == nm) a.duration = d;
             }
-            if (all && !starts_with.empty() && names[k].compare(0, starts_with.size(), starts_with) != 0) continue;
+            a.rendered = !(all && !starts_with.empty() && names[k].compare(0, starts_with.size(), starts_with) != 0);
+            const float duration32 = float(a.duration);                                        // render_animation takes f32
+            a.duration = double(duration32);
+            a.count = int(duration32 * float(fps));                                             // main.rs:1785
+            if (a.count < 1) a.count = 1;
+            a.todo = max_frames >= 0 && max_frames < a.count ? max_frames : a.count;
+            a.skip_frame.assign(size_t(a.todo), 0);
+            if (!a.rendered || to_stdout) continue;
+            if (y4m) {
+                const std::string stream = out_dir + "/" + names[k] + ".y4m";
+                a.skip_stream = skip_existing && (file_exists(stream) || to_write.count(stream));     // main.rs:1771-1779
+                if (!a.skip_stream) to_write.insert(stream);
+                continue;
+            }
+            for (int i = 0; i < a.todo; i++) {
+                const std::string f = out_dir + "/" + names[k] + "/frame_" + std::to_string(i) + frame_ext;
+                a.skip_frame[size_t(i)] = skip_existing && (file_exists(f) || to_write.count(f));   // resumes like main.rs:1789-1793
+                if (!a.skip_frame[size_t(i)]) to_write.insert(f);
+            }
+        }
+        Shared sh;
+        // A worker runs the whole loop.  It renders frame i of an animation when i mod N is its number and advances through
+        // the others, so its player's state at every frame is the sequential one (camera teleportation carries over).
+        auto run_worker = [&](size_t me) {
+            Worker& wk = workers[me];
+            for (size_t k = 0; k < names.size(); k++) {
+                if (sh.stopped()) return;
+                if (ph_player_init_animation(wk.player, names[k].c_str())) {
+                    sh.fail("Scene `" + scene_path + "` has no animation named `" + names[k] + "`");
+                    return;
+                }
+                if (ph_player_update(wk.player, 0.0)) { sh.fail(ph_player_last_error(wk.player)); return; }
+                const AnimationPlan& a = plan[k];
+                if (!a.rendered) continue;
+                if (me == 0) sh.post(k, -1, {});
+                if (y4m && a.skip_stream) continue;
+                const std::string dir = out_dir + "/" + names[k];
+                if (!y4m && !make_dirs(dir)) { sh.fail("cannot create " + dir); return; }
+                for (int i = 0; i < a.todo; i++) {
+                    if (sh.stopped()) return;
+                    if (a.skip_frame[size_t(i)]) continue;                 // neither rendered nor advanced, as the sequential loop
+                    if (size_t(i) % workers.size() != me) {
+                        if (ph_player_advance_motion_blur_frame(wk.player, i, a.count, motion_blur, a.duration)) { sh.fail(ph_player_last_error(wk.player)); return; }
+                        continue;
+                    }
+                    if (y4m) {
+                        std::vector<uint8_t> planes;
+                        if (!sh.take_buffer(wk, planes)) return;
+                        if (ph_player_render_motion_blur_frame_yuv420p10(wk.player, wk.ctx, &p, i, a.count, motion_blur, a.duration, bits,
+                                                                         reinterpret_cast<uint16_t*>(planes.data()))) {
+                            sh.fail(ph_player_last_error(wk.player));
+                            return;
+                        }
+                        sh.post(k, i, std::move(planes));
+                        continue;
+                    }
+                    uint16_t* px16 = reinterpret_cast<uint16_t*>(wk.px.data());
+                    const double dur = a.duration;
+                    if (png ? (b16 ? ph_player_render_motion_blur_frame_png16 : ph_player_render_motion_blur_frame_png)(wk.player, wk.ctx, &p, i, a.count, motion_blur, dur, wk.px.data(), wk.px.size(), &wk.png_len)
+                            : b16 ? ph_player_render_motion_blur_frame_rgba16(wk.player, wk.ctx, &p, i, a.count, motion_blur, dur, px16)
+                                  : ph_player_render_motion_blur_frame(wk.player, wk.ctx, &p, i, a.count, motion_blur, dur, wk.px.data())) {
+                        sh.fail(ph_player_last_error(wk.player));
+                        return;
+                    }
+                    const std::string name = dir + "/frame_" + std::to_string(i) + frame_ext;
+                    if (!write_frame(wk, name)) { sh.fail("cannot write " + name); return; }
+                    sh.post(k, i, {});
+                }
+            }
+        };
+        std::vector<std::thread> threads;
+        for (size_t w = 0; w < workers.size(); w++) threads.emplace_back(run_worker, w);
+        // The main thread: status lines and Y4M streams, in frame order
+        std::vector<uint8_t> planes;
+        for (size_t k = 0; k < names.size(); k++) {
+            const AnimationPlan& a = plan[k];
+            if (!a.rendered) continue;
+            if (!sh.take(k, -1, planes)) break;
             std::fprintf(status, "Rendering animation %s, %zu/%zu\n", names[k].c_str(), k + 1, names.size());
-            const float duration32 = float(duration);                                          // render_animation takes f32
-            int count = int(duration32 * float(fps));                                           // main.rs:1785
-            if (count < 1) count = 1;
-            const int todo = max_frames >= 0 && max_frames < count ? max_frames : count;
+            bool stopped = false;
             if (y4m) {
                 // one stream per animation, written under a temporary name and renamed when complete, so that an interrupted
                 // run leaves no stream for skip-existing to take as done
                 const std::string stream = out_dir + "/" + names[k] + ".y4m", part = stream + ".part";
-                if (!to_stdout && skip_existing && file_exists(stream)) {               // main.rs:1771-1779
+                if (a.skip_stream) {
                     std::fprintf(status, "Skip `%s`, because it's already exists\n", names[k].c_str());
                     continue;
                 }
-                if (!to_stdout && !make_dirs(out_dir)) { std::fprintf(stderr, "cannot create %s\n", out_dir.c_str()); return 1; }
+                if (!to_stdout && !make_dirs(out_dir)) { sh.fail("cannot create " + out_dir); break; }
                 FILE* f = to_stdout ? stdout : std::fopen(part.c_str(), "wb");
                 bool ok_stream = f && write_y4m_header(f, width, height, fps);
-                for (int i = 0; i < todo && ok_stream; i++) {
-                    if (ph_player_render_motion_blur_frame_yuv420p10(player, ctx, &p, i, count, motion_blur, double(duration32), bits, px16)) {
-                        std::fprintf(stderr, "%s\n", ph_player_last_error(player));
-                        return 1;
-                    }
-                    ok_stream = write_y4m_frame(f, px);
-                    std::fprintf(status, "\r%d/%d done      ", i + 1, count);
+                for (int i = 0; i < a.todo && ok_stream; i++) {
+                    if (!sh.take(k, i, planes)) { stopped = true; break; }
+                    ok_stream = write_y4m_frame(f, planes);
+                    sh.give_back(workers[size_t(i) % workers.size()], planes);
+                    std::fprintf(status, "\r%d/%d done      ", i + 1, a.count);
                     std::fflush(status);
                 }
                 if (f) ok_stream = (to_stdout ? std::fflush(f) : std::fclose(f)) == 0 && ok_stream;
+                if (stopped) break;                                        // the stream keeps its .part name
                 if (!ok_stream || (!to_stdout && std::rename(part.c_str(), stream.c_str()) != 0)) {
-                    std::fprintf(stderr, "cannot write %s\n", to_stdout ? "the stream to stdout" : stream.c_str());
-                    return 1;
+                    sh.fail(std::string("cannot write ") + (to_stdout ? "the stream to stdout" : stream.c_str()));
+                    break;
                 }
                 std::fprintf(status, "\n");
                 continue;
             }
-            const std::string dir = out_dir + "/" + names[k];
-            if (!make_dirs(dir)) { std::fprintf(stderr, "cannot create %s\n", dir.c_str()); return 1; }
-            for (int i = 0; i < todo; i++) {
-                if (skip_existing && file_exists(dir + "/frame_" + std::to_string(i) + frame_ext)) continue;   // resumes like main.rs:1789-1793
-                const double dur = double(duration32);
-                if (png ? (b16 ? ph_player_render_motion_blur_frame_png16 : ph_player_render_motion_blur_frame_png)(player, ctx, &p, i, count, motion_blur, dur, px.data(), px.size(), &png_len)
-                        : b16 ? ph_player_render_motion_blur_frame_rgba16(player, ctx, &p, i, count, motion_blur, dur, px16)
-                              : ph_player_render_motion_blur_frame(player, ctx, &p, i, count, motion_blur, dur, px.data())) {
-                    std::fprintf(stderr, "%s\n", ph_player_last_error(player));
-                    return 1;
-                }
-                const std::string name = dir + "/frame_" + std::to_string(i) + frame_ext;
-                if (!write_frame(name)) { std::fprintf(stderr, "cannot write %s\n", name.c_str()); return 1; }
-                std::printf("\r%d/%d done      ", i + 1, count);
-                std::fflush(stdout);
+            for (int i = 0; i < a.todo && !stopped; i++) {
+                if (a.skip_frame[size_t(i)]) continue;
+                if (!sh.take(k, i, planes)) { stopped = true; break; }
+                std::fprintf(status, "\r%d/%d done      ", i + 1, a.count);
+                std::fflush(status);
             }
-            std::printf("\n");
+            if (stopped) break;
+            std::fprintf(status, "\n");
+        }
+        for (std::thread& t : threads) t.join();
+        if (sh.stop) {
+            std::fprintf(stderr, "%s\n", sh.error.c_str());
+            exit_code = 1;
         }
     }
-    for (VideoRuntime& v : video_state.videos) {
-        if (v.planes) pe_host_free(ctx, v.planes);
-        ph_y4m_close(v.clip);
+    for (Worker& wk : workers) {
+        for (VideoRuntime& v : wk.video_state.videos) {
+            if (v.planes) pe_host_free(wk.ctx, v.planes);
+            ph_y4m_close(v.clip);
+        }
+        ph_player_free(wk.player);
+        pe_destroy(wk.ctx);
+        ph_scene_free(wk.scene);
     }
-    ph_player_free(player);
-    pe_destroy(ctx);
-    ph_scene_free(scene);
-    return 0;
+    return exit_code;
 }
+

@@ -34,7 +34,7 @@ struct PeLaunchHost {  // must match `PeLaunch` in device/pe_kernel.cuh
 };
 static_assert(sizeof(PeLaunchHost) == 72, "PeLaunch layout");
 
-std::string g_create_error;
+thread_local std::string g_create_error;     // per thread: another thread's pe_create cannot rewrite it under a reader
 std::mutex g_create_mutex;
 
 bool cuda_ok(pe_ctx* c, cudaError_t e, const char* what) {

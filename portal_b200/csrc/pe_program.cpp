@@ -5,6 +5,7 @@
 #include <sys/stat.h>
 #include <unistd.h>
 
+#include <atomic>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -152,7 +153,10 @@ bool compile_cubin(pe_ctx* c, const std::string& source, std::vector<char>& cubi
     N.GetCUBIN(prog, cubin.data());
     N.DestroyProgram(&prog);
     {
-        std::string tmp = path + ".tmp" + std::to_string((long long)getpid());
+        // private to this write: several processes, and several threads of one (portal_b200_render --devices 0,0), may
+        // compile the same variant at once
+        static std::atomic<unsigned long long> writes{0};
+        std::string tmp = path + ".tmp" + std::to_string((long long)getpid()) + "." + std::to_string(writes.fetch_add(1));
         std::ofstream f(tmp, std::ios::binary);
         if (f) {
             f.write(cubin.data(), std::streamsize(cubin.size()));

@@ -260,6 +260,12 @@ class HostPlayer:
                                                                  motion_blur_frames, float(duration_seconds), out.ctypes.data))
         return out
 
+    def advance_motion_blur_frame(self, frame_index, frame_count, motion_blur_frames, duration_seconds):
+        """The sub-frame updates of render_motion_blur_frame (same times, order and probes) without the update hook, the
+        uniform upload or the render: keeps a player that skips a frame in the state the frame leaves behind."""
+        self._check(self._lib.ph_player_advance_motion_blur_frame(self._p, int(frame_index), int(frame_count),
+                                                                  int(motion_blur_frames), float(duration_seconds)))
+
     def render_frame_rgba16(self, width, height, depth, aa_count=1, aa_start=0) -> np.ndarray:
         """The frame of render_frame as unorm16 (uint16 [h, w, 4]): the float frame quantised by pe_quantize_rgba16."""
         p = PhFrameParams(width, height, depth, aa_count, aa_start, 0)
