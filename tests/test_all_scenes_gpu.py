@@ -2,34 +2,19 @@
 C ABI and held, bit for bit, to the strict oracle's frame -- by sha256 of the float frame, so that the 81 checkers need not
 travel (tools/export_all_scenes.py wrote tests/golden/scenes_all/ from /root/reference in the build container).  Scenes that
 call exp / log / pow are in here like the rest: those functions are part of the pinned numeric profile (DESIGN.md section 4).
-On a mismatch the oracle is built on the spot to say how many pixels differ."""
-import gzip
+On a mismatch the oracle is built on the spot to say how many pixels differ.  tests/test_all_scenes_shapes_gpu.py holds
+the same scenes in the product's other kernel shapes."""
 import hashlib
-import json
-import os
 
 import numpy as np
 import pytest
 
-from conftest import GOLDEN
+from helpers.scenes_all import load_pins, load_scene
 
 pytestmark = pytest.mark.gpu
 
-ALL = os.path.join(GOLDEN, "scenes_all")
-with open(os.path.join(ALL, "sha256.json")) as _f:
-    PINS = json.load(_f)
+PINS = load_pins()
 W, H, DEPTH = PINS["width"], PINS["height"], PINS["depth"]
-
-
-def load_scene(name):
-    with gzip.open(os.path.join(ALL, f"{name}.scene.json.gz"), "rb") as f:
-        ir = json.loads(f.read().decode())
-    tex = {}
-    if ir["textures"]:
-        with np.load(os.path.join(ALL, "textures.npz")) as z:
-            for t in ir["textures"]:
-                tex[t["name"]] = np.ascontiguousarray(z[t["path"].replace("/", "__").replace(".", "_")])
-    return ir, tex
 
 
 @pytest.mark.parametrize("name", sorted(PINS["frames"]))
