@@ -136,8 +136,8 @@ PE_API int ph_player_select_camera(ph_player* p, const char* camera_name);
 /* SceneRenderer::update(memory, time): `time_seconds` is wall time; inside a real animation the formula
  * variable `time` becomes (time % duration) / duration and `total_time` adds the earlier animations. */
 PE_API int ph_player_update(ph_player* p, double time_seconds);
-/* Called after every update the player performs -- ph_player_update and each motion-blur sub-frame of
- * ph_player_render_motion_blur_frame -- before the frame's uniforms are uploaded: the place of SceneRenderer::update's tail
+/* Called after every update the player performs -- ph_player_update and each sub-frame of a motion-blurred frame --
+ * before the frame's uniforms are uploaded: the place of SceneRenderer::update's tail
  * (src/main.rs:1536-1542), where the reference swaps in the current frame of every video (ph_scene_video_frame + pe_set_texture).
  * Non-zero return aborts the call.  NULL removes the hook. */
 typedef int (*ph_update_hook)(void* user);
@@ -169,67 +169,49 @@ PE_API int ph_scene_animation_count(ph_scene* s);
 PE_API int ph_scene_animation(ph_scene* s, int k, const char** name, double* duration);
 PE_API int ph_scene_camera_count(ph_scene* s);
 PE_API int ph_scene_camera_name(ph_scene* s, int k, const char** name);
-/* draw_texture + readback with the player's camera and the scene's current uniforms (width, height, depth,
- * aa_count, aa_start of `p` are used; its camera fields are ignored). */
-PE_API int ph_player_render_frame(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, void* out_host, int rgba8);
-/* One output frame of render_animation (src/main.rs:1786-1817) inside the player's current animation: every
- * sub-frame j calls update(t_j * duration_seconds) -- time mapping, camera interpolation, teleportation --
- * renders with `_aa_start` = j into an RGBA8 target, and the sub-frames are averaged in gamma-2 space. */
-PE_API int ph_player_render_motion_blur_frame(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index,
-                                              int frame_count, int motion_blur_frames, double duration_seconds,
-                                              uint8_t* out_host_rgba8);
-/* The player state of ph_player_render_motion_blur_frame* without the frame: exactly the same sub-frame updates -- the same
- * times t_j * duration_seconds, in the same order, with the same probes through the attached context or probe function --
- * and the same refusal of bad arguments, but no update hook, no uniform upload and no render.  A caller that deals the
- * frames of one animation out to several players (`portal_b200_render render --devices`) advances every player through the
- * frames it does not render, so that each one's camera, teleport matrix and subspace flag at frame i are the sequential
- * ones.  Skipping the hook is safe when, as in the render CLI's video hook, what the hook binds is derived from the scene's
- * current state alone: the next update that does call it binds the right frame. */
+/* ---- the player's frames: one call for every output format
+ * draw_texture + readback with the player's camera and the scene's current uniforms (width, height, depth, aa_count, aa_start of
+ * `p` are used; its camera fields are ignored), stereo, adaptive anti-aliasing and the update hook included, in three steps:
+ * - stage the frame on the device at `bits` 8 (RGBA8), 16 (float RGBA quantised to unorm16 by pe_quantize_rgba16; opt-in, for
+ *   10-bit video encodes -- the reference's frames are 8-bit) or 32 (float RGBA; PH_OUT_PIXELS without motion blur only): one
+ *   frame at the player's current update (`mb` NULL), or one motion-blurred frame of the current animation (ph_motion_blur);
+ * - convert it to `container`: none, a PNG file (pe_encode_png_rgba8 / _rgba16, into the context's own file buffer) or
+ *   Y'CbCr 4:2:0 planes at 10 bits (pe_rgba_to_yuv420p10, DESIGN.md section 5.4: Y, then Cb, then Cr);
+ * - read it back into out_host (capacity >= ph_output_bytes), *len bytes.  Pixels and planes are in host byte order.
+ * Any other combination, bad motion-blur arguments or a short capacity are refused before any launch.
+ * Scratch slots (pe_scratch_buffer) of the context, with M sub-frames (0 without motion blur): slot 0 holds the frame, slots
+ * 1 .. M the sub-frames, at 16 bits the next slot the floats each (sub-)frame is rendered into, and the next free slot the
+ * Y'CbCr planes.  At 16 bits that is 8 (M + 1) + 16 bytes per pixel before the planes, 17.8 GB at 7680 x 4320 with M = 64.
+ * A single frame of RGBA8 or float pixels without adaptive anti-aliasing is rendered straight into host memory
+ * (pe_render_host_rgba8 / pe_render_host) and uses no slot. */
+enum { PH_OUT_PIXELS = 0, PH_OUT_PNG = 1, PH_OUT_YUV420P10 = 2 };
+/* One output frame of render_animation (src/main.rs:1786-1817): sub-frame j of frame `frame_index` (of `frame_count`) calls
+ * update(t_j * duration_seconds), t_j = frame_index/frame_count + j/motion_blur_frames/frame_count * 0.5 -- time mapping,
+ * camera interpolation, teleportation and the update hook --, renders with `_aa_start` = j, and the sub-frames are averaged
+ * in gamma-2 space (average_images, src/main.rs:664-722; at 16 bits in exact integers, DESIGN.md section 5.3).
+ * 1 <= motion_blur_frames <= 64. */
+typedef struct ph_motion_blur {
+    int32_t frame_index, frame_count, motion_blur_frames;
+    double duration_seconds;
+} ph_motion_blur;
+/* The capacity a `container` of a width x height frame at `bits` needs: w * h * bits / 2 (pixels), pe_png_bound /
+ * pe_png_bound_rgba16 (PNG), pe_yuv420p10_bytes (Y'CbCr); 0 when there is no such output. */
+PE_API size_t ph_output_bytes(int container, int bits, int width, int height);
+PE_API int ph_player_render(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, const ph_motion_blur* mb, int container,
+                            int bits, void* out_host, size_t capacity, size_t* len);
+/* The player's state of a motion-blurred frame without the frame: exactly the same sub-frame updates -- the same times
+ * t_j * duration_seconds, in the same order, with the same probes through the attached context or probe function -- and the
+ * same refusal of bad arguments, but no update hook, no uniform upload and no render.  A caller that deals the frames of one
+ * animation out to several players (`portal_b200_render render --devices`) advances every player through the frames it does
+ * not render, so that each one's camera, teleport matrix and subspace flag at frame i are the sequential ones.  Skipping the
+ * hook is safe when, as in the render CLI's video hook, what the hook binds is derived from the scene's current state alone:
+ * the next update that does call it binds the right frame. */
 PE_API int ph_player_advance_motion_blur_frame(ph_player* pl, int frame_index, int frame_count, int motion_blur_frames,
                                                double duration_seconds);
-/* Adaptive anti-aliasing for the player's frames (off by default): when on, ph_player_render_frame and every sub-frame of
- * ph_player_render_motion_blur_frame (before the unchanged gamma-2 average) are rendered by pe_render_adaptive with
- * `threshold` -- one sample everywhere, all aa_count samples where the one-sample frame has an edge.  ph_player_render_frame
- * then stages the frame in the context's scratch slot 0.  The scene-level ph_render_* functions are not affected. */
+/* Adaptive anti-aliasing for the player's frames (off by default): when on, every frame and motion-blur sub-frame (before the
+ * unchanged gamma-2 average) is rendered by pe_render_adaptive with `threshold` -- one sample everywhere, all aa_count samples
+ * where the one-sample frame has an edge.  The scene-level ph_render_* functions are not affected. */
 PE_API int ph_player_set_adaptive_aa(ph_player* pl, int on, int threshold);
-/* PNG twins of ph_player_render_frame (RGBA8) and ph_player_render_motion_blur_frame: the same frame, rendered the same way
- * (adaptive anti-aliasing, stereo and the update hook included), encoded on the device by pe_encode_png_rgba8 instead of
- * read back.  The file (*len bytes) goes into `png` (capacity >= pe_png_bound(width, height)).  The frame is staged in the
- * context's scratch slot 0; the motion-blur sub-frames use slots 1 .. motion_blur_frames, as in the RGBA8 twin. */
-PE_API int ph_player_render_frame_png(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, uint8_t* png, size_t capacity,
-                                      size_t* len);
-PE_API int ph_player_render_motion_blur_frame_png(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index,
-                                                  int frame_count, int motion_blur_frames, double duration_seconds,
-                                                  uint8_t* png, size_t capacity, size_t* len);
-/* 16-bit twins (opt-in, for 10-bit video encodes; the reference's frames are 8-bit): the same frame, rendered the same way
- * (adaptive anti-aliasing, stereo and the update hook included) but as floats -- pe_render, or pe_render_adaptive with rgba8 = 0
- * -- and quantised by pe_quantize_rgba16 instead of to unorm8.  The motion-blur twins run the same sub-frame loop (time,
- * `_aa_start` = j, update, upload) with RGBA16 sub-frames averaged by pe_average_frames_rgba16.  Output: RGBA16 pixels
- * (w * h * 4 uint16, host byte order) or a 16-bit PNG encoded by pe_encode_png_rgba16 (capacity >= pe_png_bound_rgba16).
- * Scratch slots: the frame is staged as RGBA16 in slot 0.  Single frames render their floats into slot 1.  Motion blur with
- * M sub-frames keeps them in slots 1 .. M (8 B per pixel each) and renders each one's floats into slot M + 1 (16 B per pixel):
- * 8 * (M + 1) + 16 bytes per pixel, 17.8 GB (16.6 GiB) at 7680 x 4320 with M = 64 (the RGBA8 path: 4 * (M + 1)). */
-PE_API int ph_player_render_frame_rgba16(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, uint16_t* out_host_rgba16);
-PE_API int ph_player_render_frame_png16(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, uint8_t* png, size_t capacity,
-                                        size_t* len);
-PE_API int ph_player_render_motion_blur_frame_rgba16(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index,
-                                                     int frame_count, int motion_blur_frames, double duration_seconds,
-                                                     uint16_t* out_host_rgba16);
-PE_API int ph_player_render_motion_blur_frame_png16(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index,
-                                                    int frame_count, int motion_blur_frames, double duration_seconds,
-                                                    uint8_t* png, size_t capacity, size_t* len);
-/* Y'CbCr 4:2:0 10-bit twins (DESIGN.md section 5.4): the frame exactly as the RGBA8 twin (`bits` 8: ph_player_render_frame with
- * rgba8 = 1, ph_player_render_motion_blur_frame) or the RGBA16 twin (`bits` 16) renders it -- adaptive anti-aliasing, stereo and
- * the update hook included -- converted on the device by pe_rgba_to_yuv420p10; only the planes are read back, into `out_host`
- * (pe_yuv420p10_bytes(width, height) bytes: Y, then Cb, then Cr).  Scratch slots: the frame is staged in slot 0 as in the
- * twins (a single RGBA8 frame is always staged there; single RGBA16 frames render their floats into slot 1; motion blur with M
- * sub-frames keeps them in slots 1 .. M, and at 16 bits renders their floats into slot M + 1).  The planes go into the first
- * slot after those: 1 (single frame, 8 bits), 2 (single frame, 16 bits), M + 1 (motion blur, 8 bits), M + 2 (motion blur,
- * 16 bits). */
-PE_API int ph_player_render_frame_yuv420p10(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int bits, uint16_t* out_host);
-PE_API int ph_player_render_motion_blur_frame_yuv420p10(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index,
-                                                        int frame_count, int motion_blur_frames, double duration_seconds, int bits,
-                                                        uint16_t* out_host);
 
 /* ---- image files either side of the path ------------------------------------------------------------------------
  * Textures reach the reference as PNG files (Texture2D::from_file_with_format, src/main.rs:1066-1085) and frames leave it as

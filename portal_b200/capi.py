@@ -31,6 +31,13 @@ class PhFrameParams(C.Structure):
                 ("beta", C.c_double), ("r", C.c_double)]
 
 
+class PhMotionBlur(C.Structure):
+    _fields_ = [("frame_index", C.c_int32), ("frame_count", C.c_int32), ("motion_blur_frames", C.c_int32),
+                ("duration_seconds", C.c_double)]
+
+
+PH_OUT_PIXELS, PH_OUT_PNG, PH_OUT_YUV420P10 = 0, 1, 2
+
 PE_YUV_BT709, PE_YUV_BT601 = 0, 1
 PE_YUV_SITING_LEFT, PE_YUV_SITING_CENTER = 0, 1
 MATRICES = {"bt709": PE_YUV_BT709, "bt601": PE_YUV_BT601}
@@ -205,26 +212,17 @@ def lib() -> C.CDLL:
         "ph_scene_animation": (i32, [vp, i32, C.POINTER(cp), f64p]),
         "ph_scene_camera_count": (i32, [vp]),
         "ph_scene_camera_name": (i32, [vp, i32, C.POINTER(cp)]),
-        "ph_player_render_frame": (i32, [vp, vp, C.POINTER(PhFrameParams), vp, i32]),
-        "ph_player_render_motion_blur_frame": (i32, [vp, vp, C.POINTER(PhFrameParams), i32, i32, i32, C.c_double, vp]),
+        "ph_output_bytes": (C.c_size_t, [i32, i32, i32, i32]),
+        "ph_player_render": (i32, [vp, vp, C.POINTER(PhFrameParams), C.POINTER(PhMotionBlur), i32, i32, vp, C.c_size_t,
+                                   C.POINTER(C.c_size_t)]),
         "ph_player_advance_motion_blur_frame": (i32, [vp, i32, i32, i32, C.c_double]),
         "ph_player_set_adaptive_aa": (i32, [vp, i32, i32]),
-        "ph_player_render_frame_png": (i32, [vp, vp, C.POINTER(PhFrameParams), vp, C.c_size_t, C.POINTER(C.c_size_t)]),
-        "ph_player_render_motion_blur_frame_png": (i32, [vp, vp, C.POINTER(PhFrameParams), i32, i32, i32, C.c_double, vp, C.c_size_t,
-                                                         C.POINTER(C.c_size_t)]),
-        "ph_player_render_frame_rgba16": (i32, [vp, vp, C.POINTER(PhFrameParams), vp]),
-        "ph_player_render_frame_png16": (i32, [vp, vp, C.POINTER(PhFrameParams), vp, C.c_size_t, C.POINTER(C.c_size_t)]),
-        "ph_player_render_motion_blur_frame_rgba16": (i32, [vp, vp, C.POINTER(PhFrameParams), i32, i32, i32, C.c_double, vp]),
-        "ph_player_render_motion_blur_frame_png16": (i32, [vp, vp, C.POINTER(PhFrameParams), i32, i32, i32, C.c_double, vp, C.c_size_t,
-                                                           C.POINTER(C.c_size_t)]),
-        "ph_player_render_frame_yuv420p10": (i32, [vp, vp, C.POINTER(PhFrameParams), i32, vp]),
         "ph_y4m_open": (vp, [cp, i32, cp, C.c_size_t]),
         "ph_y4m_info": (i32, [vp, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(PeYuvFormat),
                               C.POINTER(C.c_int64)]),
         "ph_y4m_read_frame": (i32, [vp, C.c_int64, vp, C.c_size_t]),
         "ph_y4m_last_error": (cp, [vp]),
         "ph_y4m_close": (None, [vp]),
-        "ph_player_render_motion_blur_frame_yuv420p10": (i32, [vp, vp, C.POINTER(PhFrameParams), i32, i32, i32, C.c_double, i32, vp]),
     })
     for name, (res, args) in sig.items():
         fn = getattr(L, name)

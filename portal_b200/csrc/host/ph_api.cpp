@@ -99,6 +99,20 @@ int upload_renderer_uniforms_cam(ph_scene* s, pe_ctx* ctx, const ph_frame_params
     return 0;
 }
 
+// The sub-frame update times of one output frame of render_animation (main.rs:1786-1797): sub-frame j at t * duration_seconds,
+// t = frame_index / frame_count + j / motion_blur_frames / frame_count * exposure, exposure 0.5.  False on bad arguments.  Every
+// motion-blur path -- the scene's, the player's render and its advance -- takes its times here, so that they cannot drift apart.
+bool motion_blur_times(int frame_index, int frame_count, int motion_blur_frames, double duration_seconds, std::vector<double>& times) {
+    if (frame_count < 1 || motion_blur_frames < 1 || motion_blur_frames > 64 || frame_index < 0) return false;
+    const double exposure = 0.5;
+    times.resize(size_t(motion_blur_frames));
+    for (int j = 0; j < motion_blur_frames; j++) {
+        const double tt = double(frame_index) / double(frame_count) + double(j) / double(motion_blur_frames) / double(frame_count) * exposure;
+        times[size_t(j)] = tt * duration_seconds;
+    }
+    return true;
+}
+
 }  // namespace
 
 extern "C" {
@@ -338,7 +352,8 @@ int ph_render_target(ph_scene* s, pe_ctx* ctx, const ph_frame_params* p, const p
 int ph_render_motion_blur_frame(ph_scene* s, pe_ctx* ctx, const ph_frame_params* p, int frame_index, int frame_count,
                                 int motion_blur_frames, double duration_seconds, uint8_t* out_host) {
     if (!s || !ctx || !p || !out_host) return 1;
-    if (frame_count < 1 || motion_blur_frames < 1 || motion_blur_frames > 64 || frame_index < 0 || p->width <= 0 || p->height <= 0 ||
+    std::vector<double> times;
+    if (!motion_blur_times(frame_index, frame_count, motion_blur_frames, duration_seconds, times) || p->width <= 0 || p->height <= 0 ||
         p->width > 65536 || p->height > 65536)
         return fail(s, "ph_render_motion_blur_frame: bad frame arguments");
     const size_t n = size_t(p->width) * size_t(p->height);
@@ -350,13 +365,10 @@ int ph_render_motion_blur_frame(ph_scene* s, pe_ctx* ctx, const ph_frame_params*
     const double saved_time = s->scene.time, saved_total = s->scene.total_time;
     if (!rc) {
         pe_target t = {p->width, p->height, p->height, 0, 1, 1, 1};
-        const double exposure = 0.5;  // main.rs:1787
         for (int j = 0; j < motion_blur_frames && !rc; j++) {
-            const double tt = double(frame_index) / double(frame_count) +
-                              double(j) / double(motion_blur_frames) / double(frame_count) * exposure;
             ph_frame_params q = *p;
             q.aa_start = j;                                            // main.rs:1797
-            ph_scene_set_time(s, tt * duration_seconds, tt * duration_seconds);   // Scene::update, Dev/Animation stage branch
+            ph_scene_set_time(s, times[size_t(j)], times[size_t(j)]);  // Scene::update, Dev/Animation stage branch
             rc = upload_frame_uniforms(s, ctx, &q) ||
                  pe_render_rgba8(ctx, &t, sub[size_t(j)], nullptr);   // RGBA8 render target, quantised by the kernel
         }
@@ -567,46 +579,6 @@ static int upload_player_uniforms(ph_player* pl, pe_ctx* ctx, const ph_frame_par
     return upload_stereo_uniforms(pl, ctx);
 }
 
-// The frame into device memory `dev` (RGBA8 or float RGBA): adaptively when the player is set so.
-static int render_player_device(ph_player* pl, pe_ctx* ctx, const pe_target* t, int rgba8, void* dev) {
-    if (pl->adaptive_aa) return pe_render_adaptive(ctx, t, pl->adaptive_threshold, rgba8, dev, nullptr, nullptr);
-    return rgba8 ? pe_render_rgba8(ctx, t, dev, nullptr) : pe_render(ctx, t, dev, nullptr, nullptr);
-}
-
-int ph_player_render_frame(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, void* out_host, int rgba8) {
-    if (!pl || !ctx || !p || !out_host) return 1;
-    if (upload_player_uniforms(pl, ctx, p)) return 1;
-    pe_target t = {p->width, p->height, p->height, 0, 1, 1, 1};
-    int rc;
-    if (pl->adaptive_aa) {
-        // the frame lands in scratch slot 0 (reused by every frame) and is read back from there
-        const size_t bytes = size_t(p->width) * size_t(p->height) * (rgba8 ? 4 : 16);
-        void* dev = nullptr;
-        rc = pe_scratch_buffer(ctx, 0, bytes, &dev) || render_player_device(pl, ctx, &t, rgba8, dev) || pe_memcpy_d2h(ctx, out_host, dev, bytes, nullptr);
-    } else {
-        rc = rgba8 ? pe_render_host_rgba8(ctx, &t, (uint8_t*)out_host) : pe_render_host(ctx, &t, (float*)out_host);
-    }
-    if (rc) return pfail(pl, std::string("render failed: ") + pe_last_error(ctx));
-    return 0;
-}
-
-// The frame as RGBA8 in scratch slot 0 (*out8).
-static int render_player_rgba8(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, void** out8) {
-    if (upload_player_uniforms(pl, ctx, p)) return 1;
-    pe_target t = {p->width, p->height, p->height, 0, 1, 1, 1};
-    if (pe_scratch_buffer(ctx, 0, size_t(p->width) * size_t(p->height) * 4, out8) || render_player_device(pl, ctx, &t, 1, *out8))
-        return pfail(pl, std::string("render failed: ") + pe_last_error(ctx));
-    return 0;
-}
-
-int ph_player_render_frame_png(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, uint8_t* png, size_t capacity, size_t* len) {
-    if (!pl || !ctx || !p || !png || !len) return 1;
-    void* dev = nullptr;
-    if (render_player_rgba8(pl, ctx, p, &dev)) return 1;
-    if (pe_encode_png_host(ctx, dev, p->width, p->height, png, capacity, len)) return pfail(pl, std::string("PNG encoding failed: ") + pe_last_error(ctx));
-    return 0;
-}
-
 int ph_player_set_adaptive_aa(ph_player* pl, int on, int threshold) {
     if (!pl) return 1;
     pl->adaptive_aa = on != 0;
@@ -614,160 +586,110 @@ int ph_player_set_adaptive_aa(ph_player* pl, int on, int threshold) {
     return 0;
 }
 
-// The frame as RGBA16 in scratch slot 0 (*out16): rendered as floats into slot 1, then quantised.
-static int render_player_rgba16(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, void** out16) {
-    if (upload_player_uniforms(pl, ctx, p)) return 1;
-    pe_target t = {p->width, p->height, p->height, 0, 1, 1, 1};
-    const size_t n = size_t(p->width) * size_t(p->height);
-    void* f32 = nullptr;
-    if (pe_scratch_buffer(ctx, 0, n * 8, out16) || pe_scratch_buffer(ctx, 1, n * 16, &f32) || render_player_device(pl, ctx, &t, 0, f32) ||
-        pe_quantize_rgba16(ctx, f32, *out16, n, nullptr))
-        return pfail(pl, std::string("render failed: ") + pe_last_error(ctx));
-    return 0;
-}
-
-int ph_player_render_frame_rgba16(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, uint16_t* out_host) {
-    if (!pl || !ctx || !p || !out_host) return 1;
-    void* dev = nullptr;
-    if (render_player_rgba16(pl, ctx, p, &dev)) return 1;
-    if (pe_memcpy_d2h(ctx, out_host, dev, size_t(p->width) * size_t(p->height) * 8, nullptr)) return pfail(pl, std::string("render failed: ") + pe_last_error(ctx));
-    return 0;
-}
-
-int ph_player_render_frame_png16(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, uint8_t* png, size_t capacity, size_t* len) {
-    if (!pl || !ctx || !p || !png || !len) return 1;
-    void* dev = nullptr;
-    if (render_player_rgba16(pl, ctx, p, &dev)) return 1;
-    if (pe_encode_png_host_rgba16(ctx, dev, p->width, p->height, png, capacity, len)) return pfail(pl, std::string("PNG encoding failed: ") + pe_last_error(ctx));
-    return 0;
-}
-
-// The sub-frame update times of one output frame of render_animation (main.rs:1786-1797): sub-frame j at t * duration_seconds,
-// t = frame_index / frame_count + j / motion_blur_frames / frame_count * exposure, exposure 0.5.  The render and the advance
-// paths both check their arguments and take their times here, so that they cannot drift apart.
-static int motion_blur_times(ph_player* pl, const char* fn, int frame_index, int frame_count, int motion_blur_frames, double duration_seconds,
-                             std::vector<double>& times) {
-    if (frame_count < 1 || motion_blur_frames < 1 || motion_blur_frames > 64 || frame_index < 0)
-        return pfail(pl, std::string(fn) + ": bad frame arguments");
-    const double exposure = 0.5;
-    times.resize(size_t(motion_blur_frames));
-    for (int j = 0; j < motion_blur_frames; j++) {
-        const double tt = double(frame_index) / double(frame_count) + double(j) / double(motion_blur_frames) / double(frame_count) * exposure;
-        times[size_t(j)] = tt * duration_seconds;
-    }
-    return 0;
-}
-
-// The device half of ph_player_render_motion_blur_frame*: the sub-frames and their gamma-2 average, left in scratch slot 0
-// (*out); the sub-frames use slots 1 .. motion_blur_frames.  `bits` is the sub-frames' format: 8 -- RGBA8, rendered so by
-// the render kernel; 16 -- RGBA16, each rendered as floats into slot motion_blur_frames + 1 and quantised from there.
-static int motion_blur_device(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index, int frame_count, int motion_blur_frames,
-                              double duration_seconds, int bits, void** out) {
-    std::vector<double> times;
-    if (motion_blur_times(pl, "ph_player_render_motion_blur_frame", frame_index, frame_count, motion_blur_frames, duration_seconds, times)) return 1;
-    const size_t n = size_t(p->width) * size_t(p->height), px_bytes = bits == 16 ? 8 : 4;
-    std::vector<void*> sub(size_t(motion_blur_frames), nullptr);
-    void* f32 = nullptr;
-    int rc = pe_scratch_buffer(ctx, 0, n * px_bytes, out);
-    for (size_t j = 0; j < sub.size(); j++) rc |= pe_scratch_buffer(ctx, 1 + int(j), n * px_bytes, &sub[j]);
-    if (bits == 16) rc |= pe_scratch_buffer(ctx, 1 + motion_blur_frames, n * 16, &f32);
-    if (rc) pl->err = std::string("device allocation failed: ") + pe_last_error(ctx);
-    pe_target t = {p->width, p->height, p->height, 0, 1, 1, 1};
-    for (int j = 0; j < motion_blur_frames && !rc; j++) {
-        ph_frame_params q = *p;
-        q.aa_start = j;  // main.rs:1797
-        if (!pl->player.update(times[size_t(j)])) {   // self.update(memory, t * duration)
-            pl->err = pl->player.error;
-            rc = 1;
-            break;
-        }
-        if (pl->hook && pl->hook(pl->hook_user)) { pl->err = "the update hook failed"; rc = 1; break; }   // ... whose tail swaps video frames
-        if (upload_player_uniforms(pl, ctx, &q)) {
-            rc = 1;
-        } else if (bits == 16 ? render_player_device(pl, ctx, &t, 0, f32) || pe_quantize_rgba16(ctx, f32, sub[size_t(j)], n, nullptr)
-                              : render_player_device(pl, ctx, &t, 1, sub[size_t(j)])) {
-            pl->err = std::string("render failed: ") + pe_last_error(ctx);
-            rc = 1;
-        }
-    }
-    if (!rc && (bits == 16 ? pe_average_frames_rgba16(ctx, sub.data(), motion_blur_frames, *out, n, nullptr)
-                           : pe_average_frames_rgba8(ctx, sub.data(), motion_blur_frames, *out, n, nullptr))) {
-        pl->err = std::string("motion-blur average failed: ") + pe_last_error(ctx);
-        rc = 1;
-    }
-    return rc ? 1 : 0;
-}
-
 int ph_player_advance_motion_blur_frame(ph_player* pl, int frame_index, int frame_count, int motion_blur_frames, double duration_seconds) {
     if (!pl) return 1;
     std::vector<double> times;
-    if (motion_blur_times(pl, "ph_player_advance_motion_blur_frame", frame_index, frame_count, motion_blur_frames, duration_seconds, times)) return 1;
+    if (!motion_blur_times(frame_index, frame_count, motion_blur_frames, duration_seconds, times))
+        return pfail(pl, "ph_player_advance_motion_blur_frame: bad frame arguments");
     for (double t : times)
         if (!pl->player.update(t)) return pfail(pl, pl->player.error);
     return 0;
 }
 
-int ph_player_render_motion_blur_frame(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index, int frame_count,
-                                       int motion_blur_frames, double duration_seconds, uint8_t* out_host) {
-    if (!pl || !ctx || !p || !out_host) return 1;
-    void* out8 = nullptr;
-    if (motion_blur_device(pl, ctx, p, frame_index, frame_count, motion_blur_frames, duration_seconds, 8, &out8)) return 1;
-    if (pe_memcpy_d2h(ctx, out_host, out8, size_t(p->width) * size_t(p->height) * 4, nullptr)) return pfail(pl, std::string("motion-blur average failed: ") + pe_last_error(ctx));
+size_t ph_output_bytes(int container, int bits, int width, int height) {
+    if (width <= 0 || height <= 0) return 0;
+    switch (container) {
+        case PH_OUT_PIXELS:   // four channels of bits / 8 bytes
+            return bits == 8 || bits == 16 || bits == 32 ? size_t(width) * size_t(height) * size_t(bits / 2) : 0;
+        case PH_OUT_PNG: return bits == 8 ? pe_png_bound(width, height) : bits == 16 ? pe_png_bound_rgba16(width, height) : 0;
+        case PH_OUT_YUV420P10: return bits == 8 || bits == 16 ? pe_yuv420p10_bytes(width, height) : 0;
+    }
     return 0;
 }
 
-int ph_player_render_motion_blur_frame_png(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index, int frame_count,
-                                           int motion_blur_frames, double duration_seconds, uint8_t* png, size_t capacity, size_t* len) {
-    if (!pl || !ctx || !p || !png || !len) return 1;
-    void* out8 = nullptr;
-    if (motion_blur_device(pl, ctx, p, frame_index, frame_count, motion_blur_frames, duration_seconds, 8, &out8)) return 1;
-    if (pe_encode_png_host(ctx, out8, p->width, p->height, png, capacity, len)) return pfail(pl, std::string("PNG encoding failed: ") + pe_last_error(ctx));
+// The frame of the uploaded uniforms into device memory `dev` at `bits` 8 (RGBA8), 16 (RGBA16: rendered as floats into `f32`,
+// then quantised) or 32 (float RGBA); adaptively when the player is set so.
+static int render_device(ph_player* pl, pe_ctx* ctx, const pe_target* t, int bits, void* dev, void* f32) {
+    void* out = bits == 16 ? f32 : dev;
+    const int rgba8 = bits == 8;
+    const int rc = pl->adaptive_aa ? pe_render_adaptive(ctx, t, pl->adaptive_threshold, rgba8, out, nullptr, nullptr)
+                                   : rgba8 ? pe_render_rgba8(ctx, t, out, nullptr) : pe_render(ctx, t, out, nullptr, nullptr);
+    return rc || (bits == 16 && pe_quantize_rgba16(ctx, f32, dev, size_t(t->width) * size_t(t->height), nullptr));
+}
+
+// Stage, convert, read back.  The scratch slots follow one rule (portal_b200_host.h): 0 the frame, 1 .. M the sub-frames,
+// M + 1 the floats of a 16-bit frame, then the Y'CbCr planes.
+int ph_player_render(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, const ph_motion_blur* mb, int container, int bits,
+                     void* out_host, size_t capacity, size_t* len) {
+    if (!pl || !ctx || !p || !out_host || !len) return 1;
+    if (container != PH_OUT_PIXELS && container != PH_OUT_PNG && container != PH_OUT_YUV420P10)
+        return pfail(pl, "ph_player_render: unknown container " + std::to_string(container));
+    if (container != PH_OUT_PIXELS && bits != 8 && bits != 16) return pfail(pl, "ph_player_render: bits must be 8 or 16 for PNG and Y'CbCr");
+    if (bits != 8 && bits != 16 && bits != 32) return pfail(pl, "ph_player_render: bits must be 8, 16 or 32");
+    if (bits == 32 && mb) return pfail(pl, "ph_player_render: motion blur needs bits 8 or 16 (its sub-frames are averaged as integers)");
+    std::vector<double> times;
+    if (mb && !motion_blur_times(mb->frame_index, mb->frame_count, mb->motion_blur_frames, mb->duration_seconds, times))
+        return pfail(pl, "ph_player_render: bad frame arguments");
+    const size_t bytes = ph_output_bytes(container, bits, p->width, p->height);
+    if (!bytes) return pfail(pl, "ph_player_render: invalid frame size " + std::to_string(p->width) + " x " + std::to_string(p->height));
+    if (capacity < bytes) return pfail(pl, "ph_player_render: capacity " + std::to_string(capacity) + " is below ph_output_bytes = " + std::to_string(bytes));
+    const pe_target t = {p->width, p->height, p->height, 0, 1, 1, 1};
+    const size_t n = size_t(p->width) * size_t(p->height);
+    const int M = mb ? mb->motion_blur_frames : 0;
+
+    // stage: the frame in slot 0
+    if (!mb) {
+        if (upload_player_uniforms(pl, ctx, p)) return 1;
+        if (container == PH_OUT_PIXELS && bits != 16 && !pl->adaptive_aa) {   // rendered straight into host memory, no slot
+            if (bits == 8 ? pe_render_host_rgba8(ctx, &t, static_cast<uint8_t*>(out_host)) : pe_render_host(ctx, &t, static_cast<float*>(out_host)))
+                return pfail(pl, std::string("render failed: ") + pe_last_error(ctx));
+            *len = bytes;
+            return 0;
+        }
+    }
+    std::vector<void*> slot(size_t(M) + 2, nullptr);
+    int rc = 0;
+    for (int k = 0; k <= M; k++) rc |= pe_scratch_buffer(ctx, k, n * size_t(bits / 2), &slot[size_t(k)]);
+    if (bits == 16) rc |= pe_scratch_buffer(ctx, M + 1, n * 16, &slot[size_t(M) + 1]);
+    void* const frame = slot[0];
+    void* const f32 = slot[size_t(M) + 1];
+    if (!mb) {
+        if (rc || render_device(pl, ctx, &t, bits, frame, f32)) return pfail(pl, std::string("render failed: ") + pe_last_error(ctx));
+    } else {
+        // one output frame of render_animation (main.rs:1786-1817): every sub-frame j updates the player to times[j] (and runs
+        // the update hook, whose tail swaps video frames), renders with `_aa_start` = j, and the sub-frames are averaged in
+        // gamma-2 space
+        if (rc) return pfail(pl, std::string("device allocation failed: ") + pe_last_error(ctx));
+        for (int j = 0; j < M; j++) {
+            ph_frame_params q = *p;
+            q.aa_start = j;  // main.rs:1797
+            if (!pl->player.update(times[size_t(j)])) return pfail(pl, pl->player.error);
+            if (pl->hook && pl->hook(pl->hook_user)) return pfail(pl, "the update hook failed");
+            if (upload_player_uniforms(pl, ctx, &q)) return 1;
+            if (render_device(pl, ctx, &t, bits, slot[size_t(j) + 1], f32)) return pfail(pl, std::string("render failed: ") + pe_last_error(ctx));
+        }
+        if (bits == 16 ? pe_average_frames_rgba16(ctx, slot.data() + 1, M, frame, n, nullptr)
+                       : pe_average_frames_rgba8(ctx, slot.data() + 1, M, frame, n, nullptr))
+            return pfail(pl, std::string("motion-blur average failed: ") + pe_last_error(ctx));
+    }
+
+    // convert and read back
+    if (container == PH_OUT_PNG) {
+        if (bits == 16 ? pe_encode_png_host_rgba16(ctx, frame, p->width, p->height, static_cast<uint8_t*>(out_host), capacity, len)
+                       : pe_encode_png_host(ctx, frame, p->width, p->height, static_cast<uint8_t*>(out_host), capacity, len))
+            return pfail(pl, std::string("PNG encoding failed: ") + pe_last_error(ctx));
+        return 0;
+    }
+    if (container == PH_OUT_YUV420P10) {
+        void* yuv = nullptr;
+        if (pe_scratch_buffer(ctx, M + (bits == 16 ? 2 : 1), bytes, &yuv) || pe_rgba_to_yuv420p10(ctx, frame, bits, p->width, p->height, yuv, nullptr) ||
+            pe_memcpy_d2h(ctx, out_host, yuv, bytes, nullptr))
+            return pfail(pl, std::string("Y'CbCr conversion failed: ") + pe_last_error(ctx));
+    } else if (pe_memcpy_d2h(ctx, out_host, frame, bytes, nullptr)) {
+        return pfail(pl, std::string(mb ? "motion-blur average failed: " : "render failed: ") + pe_last_error(ctx));
+    }
+    *len = bytes;
     return 0;
-}
-
-int ph_player_render_motion_blur_frame_rgba16(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index, int frame_count,
-                                              int motion_blur_frames, double duration_seconds, uint16_t* out_host) {
-    if (!pl || !ctx || !p || !out_host) return 1;
-    void* out16 = nullptr;
-    if (motion_blur_device(pl, ctx, p, frame_index, frame_count, motion_blur_frames, duration_seconds, 16, &out16)) return 1;
-    if (pe_memcpy_d2h(ctx, out_host, out16, size_t(p->width) * size_t(p->height) * 8, nullptr)) return pfail(pl, std::string("motion-blur average failed: ") + pe_last_error(ctx));
-    return 0;
-}
-
-int ph_player_render_motion_blur_frame_png16(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index, int frame_count,
-                                             int motion_blur_frames, double duration_seconds, uint8_t* png, size_t capacity, size_t* len) {
-    if (!pl || !ctx || !p || !png || !len) return 1;
-    void* out16 = nullptr;
-    if (motion_blur_device(pl, ctx, p, frame_index, frame_count, motion_blur_frames, duration_seconds, 16, &out16)) return 1;
-    if (pe_encode_png_host_rgba16(ctx, out16, p->width, p->height, png, capacity, len)) return pfail(pl, std::string("PNG encoding failed: ") + pe_last_error(ctx));
-    return 0;
-}
-
-// A frame already on the device (RGBA8 or RGBA16 per `bits`) -> its Y'CbCr 4:2:0 planes in scratch slot `slot` -> out_host.
-static int read_back_yuv420p10(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int bits, const void* frame, int slot, uint16_t* out_host) {
-    const size_t bytes = pe_yuv420p10_bytes(p->width, p->height);
-    void* yuv = nullptr;
-    if (!bytes || pe_scratch_buffer(ctx, slot, bytes, &yuv) || pe_rgba_to_yuv420p10(ctx, frame, bits, p->width, p->height, yuv, nullptr) ||
-        pe_memcpy_d2h(ctx, out_host, yuv, bytes, nullptr))
-        return pfail(pl, std::string("Y'CbCr conversion failed: ") + (bytes ? pe_last_error(ctx) : "invalid frame size"));
-    return 0;
-}
-
-int ph_player_render_frame_yuv420p10(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int bits, uint16_t* out_host) {
-    if (!pl || !ctx || !p || !out_host) return 1;
-    if (bits != 8 && bits != 16) return pfail(pl, "ph_player_render_frame_yuv420p10: bits must be 8 or 16");
-    void* dev = nullptr;
-    if (bits == 16 ? render_player_rgba16(pl, ctx, p, &dev) : render_player_rgba8(pl, ctx, p, &dev)) return 1;
-    return read_back_yuv420p10(pl, ctx, p, bits, dev, bits == 16 ? 2 : 1, out_host);
-}
-
-int ph_player_render_motion_blur_frame_yuv420p10(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, int frame_index, int frame_count,
-                                                 int motion_blur_frames, double duration_seconds, int bits, uint16_t* out_host) {
-    if (!pl || !ctx || !p || !out_host) return 1;
-    if (bits != 8 && bits != 16) return pfail(pl, "ph_player_render_motion_blur_frame_yuv420p10: bits must be 8 or 16");
-    void* dev = nullptr;
-    if (motion_blur_device(pl, ctx, p, frame_index, frame_count, motion_blur_frames, duration_seconds, bits, &dev)) return 1;
-    return read_back_yuv420p10(pl, ctx, p, bits, dev, motion_blur_frames + (bits == 16 ? 2 : 1), out_host);
 }
 
 // ---- image files (ph_png.cpp)

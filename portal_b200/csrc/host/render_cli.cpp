@@ -19,24 +19,24 @@
 //
 // --bit-depth 16 (not in the reference; 8 by default): frames of 16 bits per channel for a 10-bit video encode.  Every frame /
 // sub-frame is rendered as floats and quantised to unorm16 (motion blur averages the RGBA16 sub-frames), then written as a
-// 16-bit PNG (encoded on the device: ph_player_render_frame_png16, pe_encode_png_rgba16), as raw little-endian RGBA16 for
-// .rgba, or as a P6 PPM with maxval 65535 (big-endian samples, alpha dropped).
+// 16-bit PNG (encoded on the device: pe_encode_png_rgba16), as raw little-endian RGBA16 for .rgba, or as a P6 PPM with maxval
+// 65535 (big-endian samples, alpha dropped).
 //
 // --frame-format y4m / --output *.y4m (not in the reference, whose ffmpeg step does this conversion): the frames the other
 // formats would write (RGBA8, or RGBA16 with --bit-depth 16) converted on the device to Y'CbCr 4:2:0 at 10 bits, BT.709, full
-// range (ph_player_render_*_yuv420p10, pe_rgba_to_yuv420p10; DESIGN.md section 5.4), written as a YUV4MPEG2 stream of
-// yuv420p10le frames -- the raw input ffmpeg and x265 read from a file or a pipe.  `render` writes one stream per animation,
-// DIR/<animation>.y4m at --fps, and skips an animation whose stream exists (as the reference skips an existing .mov,
-// main.rs:1771-1779); --out-dir - writes the stream of the one selected animation to stdout, with every status line on
-// stderr.  render-frame writes a one-frame stream at 25 fps.
+// range (pe_rgba_to_yuv420p10; DESIGN.md section 5.4), written as a YUV4MPEG2 stream of yuv420p10le frames -- the raw input
+// ffmpeg and x265 read from a file or a pipe.  `render` writes one stream per animation, DIR/<animation>.y4m at --fps, and
+// skips an animation whose stream exists (as the reference skips an existing .mov, main.rs:1771-1779); --out-dir - writes the
+// stream of the one selected animation to stdout, with every status line on stderr.  render-frame writes a one-frame stream
+// at 25 fps.
 //
 // Output: the RGBA8 frame the reference hands to export_png (main.rs:2939-2943) as a PNG when the name ends in .png (encoded
-// on the device: ph_player_render_frame_png / ph_player_render_motion_blur_frame_png, pe_encode_png_rgba8), as raw RGBA8 for
-// .rgba, else as a binary PPM (P6, alpha dropped).  Textures: every texture of the
-// scene is loaded from its stored path (a PNG, relative to --assets, default the working directory) like reload_textures
-// (main.rs:1066-1085) -- a file that cannot be read is reported and the sampler stays unbound, as there; --texture overrides one
-// by name (PNG, or raw RGBA8 with :WxH).  Videos: the frames of video_png/<stem>/*.png, sorted, the one the video's uniform
-// selects swapped in after every update (VideoRuntime, main.rs:771-930).
+// on the device: pe_encode_png_rgba8), as raw RGBA8 for .rgba, else as a binary PPM (P6, alpha dropped).  Every format is one
+// ph_player_render call per frame.  Textures: every texture of the scene is loaded from its stored path (a PNG, relative to
+// --assets, default the working directory) like reload_textures (main.rs:1066-1085) -- a file that cannot be read is reported
+// and the sampler stays unbound, as there; --texture overrides one by name (PNG, or raw RGBA8 with :WxH).  Videos: the frames
+// of video_png/<stem>/*.png, sorted, the one the video's uniform selects swapped in after every update (VideoRuntime,
+// main.rs:771-930).
 //
 // Y4M clips (not in the reference, which decodes a PNG per frame change): a video's frames may instead come from a YUV4MPEG2
 // stream of raw 4:2:0 frames (`ffmpeg -i clip.mp4 -pix_fmt yuv420p clip.y4m`), read with one pread per frame change and
@@ -99,44 +99,38 @@ static bool write_y4m_frame(FILE* f, const std::vector<uint8_t>& planes) {
     return std::fputs("FRAME\n", f) >= 0 && std::fwrite(planes.data(), 1, planes.size(), f) == planes.size();
 }
 
-static bool write_bytes(const std::string& output, const std::vector<uint8_t>& bytes, size_t n) {
-    std::ofstream out(output, std::ios::binary);
-    if (!out) return false;
-    out.write(reinterpret_cast<const char*>(bytes.data()), std::streamsize(n));
-    return bool(out);
-}
+// How a frame becomes output, decided once from --output / --frame-format and --bit-depth: what ph_player_render delivers (the
+// container, rendered at `bits`) and how those bytes become a file
+enum FrameFile { AS_RETURNED, PPM, Y4M };
+struct FrameFormat {
+    FrameFile file;
+    int container, bits;
+};
 
-// .rgba / .ppm frames (PNG frames are encoded on the device and written by write_bytes)
-static bool write_image(const std::string& output, const std::vector<uint8_t>& px, int width, int height) {
-    std::ofstream out(output, std::ios::binary);
-    if (!out) return false;
-    if (ends_with(output, ".rgba")) {
-        out.write(reinterpret_cast<const char*>(px.data()), std::streamsize(px.size()));
-    } else {
-        out << "P6\n" << width << " " << height << "\n255\n";
-        for (size_t i = 0; i < size_t(width) * size_t(height); i++) out.write(reinterpret_cast<const char*>(&px[4 * i]), 3);
+// One frame as ph_player_render returned it (`len` bytes of `px`) -> the file `path`: the bytes as they are (PNG; raw RGBA8, or
+// RGBA16 in host byte order, which is little-endian), a P6 PPM with alpha dropped (maxval 255, or 65535 with big-endian samples,
+// as the format defines), or a one-frame Y4M stream at 25 fps
+static bool write_frame(const std::string& path, const FrameFormat& fmt, const std::vector<uint8_t>& px, size_t len, int width, int height) {
+    if (fmt.file == Y4M) {
+        FILE* f = std::fopen(path.c_str(), "wb");
+        if (!f) return false;
+        const bool ok = write_y4m_header(f, width, height, 25) && write_y4m_frame(f, px);
+        return std::fclose(f) == 0 && ok;
     }
-    return bool(out);
-}
-
-// The same for an RGBA16 frame (`px` holds its uint16 samples in host byte order): .rgba is raw RGBA16, little-endian; .ppm is
-// P6 with maxval 65535, alpha dropped, samples big-endian (as the format defines)
-static bool write_image16(const std::string& output, const std::vector<uint8_t>& px, int width, int height) {
-    const uint16_t* s = reinterpret_cast<const uint16_t*>(px.data());
-    const size_t n = size_t(width) * size_t(height);
-    const bool rgba = ends_with(output, ".rgba");
-    std::vector<uint8_t> bytes;
-    bytes.reserve(n * (rgba ? 8 : 6));
-    for (size_t i = 0; i < n; i++)
-        for (int k = 0; k < (rgba ? 4 : 3); k++) {
-            const uint16_t v = s[4 * i + size_t(k)];
-            if (rgba) { bytes.push_back(uint8_t(v)); bytes.push_back(uint8_t(v >> 8)); }
-            else { bytes.push_back(uint8_t(v >> 8)); bytes.push_back(uint8_t(v)); }
-        }
-    std::ofstream out(output, std::ios::binary);
+    std::ofstream out(path, std::ios::binary);
     if (!out) return false;
-    if (!rgba) out << "P6\n" << width << " " << height << "\n65535\n";
-    out.write(reinterpret_cast<const char*>(bytes.data()), std::streamsize(bytes.size()));
+    if (fmt.file == AS_RETURNED) {
+        out.write(reinterpret_cast<const char*>(px.data()), std::streamsize(len));
+        return bool(out);
+    }
+    const size_t n = size_t(width) * size_t(height), bytes = size_t(fmt.bits / 8);   // per sample
+    std::vector<uint8_t> rgb(n * 3 * bytes);
+    uint8_t* o = rgb.data();
+    for (size_t i = 0; i < n; i++)
+        for (size_t c = 0; c < 3; c++)
+            for (size_t b = 0; b < bytes; b++) *o++ = px[(4 * i + c) * bytes + bytes - 1 - b];
+    out << "P6\n" << width << " " << height << "\n" << (bytes == 2 ? 65535 : 255) << "\n";
+    out.write(reinterpret_cast<const char*>(rgb.data()), std::streamsize(rgb.size()));
     return bool(out);
 }
 
@@ -297,8 +291,8 @@ struct Worker {
     ph_scene* scene = nullptr;
     ph_player* player = nullptr;
     VideoState video_state;                           // the player's update hook points here: workers never move
-    std::vector<uint8_t> px;                          // the frame: RGBA8 / RGBA16 pixels or a PNG file
-    size_t png_len = 0;
+    std::vector<uint8_t> px;                          // the frame as ph_player_render returns it
+    size_t len = 0;                                   // its bytes
     std::vector<std::vector<uint8_t>> free_planes;   // `render` to Y4M: the plane buffers the main thread does not hold
 };
 
@@ -462,8 +456,12 @@ int main(int argc, char** argv) {
         }
         for (const std::string& nm : names) selected += !all || starts_with.empty() || nm.compare(0, starts_with.size(), starts_with) == 0;
     }
-    const bool y4m = frame_cmd ? ends_with(output, ".y4m") : frame_ext == ".y4m";
-    const bool to_stdout = anim_cmd && y4m && out_dir == "-";
+    // the frame's format: from the output's name (render-frame) or --frame-format (render), at --bit-depth
+    auto format_is = [&](const char* ext) { return frame_cmd ? ends_with(output, ext) : frame_ext == ext; };
+    const FrameFormat fmt = format_is(".png")   ? FrameFormat{AS_RETURNED, PH_OUT_PNG, bits}   // Image::export_png (main.rs:2939-2943)
+                            : format_is(".y4m") ? FrameFormat{Y4M, PH_OUT_YUV420P10, bits}
+                                                : FrameFormat{ends_with(frame_cmd ? output : frame_ext, ".rgba") ? AS_RETURNED : PPM, PH_OUT_PIXELS, bits};
+    const bool to_stdout = anim_cmd && fmt.file == Y4M && out_dir == "-";
     if (to_stdout && selected != 1) {
         std::fprintf(stderr, "--out-dir - writes one Y4M stream to stdout: select exactly one animation (%zu selected)\n", selected);
         return 2;
@@ -601,42 +599,27 @@ int main(int argc, char** argv) {
         if (const int rc = set_up(workers[w], w == 0)) return rc;
     }
     if (stereo) width *= 2;         // side-by-side eyes, doubled width
-    const bool png = frame_cmd ? ends_with(output, ".png") : frame_ext == ".png";       // Image::export_png (main.rs:2939-2943)
-    // one buffer per worker for the frame: RGBA8 / RGBA16 pixels, a PNG file of at most pe_png_bound(_rgba16) bytes, or Y'CbCr
-    // planes (`render` to Y4M: two, which travel to the main thread and back)
-    const bool b16 = bits == 16;
-    const size_t frame_bytes = png ? (b16 ? pe_png_bound_rgba16(width, height) : pe_png_bound(width, height))
-                                   : y4m ? pe_yuv420p10_bytes(width, height) : size_t(width) * size_t(height) * (b16 ? 8 : 4);
-    if (!frame_bytes) { std::fprintf(stderr, "no %s for a %d x %d frame\n", y4m ? "Y4M stream" : "PNG", width, height); return 1; }
+    // one buffer per worker for the frame (`render` to Y4M: two for its planes, which travel to the main thread and back)
+    const size_t frame_bytes = ph_output_bytes(fmt.container, fmt.bits, width, height);
+    if (!frame_bytes) {
+        static const char* const what[] = {"image", "PNG", "Y4M stream"};
+        std::fprintf(stderr, "no %s for a %d x %d frame\n", what[fmt.container], width, height);
+        return 1;
+    }
     for (Worker& wk : workers) {
-        if (anim_cmd && y4m) wk.free_planes.assign(2, std::vector<uint8_t>(frame_bytes));
+        if (anim_cmd && fmt.file == Y4M) wk.free_planes.assign(2, std::vector<uint8_t>(frame_bytes));
         else wk.px.resize(frame_bytes);
     }
-    auto write_frame = [&](Worker& wk, const std::string& name) {
-        return png ? write_bytes(name, wk.px, wk.png_len) : b16 ? write_image16(name, wk.px, width, height) : write_image(name, wk.px, width, height);
-    };
     ph_frame_params p = {width, height, depth, aa, 0, 0, {0, 0, 0}, 0, 0, 0};
     int exit_code = 0;
     if (frame_cmd) {
         Worker& wk = workers[0];
-        uint16_t* px16 = reinterpret_cast<uint16_t*>(wk.px.data());
         if (ph_player_update(wk.player, time) ||                                                          // main.rs:2928-2929
-            (png ? (b16 ? ph_player_render_frame_png16 : ph_player_render_frame_png)(wk.player, wk.ctx, &p, wk.px.data(), wk.px.size(), &wk.png_len)
-                 : y4m ? ph_player_render_frame_yuv420p10(wk.player, wk.ctx, &p, bits, px16)
-                 : b16 ? ph_player_render_frame_rgba16(wk.player, wk.ctx, &p, px16) : ph_player_render_frame(wk.player, wk.ctx, &p, wk.px.data(), 1))) {
+            ph_player_render(wk.player, wk.ctx, &p, nullptr, fmt.container, fmt.bits, wk.px.data(), wk.px.size(), &wk.len)) {
             std::fprintf(stderr, "%s\n", ph_player_last_error(wk.player));
             return 1;
         }
-        bool written = false;
-        if (y4m) {
-            if (FILE* f = std::fopen(output.c_str(), "wb")) {
-                written = write_y4m_header(f, width, height, 25) && write_y4m_frame(f, wk.px);
-                written = std::fclose(f) == 0 && written;
-            }
-        } else {
-            written = write_frame(wk, output);
-        }
-        if (!written) { std::fprintf(stderr, "cannot write %s\n", output.c_str()); return 1; }
+        if (!write_frame(output, fmt, wk.px, wk.len, width, height)) { std::fprintf(stderr, "cannot write %s\n", output.c_str()); return 1; }
         std::printf("Rendered `%s` to `%s`\n", scene_path.c_str(), output.c_str());
     } else {
         // The plan: every skip decision from one snapshot of the output, taken now, plus what the animations before each one
@@ -659,7 +642,7 @@ int main(int argc, char** argv) {
             a.todo = max_frames >= 0 && max_frames < a.count ? max_frames : a.count;
             a.skip_frame.assign(size_t(a.todo), 0);
             if (!a.rendered || to_stdout) continue;
-            if (y4m) {
+            if (fmt.file == Y4M) {
                 const std::string stream = out_dir + "/" + names[k] + ".y4m";
                 a.skip_stream = skip_existing && (file_exists(stream) || to_write.count(stream));     // main.rs:1771-1779
                 if (!a.skip_stream) to_write.insert(stream);
@@ -686,9 +669,9 @@ int main(int argc, char** argv) {
                 const AnimationPlan& a = plan[k];
                 if (!a.rendered) continue;
                 if (me == 0) sh.post(k, -1, {});
-                if (y4m && a.skip_stream) continue;
+                if (fmt.file == Y4M && a.skip_stream) continue;
                 const std::string dir = out_dir + "/" + names[k];
-                if (!y4m && !make_dirs(dir)) { sh.fail("cannot create " + dir); return; }
+                if (fmt.file != Y4M && !make_dirs(dir)) { sh.fail("cannot create " + dir); return; }
                 for (int i = 0; i < a.todo; i++) {
                     if (sh.stopped()) return;
                     if (a.skip_frame[size_t(i)]) continue;                 // neither rendered nor advanced, as the sequential loop
@@ -696,28 +679,19 @@ int main(int argc, char** argv) {
                         if (ph_player_advance_motion_blur_frame(wk.player, i, a.count, motion_blur, a.duration)) { sh.fail(ph_player_last_error(wk.player)); return; }
                         continue;
                     }
-                    if (y4m) {
-                        std::vector<uint8_t> planes;
-                        if (!sh.take_buffer(wk, planes)) return;
-                        if (ph_player_render_motion_blur_frame_yuv420p10(wk.player, wk.ctx, &p, i, a.count, motion_blur, a.duration, bits,
-                                                                         reinterpret_cast<uint16_t*>(planes.data()))) {
-                            sh.fail(ph_player_last_error(wk.player));
-                            return;
-                        }
-                        sh.post(k, i, std::move(planes));
-                        continue;
-                    }
-                    uint16_t* px16 = reinterpret_cast<uint16_t*>(wk.px.data());
-                    const double dur = a.duration;
-                    if (png ? (b16 ? ph_player_render_motion_blur_frame_png16 : ph_player_render_motion_blur_frame_png)(wk.player, wk.ctx, &p, i, a.count, motion_blur, dur, wk.px.data(), wk.px.size(), &wk.png_len)
-                            : b16 ? ph_player_render_motion_blur_frame_rgba16(wk.player, wk.ctx, &p, i, a.count, motion_blur, dur, px16)
-                                  : ph_player_render_motion_blur_frame(wk.player, wk.ctx, &p, i, a.count, motion_blur, dur, wk.px.data())) {
+                    std::vector<uint8_t> planes;                           // Y4M: the frame goes to the main thread
+                    if (fmt.file == Y4M && !sh.take_buffer(wk, planes)) return;
+                    std::vector<uint8_t>& buf = fmt.file == Y4M ? planes : wk.px;
+                    const ph_motion_blur mb = {i, a.count, motion_blur, a.duration};
+                    if (ph_player_render(wk.player, wk.ctx, &p, &mb, fmt.container, fmt.bits, buf.data(), buf.size(), &wk.len)) {
                         sh.fail(ph_player_last_error(wk.player));
                         return;
                     }
-                    const std::string name = dir + "/frame_" + std::to_string(i) + frame_ext;
-                    if (!write_frame(wk, name)) { sh.fail("cannot write " + name); return; }
-                    sh.post(k, i, {});
+                    if (fmt.file != Y4M) {
+                        const std::string name = dir + "/frame_" + std::to_string(i) + frame_ext;
+                        if (!write_frame(name, fmt, wk.px, wk.len, width, height)) { sh.fail("cannot write " + name); return; }
+                    }
+                    sh.post(k, i, std::move(planes));
                 }
             }
         };
@@ -731,7 +705,7 @@ int main(int argc, char** argv) {
             if (!sh.take(k, -1, planes)) break;
             std::fprintf(status, "Rendering animation %s, %zu/%zu\n", names[k].c_str(), k + 1, names.size());
             bool stopped = false;
-            if (y4m) {
+            if (fmt.file == Y4M) {
                 // one stream per animation, written under a temporary name and renamed when complete, so that an interrupted
                 // run leaves no stream for skip-existing to take as done
                 const std::string stream = out_dir + "/" + names[k] + ".y4m", part = stream + ".part";

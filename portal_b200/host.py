@@ -244,21 +244,26 @@ class HostPlayer:
                 "look_at": list(orbit[:3]), "alpha": orbit[3], "beta": orbit[4], "r": orbit[5],
                 "time": times[0], "total_time": times[1], "n_probes": n.value}
 
-    def render_frame(self, width, height, depth, aa_count=1, aa_start=0, rgba8=False) -> np.ndarray:
+    def _render(self, container, bits, width, height, depth, aa_count, aa_start=0, motion_blur=None) -> np.ndarray:
+        """ph_player_render: the bytes it writes, as uint8.  motion_blur: (frame_index, frame_count, motion_blur_frames,
+        duration_seconds), or None for one frame at the current update."""
         p = PhFrameParams(width, height, depth, aa_count, aa_start, 0)
-        out = np.empty((height, width, 4), dtype=np.uint8 if rgba8 else np.float32)
-        self._check(self._lib.ph_player_render_frame(self._p, self.renderer._ctx, C.byref(p), out.ctypes.data, int(rgba8)))
-        return out
+        mb = None if motion_blur is None else C.byref(capi.PhMotionBlur(*motion_blur))
+        cap = self._lib.ph_output_bytes(container, bits, width, height)
+        out, n = np.empty(cap, dtype=np.uint8), C.c_size_t()
+        self._check(self._lib.ph_player_render(self._p, self.renderer._ctx, C.byref(p), mb, container, bits, out.ctypes.data, cap,
+                                               C.byref(n)))
+        return out[:n.value]
 
+    def render_frame(self, width, height, depth, aa_count=1, aa_start=0, rgba8=False) -> np.ndarray:
+        out = self._render(capi.PH_OUT_PIXELS, 8 if rgba8 else 32, width, height, depth, aa_count, aa_start)
+        return out.view(np.uint8 if rgba8 else np.float32).reshape(height, width, 4)
 
     def render_motion_blur_frame(self, width, height, depth, frame_index, frame_count, motion_blur_frames, duration_seconds,
                                  aa_count=1) -> np.ndarray:
         """One frame of render_animation (main.rs:1786-1817) inside the current animation, RGBA8."""
-        p = PhFrameParams(width, height, depth, aa_count, 0, 0)
-        out = np.empty((height, width, 4), dtype=np.uint8)
-        self._check(self._lib.ph_player_render_motion_blur_frame(self._p, self.renderer._ctx, C.byref(p), frame_index, frame_count,
-                                                                 motion_blur_frames, float(duration_seconds), out.ctypes.data))
-        return out
+        mb = (frame_index, frame_count, motion_blur_frames, float(duration_seconds))
+        return self._render(capi.PH_OUT_PIXELS, 8, width, height, depth, aa_count, motion_blur=mb).reshape(height, width, 4)
 
     def advance_motion_blur_frame(self, frame_index, frame_count, motion_blur_frames, duration_seconds):
         """The sub-frame updates of render_motion_blur_frame (same times, order and probes) without the update hook, the
@@ -268,37 +273,26 @@ class HostPlayer:
 
     def render_frame_rgba16(self, width, height, depth, aa_count=1, aa_start=0) -> np.ndarray:
         """The frame of render_frame as unorm16 (uint16 [h, w, 4]): the float frame quantised by pe_quantize_rgba16."""
-        p = PhFrameParams(width, height, depth, aa_count, aa_start, 0)
-        out = np.empty((height, width, 4), dtype=np.uint16)
-        self._check(self._lib.ph_player_render_frame_rgba16(self._p, self.renderer._ctx, C.byref(p), out.ctypes.data))
-        return out
+        return self._render(capi.PH_OUT_PIXELS, 16, width, height, depth, aa_count, aa_start).view(np.uint16).reshape(height, width, 4)
 
     def render_motion_blur_frame_rgba16(self, width, height, depth, frame_index, frame_count, motion_blur_frames, duration_seconds,
                                         aa_count=1) -> np.ndarray:
         """render_motion_blur_frame with RGBA16 sub-frames and average (uint16 [h, w, 4])."""
-        p = PhFrameParams(width, height, depth, aa_count, 0, 0)
-        out = np.empty((height, width, 4), dtype=np.uint16)
-        self._check(self._lib.ph_player_render_motion_blur_frame_rgba16(self._p, self.renderer._ctx, C.byref(p), frame_index, frame_count,
-                                                                        motion_blur_frames, float(duration_seconds), out.ctypes.data))
-        return out
+        mb = (frame_index, frame_count, motion_blur_frames, float(duration_seconds))
+        return self._render(capi.PH_OUT_PIXELS, 16, width, height, depth, aa_count, motion_blur=mb).view(np.uint16).reshape(height, width, 4)
 
     def render_frame_yuv420p10(self, width, height, depth, bits=8, aa_count=1, aa_start=0):
         """The frame of render_frame (rgba8=True; `bits` 8) or of render_frame_rgba16 (`bits` 16) as Y'CbCr 4:2:0 at 10 bits,
         converted on the device (DESIGN.md section 5.4): (Y, Cb, Cr), numpy uint16 arrays."""
-        p = PhFrameParams(width, height, depth, aa_count, aa_start, 0)
-        out = np.empty(self._lib.pe_yuv420p10_bytes(width, height) // 2, dtype=np.uint16)
-        self._check(self._lib.ph_player_render_frame_yuv420p10(self._p, self.renderer._ctx, C.byref(p), int(bits), out.ctypes.data))
-        return capi.yuv420p10_planes(out, width, height)
+        out = self._render(capi.PH_OUT_YUV420P10, int(bits), width, height, depth, aa_count, aa_start)
+        return capi.yuv420p10_planes(out.view(np.uint16), width, height)
 
     def render_motion_blur_frame_yuv420p10(self, width, height, depth, frame_index, frame_count, motion_blur_frames, duration_seconds,
                                            bits=8, aa_count=1):
         """render_motion_blur_frame (`bits` 8) or render_motion_blur_frame_rgba16 (`bits` 16) as Y'CbCr 4:2:0 planes."""
-        p = PhFrameParams(width, height, depth, aa_count, 0, 0)
-        out = np.empty(self._lib.pe_yuv420p10_bytes(width, height) // 2, dtype=np.uint16)
-        self._check(self._lib.ph_player_render_motion_blur_frame_yuv420p10(self._p, self.renderer._ctx, C.byref(p), frame_index, frame_count,
-                                                                           motion_blur_frames, float(duration_seconds), int(bits),
-                                                                           out.ctypes.data))
-        return capi.yuv420p10_planes(out, width, height)
+        mb = (frame_index, frame_count, motion_blur_frames, float(duration_seconds))
+        out = self._render(capi.PH_OUT_YUV420P10, int(bits), width, height, depth, aa_count, motion_blur=mb)
+        return capi.yuv420p10_planes(out.view(np.uint16), width, height)
 
 
 class HostRenderer:

@@ -114,7 +114,7 @@ def test_png16_bound_and_argument_checks_without_a_device():
         lib.pe_destroy(ctx)
 
 
-def test_player_16bit_twins_refuse_without_a_device():
+def test_player_render_16bit_refuses_without_a_device():
     from portal_b200.capi import PhFrameParams
     from portal_b200.host import HostPlayer, HostRenderer, HostScene
     hs = HostScene.from_file(os.path.join(P.ROOT, "tests", "fixtures", "two_spheres.ron"))
@@ -123,14 +123,26 @@ def test_player_16bit_twins_refuse_without_a_device():
     lib = capi.lib()
     p = PhFrameParams(16, 8, 4, 1, 0, 0)
     cap = lib.pe_png_bound_rgba16(16, 8)
-    buf, ln, px = (C.c_uint8 * cap)(), C.c_size_t(), np.empty((8, 16, 4), np.uint16)
-    calls = [lambda: lib.ph_player_render_frame_rgba16(pl._p, hr._ctx, C.byref(p), px.ctypes.data),
-             lambda: lib.ph_player_render_frame_png16(pl._p, hr._ctx, C.byref(p), buf, cap, C.byref(ln)),
-             lambda: lib.ph_player_render_motion_blur_frame_rgba16(pl._p, hr._ctx, C.byref(p), 0, 10, 2, 1.0, px.ctypes.data),
-             lambda: lib.ph_player_render_motion_blur_frame_png16(pl._p, hr._ctx, C.byref(p), 0, 10, 2, 1.0, buf, cap, C.byref(ln))]
-    for k, call in enumerate(calls):
-        assert call() != 0, k
-        assert b"no CPU rendering path" in lib.ph_player_last_error(pl._p), (k, lib.ph_player_last_error(pl._p))
+    assert lib.ph_output_bytes(capi.PH_OUT_PNG, 16, 16, 8) == cap
+    assert lib.ph_output_bytes(capi.PH_OUT_PIXELS, 16, 16, 8) == 16 * 8 * 8
+    assert lib.ph_output_bytes(capi.PH_OUT_PIXELS, 32, 16, 8) == 16 * 8 * 16
+    size = max(cap, 16 * 8 * 16)
+    buf, ln = (C.c_uint8 * size)(), C.c_size_t()
+    mb = C.byref(capi.PhMotionBlur(0, 10, 2, 1.0))
+    cases = [(capi.PH_OUT_PIXELS, 16, None, "no CPU rendering path"), (capi.PH_OUT_PNG, 16, None, "no CPU rendering path"),
+             (capi.PH_OUT_PIXELS, 16, mb, "no CPU rendering path"), (capi.PH_OUT_PNG, 16, mb, "no CPU rendering path"),
+             (capi.PH_OUT_PIXELS, 32, None, "no CPU rendering path"),
+             # refused before any launch
+             (capi.PH_OUT_PIXELS, 32, mb, "motion blur needs bits 8 or 16"), (capi.PH_OUT_PNG, 32, None, "bits must be 8 or 16"),
+             (capi.PH_OUT_PIXELS, 12, None, "bits must be 8, 16 or 32"),
+             (capi.PH_OUT_PIXELS, 16, C.byref(capi.PhMotionBlur(0, 10, 65, 1.0)), "bad frame arguments")]
+    for k, (container, bits, m, want) in enumerate(cases):
+        assert lib.ph_player_render(pl._p, hr._ctx, C.byref(p), m, container, bits, buf, size, C.byref(ln)) != 0, k
+        assert want.encode() in lib.ph_player_last_error(pl._p), (k, lib.ph_player_last_error(pl._p))
+    for container, m in ((capi.PH_OUT_PIXELS, None), (capi.PH_OUT_PIXELS, mb), (capi.PH_OUT_PNG, None), (capi.PH_OUT_PNG, mb)):
+        capacity = lib.ph_output_bytes(container, 16, 16, 8) - 1
+        assert lib.ph_player_render(pl._p, hr._ctx, C.byref(p), m, container, 16, buf, capacity, C.byref(ln)) != 0
+        assert b"below ph_output_bytes" in lib.ph_player_last_error(pl._p)
     pl.close()
     hr.close()
 

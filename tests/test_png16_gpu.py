@@ -2,7 +2,7 @@
 (special floats, every frame count from 1 to 64, ragged pixel counts, 16- and 8-byte aligned buffers); pe_encode_png_rgba16 is
 byte for byte the sequential restatement (tests/host_harness/png16_spec.cpp) on the CPU tests' inputs and on the five config
 scenes at their BASELINE sizes, deterministic, read-only on its input, clear of the caller's scratch slots and ordered on a
-caller's stream; the player's 16-bit twins are unorm16 of the float frames of the same updates (and of the strict oracle's
+caller's stream; the player's 16-bit frames are unorm16 of the float frames of the same updates (and of the strict oracle's
 frame); and the render CLI's 16-bit frames agree across png, rgba and ppm."""
 import ctypes as C
 import os
@@ -183,7 +183,7 @@ def test_player_rgba16_is_unorm16_of_the_strict_oracle_frame(torch_cuda):
 
 
 @pytest.mark.parametrize("adaptive", [False, True])
-def test_player_16bit_twins(torch_cuda, adaptive):
+def test_player_render_16bit(torch_cuda, adaptive):
     hs, hr, pl = _player(os.path.join(ROOT, "tests", "golden", "ron", "portal_in_portal.ron"))
     if adaptive:
         pl.set_adaptive_aa(True, 8)
@@ -196,7 +196,7 @@ def test_player_16bit_twins(torch_cuda, adaptive):
     got = pl.render_frame_rgba16(w, h, depth, aa_count=4)
     assert np.array_equal(got, Q.quantize16(f32))
     p = PhFrameParams(w, h, depth, 4, 0, 0)
-    pl._check(lib.ph_player_render_frame_png16(pl._p, hr._ctx, C.byref(p), buf, cap, C.byref(n)))
+    pl._check(lib.ph_player_render(pl._p, hr._ctx, C.byref(p), None, capi.PH_OUT_PNG, 16, buf, cap, C.byref(n)))
     assert bytes(buf[:n.value]) == Q.spec_png16(got)
     # motion blur, M = 3 at aa 2: the sub-frames of the same update sequence, as floats, quantised and averaged
     an, dur = pl.animations()[0]
@@ -212,7 +212,8 @@ def test_player_16bit_twins(torch_cuda, adaptive):
     assert np.array_equal(got, Q.average16(subs))
     pl.init_animation(an)
     p = PhFrameParams(w, h, depth, 2, 0, 0)
-    pl._check(lib.ph_player_render_motion_blur_frame_png16(pl._p, hr._ctx, C.byref(p), fi, fc, mb, dur, buf, cap, C.byref(n)))
+    pl._check(lib.ph_player_render(pl._p, hr._ctx, C.byref(p), C.byref(capi.PhMotionBlur(fi, fc, mb, dur)), capi.PH_OUT_PNG, 16, buf, cap,
+                                   C.byref(n)))
     assert bytes(buf[:n.value]) == Q.spec_png16(got)
     pl.close()
     hr.close()

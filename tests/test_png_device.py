@@ -95,7 +95,7 @@ def test_png_bound_and_argument_checks_without_a_device():
         lib.pe_destroy(ctx)
 
 
-def test_player_png_twins_refuse_without_a_device():
+def test_player_render_png_refuses_without_a_device():
     import os
     from portal_b200.capi import PhFrameParams
     from portal_b200.host import HostPlayer, HostRenderer, HostScene
@@ -105,10 +105,12 @@ def test_player_png_twins_refuse_without_a_device():
     lib = capi.lib()
     p = PhFrameParams(16, 8, 4, 1, 0, 0)
     cap = lib.pe_png_bound(16, 8)
+    assert lib.ph_output_bytes(capi.PH_OUT_PNG, 8, 16, 8) == cap
     buf, ln = (C.c_uint8 * cap)(), C.c_size_t()
-    assert lib.ph_player_render_frame_png(pl._p, hr._ctx, C.byref(p), buf, cap, C.byref(ln)) != 0
-    assert b"no CPU rendering path" in lib.ph_player_last_error(pl._p)
-    assert lib.ph_player_render_motion_blur_frame_png(pl._p, hr._ctx, C.byref(p), 0, 10, 2, 1.0, buf, cap, C.byref(ln)) != 0
-    assert b"no CPU rendering path" in lib.ph_player_last_error(pl._p)
+    for mb in (None, C.byref(capi.PhMotionBlur(0, 10, 2, 1.0))):
+        for bits, capacity, want in ((8, cap, "no CPU rendering path"), (8, cap - 1, "below ph_output_bytes"),
+                                     (32, cap, "bits must be 8 or 16")):
+            assert lib.ph_player_render(pl._p, hr._ctx, C.byref(p), mb, capi.PH_OUT_PNG, bits, buf, capacity, C.byref(ln)) != 0
+            assert want.encode() in lib.ph_player_last_error(pl._p), (mb, bits, capacity, lib.ph_player_last_error(pl._p))
     pl.close()
     hr.close()

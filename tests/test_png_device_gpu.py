@@ -1,7 +1,7 @@
 """pe_encode_png_rgba8 on the H100: byte for byte the sequential restatement (tests/host_harness/png_spec.cpp) on every input
 the CPU tests check it on, on the five config scenes rendered by the product at their BASELINE sizes and on mobius_monoportal
 at aa 4; deterministic, read-only on its input, clear of the caller's scratch slots and ordered on a caller's stream; the
-player's PNG twins equal the restatement of their RGBA8 twins' frames; and the render CLI's PNG frames are the restatement's
+player's PNG frames equal the restatement of its RGBA8 frames; and the render CLI's PNG frames are the restatement's
 files of the pixels it writes as raw RGBA8."""
 import ctypes as C
 import os
@@ -111,7 +111,7 @@ def _player(torch, adaptive):
 
 
 @pytest.mark.parametrize("adaptive", [False, True])
-def test_player_png_twins(torch_cuda, adaptive):
+def test_player_render_png(torch_cuda, adaptive):
     hs, hr, pl = _player(torch_cuda, adaptive)
     lib = capi.lib()
     w, h = 640, 360
@@ -120,13 +120,14 @@ def test_player_png_twins(torch_cuda, adaptive):
     pl.update(0.0)
     want = P.spec_png(pl.render_frame(w, h, 40, aa_count=4, rgba8=True))
     p = PhFrameParams(w, h, 40, 4, 0, 0)
-    pl._check(lib.ph_player_render_frame_png(pl._p, hr._ctx, C.byref(p), buf, cap, C.byref(n)))
+    pl._check(lib.ph_player_render(pl._p, hr._ctx, C.byref(p), None, capi.PH_OUT_PNG, 8, buf, cap, C.byref(n)))
     assert bytes(buf[:n.value]) == want
     an, dur = pl.animations()[0]
     pl.init_animation(an)
     want = P.spec_png(pl.render_motion_blur_frame(w, h, 40, 3, 30, 3, dur, aa_count=2))
     p = PhFrameParams(w, h, 40, 2, 0, 0)
-    pl._check(lib.ph_player_render_motion_blur_frame_png(pl._p, hr._ctx, C.byref(p), 3, 30, 3, dur, buf, cap, C.byref(n)))
+    mb = capi.PhMotionBlur(3, 30, 3, dur)
+    pl._check(lib.ph_player_render(pl._p, hr._ctx, C.byref(p), C.byref(mb), capi.PH_OUT_PNG, 8, buf, cap, C.byref(n)))
     assert bytes(buf[:n.value]) == want
     pl.close()
     hr.close()

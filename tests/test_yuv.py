@@ -151,7 +151,7 @@ def test_conversion_argument_checks_without_a_device():
         lib.pe_destroy(ctx)
 
 
-def test_player_twins_refuse_without_a_device():
+def test_player_render_yuv420p10_refuses_without_a_device():
     from portal_b200.capi import PhFrameParams
     from portal_b200.host import HostPlayer, HostRenderer, HostScene
     hs = HostScene.from_file(os.path.join(P.ROOT, "tests", "fixtures", "two_spheres.ron"))
@@ -159,18 +159,21 @@ def test_player_twins_refuse_without_a_device():
     pl = HostPlayer(hs)
     lib = capi.lib()
     p = PhFrameParams(16, 8, 4, 1, 0, 0)
-    out = np.empty(lib.pe_yuv420p10_bytes(16, 8) // 2, np.uint16)
-    for bits in (8, 16):
-        calls = [lambda: lib.ph_player_render_frame_yuv420p10(pl._p, hr._ctx, C.byref(p), bits, out.ctypes.data),
-                 lambda: lib.ph_player_render_motion_blur_frame_yuv420p10(pl._p, hr._ctx, C.byref(p), 0, 10, 2, 1.0, bits, out.ctypes.data)]
-        for k, call in enumerate(calls):
-            assert call() != 0, (bits, k)
-            assert b"no CPU rendering path" in lib.ph_player_last_error(pl._p), (bits, k, lib.ph_player_last_error(pl._p))
-    for bits in (0, 10, 32):
-        assert lib.ph_player_render_frame_yuv420p10(pl._p, hr._ctx, C.byref(p), bits, out.ctypes.data) != 0
-        assert b"bits must be 8 or 16" in lib.ph_player_last_error(pl._p)
-        assert lib.ph_player_render_motion_blur_frame_yuv420p10(pl._p, hr._ctx, C.byref(p), 0, 10, 2, 1.0, bits, out.ctypes.data) != 0
-        assert b"bits must be 8 or 16" in lib.ph_player_last_error(pl._p)
+    cap = lib.pe_yuv420p10_bytes(16, 8)
+    out, ln = np.empty(cap // 2, np.uint16), C.c_size_t()
+    render = lambda mb, bits, capacity=cap: lib.ph_player_render(pl._p, hr._ctx, C.byref(p), mb, capi.PH_OUT_YUV420P10, bits,  # noqa: E731
+                                                                 out.ctypes.data, capacity, C.byref(ln))
+    for mb in (None, C.byref(capi.PhMotionBlur(0, 10, 2, 1.0))):
+        for bits in (8, 16):
+            assert lib.ph_output_bytes(capi.PH_OUT_YUV420P10, bits, 16, 8) == cap
+            assert render(mb, bits) != 0, (mb, bits)
+            assert b"no CPU rendering path" in lib.ph_player_last_error(pl._p), (mb, bits, lib.ph_player_last_error(pl._p))
+            assert render(mb, bits, cap - 1) != 0
+            assert b"below ph_output_bytes" in lib.ph_player_last_error(pl._p)
+        for bits in (0, 10, 32):
+            assert lib.ph_output_bytes(capi.PH_OUT_YUV420P10, bits, 16, 8) == 0
+            assert render(mb, bits) != 0
+            assert b"bits must be 8 or 16" in lib.ph_player_last_error(pl._p)
     pl.close()
     hr.close()
 
