@@ -338,6 +338,33 @@ PE_API int pe_encode_png_rgba8(pe_ctx* ctx, const void* rgba8_device, int width,
 PE_API int pe_encode_png_host(pe_ctx* ctx, const void* rgba8_device, int width, int height, uint8_t* png_host,
                               size_t capacity, size_t* size_out);
 
+/* ---- GIF frames encoded on the device (no counterpart in the reference, whose GIFs come from a screen grabber) -------------
+ * DESIGN.md section 5.6, restated sequentially in tests/host_harness/gif_spec.cpp.  One frame block is a pure function of the
+ * RGBA8 frame (alpha ignored) and the delay: a local table of the frame's own colours when it has at most 256 (sorted by
+ * r<<16 | g<<8 | b; lossless), else a median cut of the 6-bit histogram to at most 256 entries with an ordered 8x8 Bayer
+ * dither before the nearest-entry search; a table of 2^k entries, k = max(1, ceil(log2 P)); the index stream LZW-coded in
+ * segments of 16384 indices, each with a fresh dictionary (a Clear code between them); sub-blocks of 255 bytes.  The block is
+ * a Graphic Control Extension (do not dispose, `delay_cs` centiseconds), an image descriptor at 0, 0 of the full frame with
+ * its table, the minimum code size, the sub-blocks and their 0 terminator.  A file is pe_gif_header, the blocks in order and
+ * the trailer byte 0x3B.  The bytes do not depend on the GPU, the stream or scheduling.  The work space is the context's own
+ * (never a pe_scratch_buffer slot); one context encodes on one stream at a time. */
+/* Upper bound of the frame block for a width x height frame; 0 unless 1 <= width, height <= 65535. */
+PE_API size_t pe_gif_frame_bound(int width, int height);
+/* Frame block of a row-major RGBA8 frame in device memory (4-byte aligned), encoded on the device.  Asynchronous on `stream`
+ * (NULL: the context's stream): a memset and six kernel launches.  Writes the block into out_device (capacity >=
+ * pe_gif_frame_bound) and its length into *size_device (uint64).  A bad size, alignment, capacity, a delay outside
+ * 0 .. 65535 or a context without a device are refused before any launch.  The frame is only read. */
+PE_API int pe_encode_gif_frame(pe_ctx* ctx, const void* rgba8_device, int width, int height, int delay_cs, void* out_device,
+                               size_t capacity, void* size_device, void* stream);
+/* Synchronous form on the context's stream: the block lands in host memory; *size_out = its length. */
+PE_API int pe_encode_gif_frame_host(pe_ctx* ctx, const void* rgba8_device, int width, int height, int delay_cs, uint8_t* out_host,
+                                    size_t capacity, size_t* size_out);
+/* The file's header, host only: "GIF89a", the logical screen descriptor (width, height, no global table, colour resolution
+ * bits 7, background 0, aspect 0) and, when `loop` is 1 (an animation), a NETSCAPE2.0 application extension that loops
+ * forever.  Returns the length written (13, or 32 with the loop), 0 for a bad size, a `loop` other than 0 or 1, or a capacity
+ * below that length.  The file ends with the trailer, the single byte 0x3B, after the last frame block. */
+PE_API int pe_gif_header(int width, int height, int loop, uint8_t* out, size_t capacity);
+
 /* ---- 16 bits per channel (opt-in; no counterpart in the reference, whose frames are 8-bit) ---------------------------------
  * For a 10-bit video encode: the float frame of pe_render (or pe_render_adaptive with rgba8 = 0) quantised to unorm16 instead
  * of unorm8.  An RGBA16 pixel is four uint16 (r, g, b, a) in host byte order, 8 B.  Same argument rules as the RGBA8 forms. */

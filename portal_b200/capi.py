@@ -36,7 +36,7 @@ class PhMotionBlur(C.Structure):
                 ("duration_seconds", C.c_double)]
 
 
-PH_OUT_PIXELS, PH_OUT_PNG, PH_OUT_YUV420P10 = 0, 1, 2
+PH_OUT_PIXELS, PH_OUT_PNG, PH_OUT_YUV420P10, PH_OUT_GIF = 0, 1, 2, 3
 
 PE_YUV_BT709, PE_YUV_BT601 = 0, 1
 PE_YUV_SITING_LEFT, PE_YUV_SITING_CENTER = 0, 1
@@ -143,6 +143,10 @@ def lib() -> C.CDLL:
         "pe_png_bound_rgba16": (C.c_size_t, [i32, i32]),
         "pe_encode_png_rgba16": (i32, [vp, vp, i32, i32, vp, C.c_size_t, vp, vp]),
         "pe_encode_png_host_rgba16": (i32, [vp, vp, i32, i32, vp, C.c_size_t, C.POINTER(C.c_size_t)]),
+        "pe_gif_frame_bound": (C.c_size_t, [i32, i32]),
+        "pe_encode_gif_frame": (i32, [vp, vp, i32, i32, i32, vp, C.c_size_t, vp, vp]),
+        "pe_encode_gif_frame_host": (i32, [vp, vp, i32, i32, i32, vp, C.c_size_t, C.POINTER(C.c_size_t)]),
+        "pe_gif_header": (i32, [i32, i32, i32, vp, C.c_size_t]),
         "pe_yuv420p10_bytes": (C.c_size_t, [i32, i32]),
         "pe_rgba_to_yuv420p10": (i32, [vp, vp, i32, i32, i32, vp, vp]),
         "pe_yuv420_bytes": (C.c_size_t, [i32, i32, i32]),
@@ -217,6 +221,7 @@ def lib() -> C.CDLL:
                                    C.POINTER(C.c_size_t)]),
         "ph_player_advance_motion_blur_frame": (i32, [vp, i32, i32, i32, C.c_double]),
         "ph_player_set_adaptive_aa": (i32, [vp, i32, i32]),
+        "ph_player_set_gif_delay": (i32, [vp, i32]),
         "ph_y4m_open": (vp, [cp, i32, cp, C.c_size_t]),
         "ph_y4m_info": (i32, [vp, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(PeYuvFormat),
                               C.POINTER(C.c_int64)]),
@@ -272,6 +277,42 @@ def encode_png16_device(ctx, rgba16) -> bytes:
     if L.pe_encode_png_host_rgba16(ctx, C.c_void_p(rgba16.data_ptr()), w, h, out, cap, C.byref(n)):
         raise PortalB200Error(L.pe_last_error(ctx).decode(errors="replace"))
     return bytes(memoryview(out)[:n.value])
+
+
+def encode_gif_frame(ctx, rgba8, delay_cs: int = 0) -> bytes:
+    """GIF frame block (DESIGN.md section 5.6) of a CUDA uint8 tensor [h, w, 4] (contiguous) encoded on the device by
+    pe_encode_gif_frame on context `ctx`, ordered after the work already queued on the current torch stream.  A file is
+    gif_header(w, h, loop) + the blocks + b"\\x3b"."""
+    import torch
+    if rgba8.dim() != 3 or rgba8.shape[2] != 4 or not rgba8.is_cuda or rgba8.dtype != torch.uint8 or not rgba8.is_contiguous():
+        raise ValueError("frame must be a contiguous CUDA uint8 tensor [h, w, 4]")
+    L = lib()
+    h, w = int(rgba8.shape[0]), int(rgba8.shape[1])
+    cap = L.pe_gif_frame_bound(w, h)
+    if cap == 0:
+        raise PortalB200Error(f"pe_gif_frame_bound: no GIF frame for a {w} x {h} frame")
+    out = torch.empty(cap, dtype=torch.uint8, device=rgba8.device)
+    size = torch.empty(1, dtype=torch.int64, device=rgba8.device)
+    # the read-backs go on the same stream handle (0, torch's default stream, names the context's stream)
+    stream = C.c_void_p(torch.cuda.current_stream(rgba8.device).cuda_stream)
+    n = C.c_uint64()
+    if (L.pe_encode_gif_frame(ctx, C.c_void_p(rgba8.data_ptr()), w, h, int(delay_cs), C.c_void_p(out.data_ptr()), cap,
+                              C.c_void_p(size.data_ptr()), stream)
+            or L.pe_memcpy_d2h(ctx, C.addressof(n), C.c_void_p(size.data_ptr()), 8, stream)):
+        raise PortalB200Error(L.pe_last_error(ctx).decode(errors="replace"))
+    host = (C.c_uint8 * max(1, n.value))()
+    if L.pe_memcpy_d2h(ctx, host, C.c_void_p(out.data_ptr()), n.value, stream):
+        raise PortalB200Error(L.pe_last_error(ctx).decode(errors="replace"))
+    return bytes(host[:n.value])
+
+
+def gif_header(width: int, height: int, loop: bool) -> bytes:
+    """The GIF file header pe_gif_header writes: GIF89a, the logical screen descriptor and, for an animation, the loop block."""
+    buf = (C.c_uint8 * 64)()
+    n = lib().pe_gif_header(width, height, 1 if loop else 0, buf, 64)
+    if n == 0:
+        raise PortalB200Error(f"pe_gif_header: no GIF header for a {width} x {height} frame")
+    return bytes(buf[:n])
 
 
 def yuv420p10_planes(buf, width: int, height: int):

@@ -4,15 +4,15 @@
 //   portal_b200_render render-frame <scene.ron> [--width W] [--height H] [--render-depth D] [--aa-count N]
 //                      [--time T] [--stage NAME] [--animation NAME] [--camera NAME] [--device K]
 //                      [--texture name=file.png | name=file.rgba:WxH ...] [--assets DIR] [--output out.png|.ppm|.rgba]
-//                      [--adaptive-aa T] [--bit-depth 8|16]                              (also --output out.y4m)
+//                      [--adaptive-aa T] [--bit-depth 8|16]                   (also --output out.y4m | out.gif)
 //                      [--video name=clip.y4m ...] [--video-matrix bt709|bt601]
 //   portal_b200_render render <scene.ron> [--animations a,b,... | --starts-with PREFIX] [--fps N] [--motion-blur-frames M] [--width W]
 //                      [--height H] [--render-depth D] [--aa-count N] [--stereo-image] [--no-skip-existing] [--out-dir DIR] [--max-frames K]
-//                      [--frame-format ppm|png|rgba|y4m] [--assets DIR] [--adaptive-aa T] [--bit-depth 8|16]
+//                      [--frame-format ppm|png|rgba|y4m|gif] [--assets DIR] [--adaptive-aa T] [--bit-depth 8|16]
 //                      [--video name=clip.y4m ...] [--video-matrix bt709|bt601]
 //                      (`portal render`, main.rs:2808-2873 -> render_named_animations :1876-1930 ->
 //                       render_animation :1757-1830; frames are written as DIR/<animation>/frame_<i>.<format>, or as one
-//                       Y4M stream DIR/<animation>.y4m; the HEVC encode itself is out of scope)
+//                       stream DIR/<animation>.y4m or DIR/<animation>.gif; the HEVC encode itself is out of scope)
 //
 // --adaptive-aa T (not in the reference; off by default): every frame / sub-frame is traced with one sample, and with all
 // --aa-count samples only where that frame has an edge (a 3x3 unorm8 range above T, pe_render_adaptive).
@@ -29,6 +29,16 @@
 // skips an animation whose stream exists (as the reference skips an existing .mov, main.rs:1771-1779); --out-dir - writes the
 // stream of the one selected animation to stdout, with every status line on stderr.  render-frame writes a one-frame stream
 // at 25 fps.
+//
+// --frame-format gif / --output *.gif (not in the reference, whose user records its window with a screen grabber to make
+// GIFs): every RGBA8 frame encoded on the device into one GIF frame block (pe_encode_gif_frame; DESIGN.md section 5.6: a
+// local table of the frame's own colours, or a median cut with an ordered dither past 256 of them, and segmented LZW).
+// `render` writes one stream per animation, DIR/<animation>.gif, exactly as a Y4M stream (a .part file renamed when complete,
+// skip-existing, --out-dir - for stdout, written in frame order by the main thread): the header with a NETSCAPE2.0 block that
+// loops forever, the blocks, the trailer.  Frame i shows for round(100 (i + 1) / fps) - round(100 i / fps) centiseconds
+// (halves up), so that n frames last round(100 n / fps) cs; --fps above 50 is refused, as browsers show a delay below 2 cs
+// as 10 cs.  render-frame writes a one-frame file without the loop block, delay 0.  GIF is 8-bit: --bit-depth 16 is refused,
+// and so is a frame wider or taller than 65535 pixels.
 //
 // Output: the RGBA8 frame the reference hands to export_png (main.rs:2939-2943) as a PNG when the name ends in .png (encoded
 // on the device: pe_encode_png_rgba8), as raw RGBA8 for .rgba, else as a binary PPM (P6, alpha dropped).  Every format is one
@@ -51,8 +61,8 @@
 // player, clip handles and pinned buffers, and runs the whole loop: frame i of an animation is rendered by worker i mod N and
 // replayed by every other one (ph_player_advance_motion_blur_frame), so that camera teleportation through portals -- state that
 // carries from frame to frame -- is the sequential one everywhere.  Skip-existing decides from one snapshot of the output taken
-// before the workers start.  Frame files are written by their worker; a Y4M stream by the main thread, in frame order, with at
-// most two frames per worker in flight.  Status lines come in frame order, as from one worker.  The first failure stops every
+// before the workers start.  Frame files are written by their worker; a Y4M or GIF stream by the main thread, in frame order,
+// with at most two frames per worker in flight.  Status lines come in frame order, as from one worker.  The first failure stops every
 // worker at its next frame boundary, exits 1 and renames no stream.  render-frame takes one entry.
 #include <dirent.h>
 #include <sys/stat.h>
@@ -99,9 +109,28 @@ static bool write_y4m_frame(FILE* f, const std::vector<uint8_t>& planes) {
     return std::fputs("FRAME\n", f) >= 0 && std::fwrite(planes.data(), 1, planes.size(), f) == planes.size();
 }
 
+// GIF: pe_gif_header (with the loop block for an animation), then the frame blocks as ph_player_render returns them, then the
+// trailer
+static bool write_gif_header(FILE* f, int width, int height, bool loop) {
+    uint8_t h[64];
+    const int n = pe_gif_header(width, height, loop ? 1 : 0, h, sizeof h);
+    return n > 0 && std::fwrite(h, 1, size_t(n), f) == size_t(n);
+}
+static bool write_gif_block(FILE* f, const std::vector<uint8_t>& block) {
+    return std::fwrite(block.data(), 1, block.size(), f) == block.size();
+}
+static bool write_gif_trailer(FILE* f) { return std::fputc(0x3B, f) != EOF; }
+
+// Centiseconds frame i of a GIF stream at `fps` shows for: round(100 (i + 1) / fps) - round(100 i / fps), halves up, so that
+// the first n frames last round(100 n / fps)
+static int gif_delay(int i, int fps) {
+    auto r = [fps](long long j) { return (200 * j + fps) / (2LL * fps); };
+    return int(r(i + 1) - r(i));
+}
+
 // How a frame becomes output, decided once from --output / --frame-format and --bit-depth: what ph_player_render delivers (the
 // container, rendered at `bits`) and how those bytes become a file
-enum FrameFile { AS_RETURNED, PPM, Y4M };
+enum FrameFile { AS_RETURNED, PPM, Y4M, GIF };
 struct FrameFormat {
     FrameFile file;
     int container, bits;
@@ -109,12 +138,14 @@ struct FrameFormat {
 
 // One frame as ph_player_render returned it (`len` bytes of `px`) -> the file `path`: the bytes as they are (PNG; raw RGBA8, or
 // RGBA16 in host byte order, which is little-endian), a P6 PPM with alpha dropped (maxval 255, or 65535 with big-endian samples,
-// as the format defines), or a one-frame Y4M stream at 25 fps
+// as the format defines), a one-frame Y4M stream at 25 fps, or a one-frame GIF (no loop block)
 static bool write_frame(const std::string& path, const FrameFormat& fmt, const std::vector<uint8_t>& px, size_t len, int width, int height) {
-    if (fmt.file == Y4M) {
+    if (fmt.file == Y4M || fmt.file == GIF) {
         FILE* f = std::fopen(path.c_str(), "wb");
         if (!f) return false;
-        const bool ok = write_y4m_header(f, width, height, 25) && write_y4m_frame(f, px);
+        const bool ok = fmt.file == Y4M ? write_y4m_header(f, width, height, 25) && write_y4m_frame(f, px)
+                                        : write_gif_header(f, width, height, false) &&
+                                              std::fwrite(px.data(), 1, len, f) == len && write_gif_trailer(f);
         return std::fclose(f) == 0 && ok;
     }
     std::ofstream out(path, std::ios::binary);
@@ -293,7 +324,7 @@ struct Worker {
     VideoState video_state;                           // the player's update hook points here: workers never move
     std::vector<uint8_t> px;                          // the frame as ph_player_render returns it
     size_t len = 0;                                   // its bytes
-    std::vector<std::vector<uint8_t>> free_planes;   // `render` to Y4M: the plane buffers the main thread does not hold
+    std::vector<std::vector<uint8_t>> free_planes;   // `render` to a stream: the frame buffers the main thread does not hold
 };
 
 // What `render` does with one entry of the animation list, decided before any worker starts
@@ -301,7 +332,7 @@ struct AnimationPlan {
     bool rendered = false;           // false: --starts-with filters it out (it is still initialised and updated once)
     double duration = 0.0;           // the f32 duration render_animation takes
     int count = 1, todo = 0;         // frames of the animation, frames to render (--max-frames)
-    bool skip_stream = false;        // Y4M: the stream exists
+    bool skip_stream = false;        // Y4M or GIF: the stream exists
     std::vector<char> skip_frame;    // frame files: frame i exists
 };
 
@@ -311,7 +342,7 @@ struct Shared {
     std::condition_variable cv;
     bool stop = false;
     std::string error;
-    // (animation, frame) -> the frame's Y4M planes (empty for the other formats); frame -1: the animation has begun
+    // (animation, frame) -> the frame's Y4M planes or GIF block (empty for frame files); frame -1: the animation has begun
     std::map<std::pair<size_t, int>, std::vector<uint8_t>> done;
 
     void fail(const std::string& why) {
@@ -360,9 +391,9 @@ int main(int argc, char** argv) {
     const bool anim_cmd = argc >= 3 && std::strcmp(argv[1], "render") == 0;
     if (!frame_cmd && !anim_cmd) {
         std::fprintf(stderr, "usage: %s render-frame <scene.ron> [--width W] [--height H] [--render-depth D] [--aa-count N] [--time T] "
-                             "[--stage NAME] [--animation NAME] [--camera NAME] [--device K] [--texture name=file.png|name=file.rgba:WxH] [--assets DIR] [--output out.png|.ppm|.rgba|.y4m] [--adaptive-aa T] [--bit-depth 8|16] [--video name=clip.y4m] [--video-matrix bt709|bt601]\n"
+                             "[--stage NAME] [--animation NAME] [--camera NAME] [--device K] [--texture name=file.png|name=file.rgba:WxH] [--assets DIR] [--output out.png|.ppm|.rgba|.y4m|.gif] [--adaptive-aa T] [--bit-depth 8|16] [--video name=clip.y4m] [--video-matrix bt709|bt601]\n"
                              "       %s render <scene.ron> [a,b | --animations a,b | --starts-with PREFIX] [--fps N] [--motion-blur-frames M] [--width W] [--height H] "
-                             "[--render-depth D] [--aa-count N] [--stereo-image] [--no-skip-existing] [--out-dir DIR] [--max-frames K] [--frame-format ppm|png|rgba|y4m] [--adaptive-aa T] [--bit-depth 8|16] [--video name=clip.y4m] [--video-matrix bt709|bt601] [--device K | --devices K,K,...]\n", argv[0], argv[0]);
+                             "[--render-depth D] [--aa-count N] [--stereo-image] [--no-skip-existing] [--out-dir DIR] [--max-frames K] [--frame-format ppm|png|rgba|y4m|gif] [--adaptive-aa T] [--bit-depth 8|16] [--video name=clip.y4m] [--video-matrix bt709|bt601] [--device K | --devices K,K,...]\n", argv[0], argv[0]);
         return 2;
     }
     std::string scene_path = argv[2], output = "frame.ppm", out_dir = "video";
@@ -407,7 +438,7 @@ int main(int argc, char** argv) {
             video_matrix = v == "bt601" ? PE_YUV_BT601 : PE_YUV_BT709;
         }
         else if (a == "--assets") assets = next();
-        else if (a == "--frame-format") frame_ext = std::string(".") + next();          // render: ppm (default) | png | rgba | y4m
+        else if (a == "--frame-format") frame_ext = std::string(".") + next();          // render: ppm (default) | png | rgba | y4m | gif
         else if (a == "--adaptive-aa" || a == "--adaptive_aa") {
             const char* v = next();
             char* end = nullptr;
@@ -460,11 +491,27 @@ int main(int argc, char** argv) {
     auto format_is = [&](const char* ext) { return frame_cmd ? ends_with(output, ext) : frame_ext == ext; };
     const FrameFormat fmt = format_is(".png")   ? FrameFormat{AS_RETURNED, PH_OUT_PNG, bits}   // Image::export_png (main.rs:2939-2943)
                             : format_is(".y4m") ? FrameFormat{Y4M, PH_OUT_YUV420P10, bits}
+                            : format_is(".gif") ? FrameFormat{GIF, PH_OUT_GIF, bits}
                                                 : FrameFormat{ends_with(frame_cmd ? output : frame_ext, ".rgba") ? AS_RETURNED : PPM, PH_OUT_PIXELS, bits};
-    const bool to_stdout = anim_cmd && fmt.file == Y4M && out_dir == "-";
+    const bool stream = anim_cmd && (fmt.file == Y4M || fmt.file == GIF);    // one file per animation, not per frame
+    const std::string stream_ext = fmt.file == GIF ? ".gif" : ".y4m";
+    const bool to_stdout = stream && out_dir == "-";
     if (to_stdout && selected != 1) {
-        std::fprintf(stderr, "--out-dir - writes one Y4M stream to stdout: select exactly one animation (%zu selected)\n", selected);
+        std::fprintf(stderr, "--out-dir - writes one %s stream to stdout: select exactly one animation (%zu selected)\n", fmt.file == GIF ? "GIF" : "Y4M", selected);
         return 2;
+    }
+    if (fmt.file == GIF) {                          // refused before any context exists
+        if (bits != 8) { std::fprintf(stderr, "GIF frames are 8-bit: --bit-depth 16 cannot be written as GIF\n"); return 2; }
+        if (anim_cmd && fps > 50) {
+            std::fprintf(stderr, "--fps %d is above 50: GIF delays are whole centiseconds and browsers show a delay below 2 cs as 10 cs; use --fps 50, 33 or 25\n", fps);
+            return 2;
+        }
+        if (fps < 1 && anim_cmd) { std::fprintf(stderr, "--fps must be at least 1 for GIF, got %d\n", fps); return 2; }
+        const long long gif_w = stereo && anim_cmd ? 2LL * width : width;
+        if (gif_w < 1 || height < 1 || gif_w > 65535 || height > 65535) {
+            std::fprintf(stderr, "a GIF frame is 1 .. 65535 pixels wide and high, got %lld x %d%s\n", gif_w, height, stereo && anim_cmd ? " (stereo doubles the width)" : "");
+            return 2;
+        }
     }
     FILE* status = to_stdout ? stderr : stdout;     // stdout carries the stream
     // --video name=clip.y4m: every clip is opened (and refused) before a context exists
@@ -599,15 +646,15 @@ int main(int argc, char** argv) {
         if (const int rc = set_up(workers[w], w == 0)) return rc;
     }
     if (stereo) width *= 2;         // side-by-side eyes, doubled width
-    // one buffer per worker for the frame (`render` to Y4M: two for its planes, which travel to the main thread and back)
+    // one buffer per worker for the frame (`render` to a stream: two, which travel to the main thread and back)
     const size_t frame_bytes = ph_output_bytes(fmt.container, fmt.bits, width, height);
     if (!frame_bytes) {
-        static const char* const what[] = {"image", "PNG", "Y4M stream"};
+        static const char* const what[] = {"image", "PNG", "Y4M stream", "GIF frame"};
         std::fprintf(stderr, "no %s for a %d x %d frame\n", what[fmt.container], width, height);
         return 1;
     }
     for (Worker& wk : workers) {
-        if (anim_cmd && fmt.file == Y4M) wk.free_planes.assign(2, std::vector<uint8_t>(frame_bytes));
+        if (stream) wk.free_planes.assign(2, std::vector<uint8_t>(frame_bytes));
         else wk.px.resize(frame_bytes);
     }
     ph_frame_params p = {width, height, depth, aa, 0, 0, {0, 0, 0}, 0, 0, 0};
@@ -642,10 +689,10 @@ int main(int argc, char** argv) {
             a.todo = max_frames >= 0 && max_frames < a.count ? max_frames : a.count;
             a.skip_frame.assign(size_t(a.todo), 0);
             if (!a.rendered || to_stdout) continue;
-            if (fmt.file == Y4M) {
-                const std::string stream = out_dir + "/" + names[k] + ".y4m";
-                a.skip_stream = skip_existing && (file_exists(stream) || to_write.count(stream));     // main.rs:1771-1779
-                if (!a.skip_stream) to_write.insert(stream);
+            if (stream) {
+                const std::string file = out_dir + "/" + names[k] + stream_ext;
+                a.skip_stream = skip_existing && (file_exists(file) || to_write.count(file));         // main.rs:1771-1779
+                if (!a.skip_stream) to_write.insert(file);
                 continue;
             }
             for (int i = 0; i < a.todo; i++) {
@@ -669,9 +716,9 @@ int main(int argc, char** argv) {
                 const AnimationPlan& a = plan[k];
                 if (!a.rendered) continue;
                 if (me == 0) sh.post(k, -1, {});
-                if (fmt.file == Y4M && a.skip_stream) continue;
+                if (stream && a.skip_stream) continue;
                 const std::string dir = out_dir + "/" + names[k];
-                if (fmt.file != Y4M && !make_dirs(dir)) { sh.fail("cannot create " + dir); return; }
+                if (!stream && !make_dirs(dir)) { sh.fail("cannot create " + dir); return; }
                 for (int i = 0; i < a.todo; i++) {
                     if (sh.stopped()) return;
                     if (a.skip_frame[size_t(i)]) continue;                 // neither rendered nor advanced, as the sequential loop
@@ -679,15 +726,18 @@ int main(int argc, char** argv) {
                         if (ph_player_advance_motion_blur_frame(wk.player, i, a.count, motion_blur, a.duration)) { sh.fail(ph_player_last_error(wk.player)); return; }
                         continue;
                     }
-                    std::vector<uint8_t> planes;                           // Y4M: the frame goes to the main thread
-                    if (fmt.file == Y4M && !sh.take_buffer(wk, planes)) return;
-                    std::vector<uint8_t>& buf = fmt.file == Y4M ? planes : wk.px;
+                    std::vector<uint8_t> planes;                           // a stream: the frame goes to the main thread
+                    if (stream && !sh.take_buffer(wk, planes)) return;
+                    if (stream) planes.resize(frame_bytes);                // a GIF block came back cut to its length
+                    std::vector<uint8_t>& buf = stream ? planes : wk.px;
                     const ph_motion_blur mb = {i, a.count, motion_blur, a.duration};
-                    if (ph_player_render(wk.player, wk.ctx, &p, &mb, fmt.container, fmt.bits, buf.data(), buf.size(), &wk.len)) {
+                    if ((fmt.file == GIF && ph_player_set_gif_delay(wk.player, gif_delay(i, fps))) ||
+                        ph_player_render(wk.player, wk.ctx, &p, &mb, fmt.container, fmt.bits, buf.data(), buf.size(), &wk.len)) {
                         sh.fail(ph_player_last_error(wk.player));
                         return;
                     }
-                    if (fmt.file != Y4M) {
+                    if (fmt.file == GIF) planes.resize(wk.len);
+                    if (!stream) {
                         const std::string name = dir + "/frame_" + std::to_string(i) + frame_ext;
                         if (!write_frame(name, fmt, wk.px, wk.len, width, height)) { sh.fail("cannot write " + name); return; }
                     }
@@ -697,7 +747,7 @@ int main(int argc, char** argv) {
         };
         std::vector<std::thread> threads;
         for (size_t w = 0; w < workers.size(); w++) threads.emplace_back(run_worker, w);
-        // The main thread: status lines and Y4M streams, in frame order
+        // The main thread: status lines and Y4M / GIF streams, in frame order
         std::vector<uint8_t> planes;
         for (size_t k = 0; k < names.size(); k++) {
             const AnimationPlan& a = plan[k];
@@ -705,28 +755,29 @@ int main(int argc, char** argv) {
             if (!sh.take(k, -1, planes)) break;
             std::fprintf(status, "Rendering animation %s, %zu/%zu\n", names[k].c_str(), k + 1, names.size());
             bool stopped = false;
-            if (fmt.file == Y4M) {
+            if (stream) {
                 // one stream per animation, written under a temporary name and renamed when complete, so that an interrupted
                 // run leaves no stream for skip-existing to take as done
-                const std::string stream = out_dir + "/" + names[k] + ".y4m", part = stream + ".part";
+                const std::string file = out_dir + "/" + names[k] + stream_ext, part = file + ".part";
                 if (a.skip_stream) {
                     std::fprintf(status, "Skip `%s`, because it's already exists\n", names[k].c_str());
                     continue;
                 }
                 if (!to_stdout && !make_dirs(out_dir)) { sh.fail("cannot create " + out_dir); break; }
                 FILE* f = to_stdout ? stdout : std::fopen(part.c_str(), "wb");
-                bool ok_stream = f && write_y4m_header(f, width, height, fps);
+                bool ok_stream = f && (fmt.file == GIF ? write_gif_header(f, width, height, true) : write_y4m_header(f, width, height, fps));
                 for (int i = 0; i < a.todo && ok_stream; i++) {
                     if (!sh.take(k, i, planes)) { stopped = true; break; }
-                    ok_stream = write_y4m_frame(f, planes);
+                    ok_stream = fmt.file == GIF ? write_gif_block(f, planes) : write_y4m_frame(f, planes);
                     sh.give_back(workers[size_t(i) % workers.size()], planes);
                     std::fprintf(status, "\r%d/%d done      ", i + 1, a.count);
                     std::fflush(status);
                 }
+                if (ok_stream && !stopped && fmt.file == GIF) ok_stream = write_gif_trailer(f);
                 if (f) ok_stream = (to_stdout ? std::fflush(f) : std::fclose(f)) == 0 && ok_stream;
                 if (stopped) break;                                        // the stream keeps its .part name
-                if (!ok_stream || (!to_stdout && std::rename(part.c_str(), stream.c_str()) != 0)) {
-                    sh.fail(std::string("cannot write ") + (to_stdout ? "the stream to stdout" : stream.c_str()));
+                if (!ok_stream || (!to_stdout && std::rename(part.c_str(), file.c_str()) != 0)) {
+                    sh.fail(std::string("cannot write ") + (to_stdout ? "the stream to stdout" : file.c_str()));
                     break;
                 }
                 std::fprintf(status, "\n");

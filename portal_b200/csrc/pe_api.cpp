@@ -1279,6 +1279,76 @@ int pe_encode_png_host_rgba16(pe_ctx* c, const void* rgba16, int width, int heig
     return c ? encode_png_host(c, "pe_encode_png_host_rgba16", "pe_encode_png_rgba16", 8, rgba16, width, height, png_host, capacity, size_out) : 1;
 }
 
+// ------------------------------------------------------------------------------ GIF frame blocks (pe_gif.cu)
+size_t pe_gif_frame_bound(int width, int height) { return gif_frame_bound(width, height); }
+
+int pe_gif_header(int width, int height, int loop, uint8_t* out, size_t capacity) {
+    if (!out || !gif_frame_bound(width, height) || (loop != 0 && loop != 1)) return 0;
+    const uint8_t lsd[13] = {'G', 'I', 'F', '8', '9', 'a', uint8_t(width), uint8_t(width >> 8), uint8_t(height), uint8_t(height >> 8), 0x70, 0, 0};
+    const uint8_t netscape[19] = {0x21, 0xFF, 0x0B, 'N', 'E', 'T', 'S', 'C', 'A', 'P', 'E', '2', '.', '0', 0x03, 0x01, 0x00, 0x00, 0x00};
+    const size_t n = loop ? 32 : 13;
+    if (capacity < n) return 0;
+    std::memcpy(out, lsd, 13);
+    if (loop) std::memcpy(out + 13, netscape, 19);
+    return int(n);
+}
+
+}  // extern "C"
+
+namespace {
+
+// The checks every GIF entry point makes before anything is allocated or launched
+bool check_gif(pe_ctx* c, const std::string& fn, int width, int height, int delay_cs, size_t capacity) {
+    if (!gif_frame_bound(width, height))
+        return !c->fail(fn + ": invalid size " + std::to_string(width) + " x " + std::to_string(height) + " (1 <= width, height <= 65535)");
+    if (delay_cs < 0 || delay_cs > 65535) return !c->fail(fn + ": delay " + std::to_string(delay_cs) + " cs is outside 0 .. 65535");
+    const size_t bound = gif_frame_bound(width, height);
+    if (capacity < bound) return !c->fail(fn + ": capacity " + std::to_string(capacity) + " is below pe_gif_frame_bound = " + std::to_string(bound));
+    return true;
+}
+
+int encode_gif(pe_ctx* c, const void* rgba, int width, int height, int delay_cs, void* out, size_t capacity, void* size_device, void* stream) {
+    const std::string fn = "pe_encode_gif_frame";
+    if (!rgba || !out || !size_device) return c->fail(fn + ": null argument");
+    if (!check_gif(c, fn, width, height, delay_cs, capacity)) return 1;
+    if (uintptr_t(rgba) & 3) return c->fail(fn + ": the frame must be 4-byte aligned");
+    if (!bind_device(c)) return 1;
+    if (!cuda_ok(c, c->gif_work.ensure(gif_workspace_bytes(width, height)), "cudaMalloc(GIF work space)")) return 1;
+    if (!cuda_ok(c, (cudaError_t)launch_gif_encode(rgba, width, height, delay_cs, c->gif_work.dev, out, size_device, stream_of(c, stream)), fn.c_str()))
+        return 1;
+    c->launches += 6;
+    return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int pe_encode_gif_frame(pe_ctx* c, const void* rgba8, int width, int height, int delay_cs, void* out, size_t capacity, void* size_device,
+                        void* stream) {
+    return c ? encode_gif(c, rgba8, width, height, delay_cs, out, capacity, size_device, stream) : 1;
+}
+
+int pe_encode_gif_frame_host(pe_ctx* c, const void* rgba8, int width, int height, int delay_cs, uint8_t* out_host, size_t capacity,
+                             size_t* size_out) {
+    if (!c) return 1;
+    const std::string fn = "pe_encode_gif_frame_host";
+    if (!rgba8 || !out_host || !size_out) return c->fail(fn + ": null argument");
+    if (!check_gif(c, fn, width, height, delay_cs, capacity)) return 1;
+    if (uintptr_t(rgba8) & 3) return c->fail(fn + ": the frame must be 4-byte aligned");
+    if (!bind_device(c)) return 1;
+    const size_t bound = gif_frame_bound(width, height);
+    if (!cuda_ok(c, c->gif_block.ensure(bound), "cudaMalloc(GIF block)") || !cuda_ok(c, c->gif_size.ensure(8), "cudaMalloc(GIF length)")) return 1;
+    if (encode_gif(c, rgba8, width, height, delay_cs, c->gif_block.dev, c->gif_block.bytes, c->gif_size.dev, nullptr)) return 1;
+    uint64_t n = 0;
+    if (!cuda_ok(c, cudaMemcpyAsync(&n, c->gif_size.dev, 8, cudaMemcpyDeviceToHost, c->stream), fn.c_str()) ||
+        !cuda_ok(c, cudaStreamSynchronize(c->stream), fn.c_str()) ||
+        !cuda_ok(c, cudaMemcpyAsync(out_host, c->gif_block.dev, size_t(n), cudaMemcpyDeviceToHost, c->stream), fn.c_str()) ||
+        !cuda_ok(c, cudaStreamSynchronize(c->stream), fn.c_str())) return 1;
+    *size_out = size_t(n);
+    return 0;
+}
+
 // ------------------------------------------------------------------------------ Y'CbCr 4:2:0, 10 bits (pe_yuv.cu)
 size_t pe_yuv420p10_bytes(int width, int height) { return yuv420p10_bytes(width, height); }
 

@@ -106,6 +106,9 @@ struct pe_ctx {
     // pe_encode_png_rgba8's work space: filtered stream, per-segment deflate output, segment sizes / offsets / checksums; and
     // pe_encode_png_host's device copy of the file and its length
     pe_host::DeviceBuffer png_work, png_file, png_size;
+    // pe_encode_gif_frame's work space: occupancy bitmap, histogram, palette, index stream, per-segment LZW output, segment
+    // bit lengths / offsets; and pe_encode_gif_frame_host's device copy of the block and its length
+    pe_host::DeviceBuffer gif_work, gif_block, gif_size;
     // pe_set_texture_yuv420's device copy of the Y'CbCr planes it converts
     pe_host::DeviceBuffer yuv_upload;
     // adaptive de-specialisation: a slot whose value differed between renders more than kMaxRespecialisations times is read

@@ -38,6 +38,17 @@ size_t png_workspace_bytes(int width, int height, int bpp);
 // Enqueue the five kernels: frame -> PNG file at `png` (capacity >= png_bound), its length in *(uint64*)size_out.
 int launch_png_encode(const void* rgba, int width, int height, int bpp, void* work, void* png, void* size_out, cudaStream_t s);
 
+// GIF frame blocks on the device (pe_gif.cu; the encoding is tests/host_harness/gif_spec.cpp, DESIGN.md section 5.6): the index
+// stream is LZW-coded in segments of kGifSegment indices, each with a fresh dictionary.
+constexpr size_t kGifSegment = 16384;
+// Upper bound of the frame block for a width x height frame; 0 unless 1 <= width, height <= 65535.
+size_t gif_frame_bound(int width, int height);
+// Bytes of device work space launch_gif_encode needs for a width x height frame (256-byte aligned base).
+size_t gif_workspace_bytes(int width, int height);
+// Enqueue a memset and the six kernels: RGBA8 frame -> frame block at `block` (capacity >= gif_frame_bound) with the GCE delay
+// `delay` (centiseconds), its length in *(uint64*)size_out.
+int launch_gif_encode(const void* rgba, int width, int height, int delay, void* work, void* block, void* size_out, cudaStream_t s);
+
 // RGB -> Y'CbCr 4:2:0 at 10 bits (pe_yuv.cu; DESIGN.md section 5.4).  Bytes of the Y, Cb, Cr planes of a width x height frame,
 // 0 when the size is invalid or the frame has more than 2^31 - 1 pixels.
 size_t yuv420p10_bytes(int width, int height);

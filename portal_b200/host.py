@@ -294,6 +294,20 @@ class HostPlayer:
         out = self._render(capi.PH_OUT_YUV420P10, int(bits), width, height, depth, aa_count, motion_blur=mb)
         return capi.yuv420p10_planes(out.view(np.uint16), width, height)
 
+    def set_gif_delay(self, delay_cs: int):
+        """The Graphic Control Extension delay (centiseconds) of the next GIF frame blocks."""
+        self._check(self._lib.ph_player_set_gif_delay(self._p, int(delay_cs)))
+
+    def render_frame_gif(self, width, height, depth, aa_count=1, aa_start=0) -> bytes:
+        """The frame of render_frame (rgba8=True) as one GIF frame block encoded on the device (DESIGN.md section 5.6)."""
+        return self._render(capi.PH_OUT_GIF, 8, width, height, depth, aa_count, aa_start).tobytes()
+
+    def render_motion_blur_frame_gif(self, width, height, depth, frame_index, frame_count, motion_blur_frames, duration_seconds,
+                                     aa_count=1) -> bytes:
+        """render_motion_blur_frame as one GIF frame block."""
+        mb = (frame_index, frame_count, motion_blur_frames, float(duration_seconds))
+        return self._render(capi.PH_OUT_GIF, 8, width, height, depth, aa_count, motion_blur=mb).tobytes()
+
 
 class HostRenderer:
     """SceneRenderer::new + render_frame over the C API only (no scene IR involved)."""
