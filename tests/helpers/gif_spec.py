@@ -130,6 +130,88 @@ def exact_colours(n: int, h: int, w: int, seed: int) -> np.ndarray:
     return px.reshape(h, w, 4)
 
 
+def bin_colours(bins, times=1) -> np.ndarray:
+    """All 64 RGB colours of each 6-bit bin (r, g, b) of `bins`, bin i's `times[i]` times (or `times` each): [m, 3] uint8."""
+    off = np.stack(np.meshgrid(range(4), range(4), range(4), indexing="ij"), axis=-1).reshape(64, 3)
+    times = np.broadcast_to(times, (len(bins),))
+    return np.concatenate([np.tile(4 * np.array(b) + off, (t, 1)) for b, t in zip(bins, times)]).astype(np.uint8)
+
+
+def shuffled_frame(rgb: np.ndarray, w: int, seed: int) -> np.ndarray:
+    """An RGBA8 frame [m / w, w, 4] of the colours `rgb` [m, 3] (m a multiple of w) in random places, alpha random."""
+    rng = np.random.default_rng(seed)
+    rgb = rgb[rng.permutation(len(rgb))]
+    assert len(rgb) % w == 0
+    px = np.concatenate([rgb, rng.integers(0, 256, size=(len(rgb), 1))], axis=1).astype(np.uint8)
+    return px.reshape(-1, w, 4)
+
+
+def exact_with(n: int, h: int, w: int, seed: int, include) -> np.ndarray:
+    """An RGBA8 frame [h, w, 4] of exactly n distinct RGB colours that include the colours `include` (0xRRGGBB)."""
+    rng = np.random.default_rng(seed)
+    others = np.setdiff1d(rng.choice(1 << 24, size=n + len(include), replace=False), include)[:n - len(include)]
+    cols = np.concatenate([np.array(include, np.int64), others])
+    pick = np.concatenate([np.arange(n), rng.integers(0, n, size=h * w - n)])
+    c = cols[rng.permutation(pick)]
+    return np.stack([c >> 16, (c >> 8) & 255, c & 255, rng.integers(0, 256, size=h * w)], axis=-1).astype(np.uint8).reshape(h, w, 4)
+
+
+def adversarial_inputs() -> dict:
+    """Frames built to reach the palette stage's edges (tests/test_gif_reference.py asserts that each one does):
+      - more than 256 colours in few occupied bins: the median cut stops early (P = 5, P = 8), the table is zero-padded, and
+        in `5_bins_near_black` black is nearer than every real entry to some dithered pixels, so a search over the padding
+        would show;
+      - more than 256 colours in exactly 256 and 257 occupied bins;
+      - two boxes of equal priority; a box whose r and g extents are equal and longest; a box whose count reaches half only
+        past hi - 1 (the mass on its top plane), so the cut falls back to hi - 1;
+      - colours within 4 of 0 and 255 on every channel, where the dither clamps;
+      - pixels exactly equidistant from two entries after the dither;
+      - a flat frame with a few stray colours, one bin holding almost every pixel;
+      - exact palettes of 1, 2, 255 and 256 colours with black and white, the ends of the kernel's bisection."""
+    rng = np.random.default_rng(29)
+    five = [(10, 40, 20), (50, 12, 33), (30, 30, 60), (62, 2, 45), (20, 55, 5)]
+    near_black = [(0, 0, 0), (40, 10, 20), (12, 50, 33), (60, 60, 60), (30, 2, 45)]
+    black = np.zeros((64 * 4, 3), np.uint8)                     # black pixels in the black bin, whose mean is (2, 2, 2)
+    eight = [(3, 5, 7), (3, 5, 40), (3, 45, 7), (50, 5, 7), (50, 45, 40), (20, 20, 20), (33, 60, 9), (9, 33, 60)]
+    flat = np.full((256 * 256, 3), (90, 160, 30), np.uint8)
+    flat[rng.choice(len(flat), size=300, replace=False)] = rng.integers(0, 256, size=(300, 3))
+    clamp = np.array([0, 1, 2, 3, 4, 251, 252, 253, 254, 255], np.uint8)
+    return {
+        "5_bins": shuffled_frame(bin_colours(five, 3), 32, 1),
+        "5_bins_near_black": shuffled_frame(np.concatenate([bin_colours(near_black, 2), black]), 32, 2),
+        "512_colours_8_bins": shuffled_frame(bin_colours(eight, 2), 32, 3),
+        "256_bins": shuffled_frame(np.repeat(_bins_with_two_colours(256, rng), 3, axis=0), 48, 4),
+        "257_bins": shuffled_frame(np.repeat(_bins_with_two_colours(257, rng), 3, axis=0), 6, 5),
+        # r in {0, 10, 40, 50} x g in {20, 21}: the first cut (r at 10) leaves two boxes of 256 pixels and extent 10
+        "equal_priority": shuffled_frame(bin_colours([(r, g, 9) for r in (0, 10, 40, 50) for g in (20, 21)]), 32, 6),
+        # r and g extents both 20: cut on r, which groups the bins differently from a cut on g
+        "equal_r_g_extents": shuffled_frame(bin_colours([(0, 0, 30), (20, 0, 30), (0, 20, 30), (20, 20, 30), (0, 0, 31)],
+                                                        [1, 2, 3, 4, 1]), 32, 7),
+        # ten light planes and a heavy top plane: the cumulative count reaches half only on the top plane
+        "mass_on_top_plane": shuffled_frame(bin_colours([(r, 30, 30) for r in range(11)], [1] * 10 + [20]), 32, 8),
+        "clamped_dither": shuffled_frame(np.stack(np.meshgrid(clamp, clamp, clamp, indexing="ij"), -1).reshape(-1, 3).repeat(4, 0), 40, 9),
+        # five bins side by side on r, entries 4 apart in r and equal in g and b: a pixel between two entries ties
+        "equidistant": shuffled_frame(bin_colours([(r, 20, 40) for r in range(10, 15)], 2), 32, 10),
+        "flat_with_strays": shuffled_frame(flat, 256, 11),
+        "exact_1_black": np.zeros((19, 23, 4), np.uint8),
+        "exact_1_white": np.full((23, 19, 4), 255, np.uint8),
+        "exact_2_black_white": exact_with(2, 33, 41, 12, [0x000000, 0xFFFFFF]),
+        "exact_255": exact_with(255, 50, 61, 13, [0x000000, 0xFFFFFF]),
+        "exact_256": exact_with(256, 61, 50, 14, [0x000000, 0xFFFFFF]),
+    }
+
+
+def _bins_with_two_colours(n: int, rng) -> np.ndarray:
+    """Two distinct colours in each of n random distinct bins: [2 n, 3] uint8."""
+    bins = rng.choice(1 << 18, size=n, replace=False)
+    lo = np.stack([bins >> 12 & 63, bins >> 6 & 63, bins & 63], axis=1) * 4
+    a = rng.integers(0, 4, size=(n, 3))
+    b = a.copy()
+    ch = rng.integers(0, 3, size=n)                              # b differs from a on one channel, inside the bin
+    b[np.arange(n), ch] = (a[np.arange(n), ch] + rng.integers(1, 4, size=n)) % 4
+    return np.concatenate([lo + a, lo + b]).astype(np.uint8)
+
+
 def synthetic_inputs() -> dict:
     rng = np.random.default_rng(23)
     yy, xx = np.mgrid[0:120, 0:200]
@@ -142,4 +224,5 @@ def synthetic_inputs() -> dict:
         "257_colours": exact_colours(257, 64, 80, 3),
         "gradient": grad,
         "noise": rng.integers(0, 256, size=(211, 317, 4), dtype=np.uint8),
+        **adversarial_inputs(),
     }
