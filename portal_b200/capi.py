@@ -247,36 +247,30 @@ def b(s: str) -> bytes:
     return s.encode("utf-8")
 
 
+def _encode_png(ctx, frame, dtype: str, bound: str, encode: str) -> bytes:
+    if frame.dim() != 3 or frame.shape[2] != 4 or not frame.is_cuda or str(frame.dtype) != f"torch.{dtype}" or not frame.is_contiguous():
+        raise ValueError(f"frame must be a contiguous CUDA {dtype} tensor [h, w, 4]")
+    L = lib()
+    h, w = int(frame.shape[0]), int(frame.shape[1])
+    cap = getattr(L, bound)(w, h)
+    if cap == 0:
+        raise PortalB200Error(f"{bound}: no PNG for a {w} x {h} frame")
+    out, n = (C.c_uint8 * cap)(), C.c_size_t()
+    if getattr(L, encode)(ctx, C.c_void_p(frame.data_ptr()), w, h, out, cap, C.byref(n)):
+        raise PortalB200Error(L.pe_last_error(ctx).decode(errors="replace"))
+    return bytes(memoryview(out)[:n.value])
+
+
 def encode_png_device(ctx, rgba8) -> bytes:
     """PNG file of a CUDA uint8 tensor [h, w, 4] (contiguous) encoded on the device by pe_encode_png_host on context `ctx`
     (a pe_ctx pointer: SceneRenderer._ctx / HostRenderer._ctx)."""
-    if rgba8.dim() != 3 or rgba8.shape[2] != 4 or not rgba8.is_cuda or str(rgba8.dtype) != "torch.uint8" or not rgba8.is_contiguous():
-        raise ValueError("frame must be a contiguous CUDA uint8 tensor [h, w, 4]")
-    L = lib()
-    h, w = int(rgba8.shape[0]), int(rgba8.shape[1])
-    cap = L.pe_png_bound(w, h)
-    if cap == 0:
-        raise PortalB200Error(f"pe_png_bound: no PNG for a {w} x {h} frame")
-    out, n = (C.c_uint8 * cap)(), C.c_size_t()
-    if L.pe_encode_png_host(ctx, C.c_void_p(rgba8.data_ptr()), w, h, out, cap, C.byref(n)):
-        raise PortalB200Error(L.pe_last_error(ctx).decode(errors="replace"))
-    return bytes(memoryview(out)[:n.value])
+    return _encode_png(ctx, rgba8, "uint8", "pe_png_bound", "pe_encode_png_host")
 
 
 def encode_png16_device(ctx, rgba16) -> bytes:
     """16-bit PNG file of a CUDA uint16 tensor [h, w, 4] (contiguous, host byte order) encoded on the device by
     pe_encode_png_host_rgba16 on context `ctx`."""
-    if rgba16.dim() != 3 or rgba16.shape[2] != 4 or not rgba16.is_cuda or str(rgba16.dtype) != "torch.uint16" or not rgba16.is_contiguous():
-        raise ValueError("frame must be a contiguous CUDA uint16 tensor [h, w, 4]")
-    L = lib()
-    h, w = int(rgba16.shape[0]), int(rgba16.shape[1])
-    cap = L.pe_png_bound_rgba16(w, h)
-    if cap == 0:
-        raise PortalB200Error(f"pe_png_bound_rgba16: no PNG for a {w} x {h} frame")
-    out, n = (C.c_uint8 * cap)(), C.c_size_t()
-    if L.pe_encode_png_host_rgba16(ctx, C.c_void_p(rgba16.data_ptr()), w, h, out, cap, C.byref(n)):
-        raise PortalB200Error(L.pe_last_error(ctx).decode(errors="replace"))
-    return bytes(memoryview(out)[:n.value])
+    return _encode_png(ctx, rgba16, "uint16", "pe_png_bound_rgba16", "pe_encode_png_host_rgba16")
 
 
 def encode_gif_frame(ctx, rgba8, delay_cs: int = 0) -> bytes:

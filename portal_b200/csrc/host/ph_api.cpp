@@ -114,6 +114,48 @@ bool motion_blur_times(int frame_index, int frame_count, int motion_blur_frames,
     return true;
 }
 
+// The frame of the uploaded uniforms into device memory `dev` at `bits` 8 (RGBA8), 16 (RGBA16: rendered as floats into `f32`,
+// then quantised) or 32 (float RGBA); through adaptive anti-aliasing at `threshold` when `adaptive`.
+int render_device(pe_ctx* ctx, const pe_target* t, int bits, bool adaptive, int threshold, void* dev, void* f32) {
+    void* out = bits == 16 ? f32 : dev;
+    const int rgba8 = bits == 8;
+    const int rc = adaptive ? pe_render_adaptive(ctx, t, threshold, rgba8, out, nullptr, nullptr)
+                            : rgba8 ? pe_render_rgba8(ctx, t, out, nullptr) : pe_render(ctx, t, out, nullptr, nullptr);
+    return rc || (bits == 16 && pe_quantize_rgba16(ctx, f32, dev, size_t(t->width) * size_t(t->height), nullptr));
+}
+
+const char* const kAllocFailed = "device allocation failed: ";
+
+// The frame of `p` into scratch slot 0, in the slots of portal_b200_host.h: 0 the frame, 1 .. M the sub-frames, and at 16 bits
+// M + 1 the floats each (sub-)frame is rendered into.  Without sub-frames (`times` empty) it is the frame of the uniforms
+// already uploaded.  With them it is one output frame of render_animation (main.rs:1786-1817): for every sub-frame j,
+// `prepare(times[j], q)` moves the scene to that time and uploads the uniforms of `q` (`_aa_start` = j, main.rs:1797), the
+// sub-frame is rendered into slot j + 1, and the sub-frames are averaged in gamma-2 space.  Returns nullptr, or what failed
+// as the start of a message ("" when `prepare` has reported its own failure).
+template <class Prepare>
+const char* stage_frame(pe_ctx* ctx, const ph_frame_params* p, const std::vector<double>& times, int bits, bool adaptive, int threshold,
+                        std::vector<void*>& slot, Prepare prepare) {
+    const int M = int(times.size());
+    const size_t n = size_t(p->width) * size_t(p->height);
+    slot.assign(size_t(M) + 2, nullptr);
+    int rc = 0;
+    for (int k = 0; k <= M; k++) rc |= pe_scratch_buffer(ctx, k, n * size_t(bits / 2), &slot[size_t(k)]);
+    if (bits == 16) rc |= pe_scratch_buffer(ctx, M + 1, n * 16, &slot[size_t(M) + 1]);
+    if (rc) return kAllocFailed;
+    const pe_target t = {p->width, p->height, p->height, 0, 1, 1, 1};
+    if (M == 0) return render_device(ctx, &t, bits, adaptive, threshold, slot[0], slot[1]) ? "render failed: " : nullptr;
+    for (int j = 0; j < M; j++) {
+        ph_frame_params q = *p;
+        q.aa_start = j;
+        if (prepare(times[size_t(j)], &q)) return "";
+        if (render_device(ctx, &t, bits, adaptive, threshold, slot[size_t(j) + 1], slot[size_t(M) + 1])) return "render failed: ";
+    }
+    if (bits == 16 ? pe_average_frames_rgba16(ctx, slot.data() + 1, M, slot[0], n, nullptr)
+                   : pe_average_frames_rgba8(ctx, slot.data() + 1, M, slot[0], n, nullptr))
+        return "motion-blur average failed: ";
+    return nullptr;
+}
+
 }  // namespace
 
 extern "C" {
@@ -357,30 +399,18 @@ int ph_render_motion_blur_frame(ph_scene* s, pe_ctx* ctx, const ph_frame_params*
     if (!motion_blur_times(frame_index, frame_count, motion_blur_frames, duration_seconds, times) || p->width <= 0 || p->height <= 0 ||
         p->width > 65536 || p->height > 65536)
         return fail(s, "ph_render_motion_blur_frame: bad frame arguments");
-    const size_t n = size_t(p->width) * size_t(p->height);
-    // sub-frame and output buffers are the context's scratch slots: allocated once, reused by every frame of the loop
-    void* out8 = nullptr;
-    std::vector<void*> sub(size_t(motion_blur_frames), nullptr);
-    int rc = pe_scratch_buffer(ctx, 0, n * 4, &out8);
-    for (size_t j = 0; j < sub.size(); j++) rc |= pe_scratch_buffer(ctx, 1 + int(j), n * 4, &sub[j]);
     const double saved_time = s->scene.time, saved_total = s->scene.total_time;
-    if (!rc) {
-        pe_target t = {p->width, p->height, p->height, 0, 1, 1, 1};
-        for (int j = 0; j < motion_blur_frames && !rc; j++) {
-            ph_frame_params q = *p;
-            q.aa_start = j;                                            // main.rs:1797
-            ph_scene_set_time(s, times[size_t(j)], times[size_t(j)]);  // Scene::update, Dev/Animation stage branch
-            rc = upload_frame_uniforms(s, ctx, &q) ||
-                 pe_render_rgba8(ctx, &t, sub[size_t(j)], nullptr);   // RGBA8 render target, quantised by the kernel
-        }
-        if (!rc) rc = pe_average_frames_rgba8(ctx, sub.data(), motion_blur_frames, out8, n, nullptr) ||
-                      pe_memcpy_d2h(ctx, out_host, out8, n * 4, nullptr);
-        if (rc && s->err.empty()) s->err = std::string("motion-blur frame failed: ") + pe_last_error(ctx);
-    } else {
-        s->err = std::string("device allocation failed: ") + pe_last_error(ctx);
-    }
+    // RGBA8 sub-frames (quantised by the render kernel) without adaptive anti-aliasing
+    std::vector<void*> slot;
+    const char* why = stage_frame(ctx, p, times, 8, false, 0, slot, [&](double time, const ph_frame_params* q) {
+        ph_scene_set_time(s, time, time);   // Scene::update, Dev/Animation stage branch
+        return upload_frame_uniforms(s, ctx, q);
+    });
+    const bool ok = !why && !pe_memcpy_d2h(ctx, out_host, slot[0], size_t(p->width) * size_t(p->height) * 4, nullptr);
+    if (why == kAllocFailed) s->err = kAllocFailed + std::string(pe_last_error(ctx));
+    else if (!ok && s->err.empty()) s->err = std::string("motion-blur frame failed: ") + pe_last_error(ctx);
     ph_scene_set_time(s, saved_time, saved_total);
-    return rc ? 1 : 0;      // pe_memcpy_d2h has synchronised the stream: the frame is in out_host
+    return ok ? 0 : 1;      // pe_memcpy_d2h has synchronised the stream: the frame is in out_host
 }
 
 // ------------------------------------------------------------------------------------ player
@@ -616,18 +646,7 @@ size_t ph_output_bytes(int container, int bits, int width, int height) {
     return 0;
 }
 
-// The frame of the uploaded uniforms into device memory `dev` at `bits` 8 (RGBA8), 16 (RGBA16: rendered as floats into `f32`,
-// then quantised) or 32 (float RGBA); adaptively when the player is set so.
-static int render_device(ph_player* pl, pe_ctx* ctx, const pe_target* t, int bits, void* dev, void* f32) {
-    void* out = bits == 16 ? f32 : dev;
-    const int rgba8 = bits == 8;
-    const int rc = pl->adaptive_aa ? pe_render_adaptive(ctx, t, pl->adaptive_threshold, rgba8, out, nullptr, nullptr)
-                                   : rgba8 ? pe_render_rgba8(ctx, t, out, nullptr) : pe_render(ctx, t, out, nullptr, nullptr);
-    return rc || (bits == 16 && pe_quantize_rgba16(ctx, f32, dev, size_t(t->width) * size_t(t->height), nullptr));
-}
-
-// Stage, convert, read back.  The scratch slots follow one rule (portal_b200_host.h): 0 the frame, 1 .. M the sub-frames,
-// M + 1 the floats of a 16-bit frame, then the Y'CbCr planes.
+// Stage, convert, read back.  The scratch slots are stage_frame's, then the Y'CbCr planes.
 int ph_player_render(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, const ph_motion_blur* mb, int container, int bits,
                      void* out_host, size_t capacity, size_t* len) {
     if (!pl || !ctx || !p || !out_host || !len) return 1;
@@ -644,10 +663,9 @@ int ph_player_render(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, const
     if (!bytes) return pfail(pl, "ph_player_render: invalid frame size " + std::to_string(p->width) + " x " + std::to_string(p->height));
     if (capacity < bytes) return pfail(pl, "ph_player_render: capacity " + std::to_string(capacity) + " is below ph_output_bytes = " + std::to_string(bytes));
     const pe_target t = {p->width, p->height, p->height, 0, 1, 1, 1};
-    const size_t n = size_t(p->width) * size_t(p->height);
     const int M = mb ? mb->motion_blur_frames : 0;
 
-    // stage: the frame in slot 0
+    // stage: the frame in slot 0; each motion-blur sub-frame updates the player and runs the hook (which swaps video frames)
     if (!mb) {
         if (upload_player_uniforms(pl, ctx, p)) return 1;
         if (container == PH_OUT_PIXELS && bits != 16 && !pl->adaptive_aa) {   // rendered straight into host memory, no slot
@@ -657,31 +675,12 @@ int ph_player_render(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, const
             return 0;
         }
     }
-    std::vector<void*> slot(size_t(M) + 2, nullptr);
-    int rc = 0;
-    for (int k = 0; k <= M; k++) rc |= pe_scratch_buffer(ctx, k, n * size_t(bits / 2), &slot[size_t(k)]);
-    if (bits == 16) rc |= pe_scratch_buffer(ctx, M + 1, n * 16, &slot[size_t(M) + 1]);
+    std::vector<void*> slot;
+    const char* why = stage_frame(ctx, p, times, bits, pl->adaptive_aa, pl->adaptive_threshold, slot, [&](double time, const ph_frame_params* q) {
+        return ph_player_update(pl, time) || upload_player_uniforms(pl, ctx, q);
+    });
+    if (why) return *why ? pfail(pl, (mb ? why : "render failed: ") + std::string(pe_last_error(ctx))) : 1;
     void* const frame = slot[0];
-    void* const f32 = slot[size_t(M) + 1];
-    if (!mb) {
-        if (rc || render_device(pl, ctx, &t, bits, frame, f32)) return pfail(pl, std::string("render failed: ") + pe_last_error(ctx));
-    } else {
-        // one output frame of render_animation (main.rs:1786-1817): every sub-frame j updates the player to times[j] (and runs
-        // the update hook, whose tail swaps video frames), renders with `_aa_start` = j, and the sub-frames are averaged in
-        // gamma-2 space
-        if (rc) return pfail(pl, std::string("device allocation failed: ") + pe_last_error(ctx));
-        for (int j = 0; j < M; j++) {
-            ph_frame_params q = *p;
-            q.aa_start = j;  // main.rs:1797
-            if (!pl->player.update(times[size_t(j)])) return pfail(pl, pl->player.error);
-            if (pl->hook && pl->hook(pl->hook_user)) return pfail(pl, "the update hook failed");
-            if (upload_player_uniforms(pl, ctx, &q)) return 1;
-            if (render_device(pl, ctx, &t, bits, slot[size_t(j) + 1], f32)) return pfail(pl, std::string("render failed: ") + pe_last_error(ctx));
-        }
-        if (bits == 16 ? pe_average_frames_rgba16(ctx, slot.data() + 1, M, frame, n, nullptr)
-                       : pe_average_frames_rgba8(ctx, slot.data() + 1, M, frame, n, nullptr))
-            return pfail(pl, std::string("motion-blur average failed: ") + pe_last_error(ctx));
-    }
 
     // convert and read back
     if (container == PH_OUT_PNG) {

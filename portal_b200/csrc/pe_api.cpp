@@ -1,5 +1,6 @@
 // portal_b200 C ABI (include/portal_b200.h): context, scene builder, constant-block uploader and launcher of the sm_90a
-// ray-loop kernel.  The scene program's variants (NVRTC, cubin cache, specialisation) are managed by pe_program.cpp.
+// ray-loop kernel.  The scene program's variants (NVRTC, cubin cache, specialisation) are managed by pe_program.cpp, the
+// post-processing and encoding of rendered frames by pe_frames.cpp.
 //
 // Mirrors, call for call, what the reference's SceneRenderer does with its macroquad Material
 // (/root/reference/src/main.rs:934-1064 new, :1266-1359 set_uniforms, :1411-1428 draw_texture,
@@ -36,14 +37,6 @@ static_assert(sizeof(PeLaunchHost) == 72, "PeLaunch layout");
 
 thread_local std::string g_create_error;     // per thread: another thread's pe_create cannot rewrite it under a reader
 std::mutex g_create_mutex;
-
-bool cuda_ok(pe_ctx* c, cudaError_t e, const char* what) {
-    if (e == cudaSuccess) return true;
-    c->err = std::string(what) + ": " + cudaGetErrorString(e);
-    return false;
-}
-
-cudaStream_t stream_of(pe_ctx* c, void* stream) { return stream ? (cudaStream_t)stream : c->stream; }
 
 // Gives `*target` a value for the guard's lifetime and restores the old one on every return path.  A null target (a
 // uniform the scene does not declare) is left alone.
@@ -85,6 +78,28 @@ float* fslot(pe_ctx* c, int slot) { return reinterpret_cast<float*>(c->cblock.da
 int* islot(pe_ctx* c, int slot) { return reinterpret_cast<int*>(c->cblock.data() + c->layout.off_int) + slot; }
 
 }  // namespace
+
+bool pe_host::cuda_ok(pe_ctx* c, cudaError_t e, const char* what) {
+    if (e == cudaSuccess) return true;
+    c->err = std::string(what) + ": " + cudaGetErrorString(e);
+    return false;
+}
+
+bool pe_host::launched(pe_ctx* c, int e, const char* what, int kernels) {
+    if (!cuda_ok(c, (cudaError_t)e, what)) return false;
+    c->launches += uint64_t(kernels);
+    return true;
+}
+
+bool pe_host::bind_device(pe_ctx* c) {
+    if (!c->has_gpu) {
+        c->err = "this context has no CUDA device (compile-only); portal_b200 has no CPU rendering path";
+        return false;
+    }
+    return cuda_ok(c, cudaSetDevice(c->device), "cudaSetDevice");
+}
+
+cudaStream_t pe_host::stream_of(pe_ctx* c, void* stream) { return stream ? (cudaStream_t)stream : c->stream; }
 
 void pe_host::ensure_layout(pe_ctx* c) {
     if (c->layout_valid) return;
@@ -183,14 +198,6 @@ void update_derived(pe_ctx* c) {
     }
 }
 
-bool bind_device(pe_ctx* c) {
-    if (!c->has_gpu) {
-        c->err = "this context has no CUDA device (compile-only); portal_b200 has no CPU rendering path";
-        return false;
-    }
-    return cuda_ok(c, cudaSetDevice(c->device), "cudaSetDevice");
-}
-
 bool check_target(pe_ctx* c, const pe_target* t) {
     // n_strips == 0 is legal: a rank that owns no strip (fewer strips than ranks); such a render launches nothing
     if (!t || t->width <= 0 || t->height <= 0 || t->strip_rows <= 0 || t->strip_step <= 0 || t->n_strips < 0 ||
@@ -207,6 +214,25 @@ bool check_target(pe_ctx* c, const pe_target* t) {
         return false;
     }
     return true;
+}
+
+// The 16-byte record of texture `name` in the uniform block, or nullptr (the error set) for a name the scene does not declare.
+uint8_t* texture_record(pe_ctx* c, const char* name) {
+    ensure_layout(c);
+    auto it = c->layout.tex_slot.find(name);
+    if (it == c->layout.tex_slot.end()) {
+        c->fail(std::string("unknown texture `") + name + "`");
+        return nullptr;
+    }
+    return c->cblock.data() + c->layout.off_tex + size_t(it->second) * 16;
+}
+
+// Bind a width x height RGBA8 image on the device to a texture record: its pointer, width and height.  The defaults unbind the
+// sampler, which then reads no image.
+void set_texture_record(uint8_t* rec, const void* image = nullptr, int width = 0, int height = 0) {
+    std::memcpy(rec, &image, 8);
+    std::memcpy(rec + 8, &width, 4);
+    std::memcpy(rec + 12, &height, 4);
 }
 
 }  // namespace
@@ -526,9 +552,8 @@ int pe_set_uniform_i32(pe_ctx* c, const char* name, int32_t v) {
 
 int pe_set_texture(pe_ctx* c, const char* name, const uint8_t* rgba8, int w, int h) {
     if (!c || !name || !rgba8 || w <= 0 || h <= 0) return c ? c->fail("pe_set_texture: bad arguments") : 1;
-    ensure_layout(c);
-    auto it = c->layout.tex_slot.find(name);
-    if (it == c->layout.tex_slot.end()) return c->fail(std::string("unknown texture `") + name + "`", 2);
+    uint8_t* rec = texture_record(c, name);
+    if (!rec) return 2;
     if (!bind_device(c)) return 1;
     DeviceBuffer& t = c->textures[name];
     size_t bytes = size_t(w) * size_t(h) * 4;
@@ -537,13 +562,40 @@ int pe_set_texture(pe_ctx* c, const char* name, const uint8_t* rgba8, int w, int
     // If that wait fails the old image stays allocated and bound.
     if (t.dev && !cuda_ok(c, cudaDeviceSynchronize(), "pe_set_texture: waiting for queued renders")) return 1;
     t.release();
-    uint8_t* rec = c->cblock.data() + c->layout.off_tex + size_t(it->second) * 16;
-    std::memset(rec, 0, 16);   // until the new image is in place the sampler is unbound, never the freed image
+    set_texture_record(rec);   // until the new image is in place the sampler is unbound, never the freed image
     if (!cuda_ok(c, t.ensure(bytes), "cudaMalloc(texture)")) return 1;
     if (!cuda_ok(c, cudaMemcpy(t.dev, rgba8, bytes, cudaMemcpyHostToDevice), "cudaMemcpy(texture)")) return 1;
-    std::memcpy(rec, &t.dev, 8);
-    std::memcpy(rec + 8, &w, 4);
-    std::memcpy(rec + 12, &h, 4);
+    set_texture_record(rec, t.dev, w, h);
+    return 0;
+}
+
+int pe_set_texture_yuv420(pe_ctx* c, const char* name, const void* yuv_host, const pe_yuv_format* format, int width, int height) {
+    if (!c) return 1;
+    const std::string fn = "pe_set_texture_yuv420";
+    if (!name || !yuv_host) return c->fail(fn + ": null argument");
+    if (!check_yuv420(c, fn, format, width, height)) return 1;
+    uint8_t* rec = texture_record(c, name);
+    if (!rec) return 2;
+    if (!bind_device(c)) return 1;
+    DeviceBuffer& t = c->textures[name];
+    const size_t bytes = size_t(width) * size_t(height) * 4, planes = yuv420_bytes(width, height, format->bits);
+    // As pe_set_texture: a render queued on any stream may still read the image, so wait for the device before touching it.
+    // If that wait fails the old image stays allocated and bound.
+    if (t.dev && !cuda_ok(c, cudaDeviceSynchronize(), "pe_set_texture_yuv420: waiting for queued renders")) return 1;
+    if (t.bytes != bytes) {            // another size: free the old image; until the new one is in place the sampler is unbound
+        t.release();
+        set_texture_record(rec);
+        if (!cuda_ok(c, t.ensure(bytes), "cudaMalloc(texture)")) return 1;
+    }
+    if (!cuda_ok(c, c->yuv_upload.ensure(planes), "cudaMalloc(texture planes)") ||
+        !cuda_ok(c, cudaMemcpyAsync(c->yuv_upload.dev, yuv_host, planes, cudaMemcpyHostToDevice, c->stream), "cudaMemcpy(texture planes)") ||
+        !launched(c, launch_yuv420_to_rgba8(c->yuv_upload.dev, format->bits, format->matrix, format->full_range, format->siting, width, height,
+                                            t.dev, c->stream), fn.c_str()) ||
+        !cuda_ok(c, cudaStreamSynchronize(c->stream), fn.c_str())) {
+        set_texture_record(rec);       // the image may be half written: unbind it, keep the memory (it is freed with the context)
+        return 1;
+    }
+    set_texture_record(rec, t.dev, width, height);
     return 0;
 }
 
@@ -707,13 +759,10 @@ int render_adaptive_impl(pe_ctx* c, const pe_target* t, int threshold, bool rgba
     unsigned* counter = (unsigned*)B.refine_count.dev;
     if (!cuda_ok(c, cudaMemsetAsync(counter, 0, 16, s), "adaptive anti-aliasing: counter reset")) return 1;
     const RefineTarget rt = {t->width, t->height, S, t->strip_first, step, t->n_strips, t->full_frame_layout ? 1 : 0, local_rows};
-    if (local_rows > 0) {
-        if (!cuda_ok(c, (cudaError_t)launch_refine_list(out_device, rgba8, rt, (const unsigned*)B.halo_above.dev, above_first,
-                                                         (const unsigned*)B.halo_below.dev, threshold, list, counter, s),
-                     "adaptive anti-aliasing: refine list"))
-            return 1;
-        c->launches++;
-    }
+    if (local_rows > 0 && !launched(c, launch_refine_list(out_device, rgba8, rt, (const unsigned*)B.halo_above.dev, above_first,
+                                                          (const unsigned*)B.halo_below.dev, threshold, list, counter, s),
+                                    "adaptive anti-aliasing: refine list"))
+        return 1;
     if (refined_count_device &&
         !cuda_ok(c, cudaMemcpyAsync(refined_count_device, counter, 4, cudaMemcpyDeviceToDevice, s), "refined count copy"))
         return 1;
@@ -732,6 +781,33 @@ int render_adaptive_impl(pe_ctx* c, const pe_target* t, int threshold, bool rgba
     if (r != 0) return c->fail("cuLaunchKernel(pe_refine_kernel): " + driver_error(c->drv, r));
     c->launches++;
     return 0;
+}
+
+// The checks of the adaptive entry points (`fn` names the entry in the messages), then render_adaptive_impl.
+// `whole_frame_only`: pe_render_adaptive, which takes whole-frame targets only.
+int render_adaptive_checked(pe_ctx* c, const char* fn, const pe_target* t, int threshold, int rgba8, void* out_device,
+                            void* refined_count_device, void* stream, int instance, bool whole_frame_only = false) {
+    if (!c) return 1;
+    if (!out_device) return c->fail(std::string(fn) + ": out_device is null");
+    if (!check_target(c, t) || !bind_device(c)) return 1;
+    if (t->n_strips == 0) return 0;   // nothing of this frame belongs to the caller
+    if (whole_frame_only && (t->strip_first != 0 || t->n_strips != 1 || t->strip_rows < t->height))
+        return c->fail("pe_render_adaptive: only whole-frame targets ({w, h, h, 0, 1, 1, layout}) are supported -- use "
+                       "pe_render_adaptive_strips for strip targets");
+    return render_adaptive_impl(c, t, threshold, rgba8 != 0, out_device, refined_count_device, stream_of(c, stream), instance);
+}
+
+// pe_render_host / pe_render_host_rgba8: render into the context's staging buffer, then read it back
+int render_host(pe_ctx* c, const char* fn, const pe_target* t, void* out_host, bool rgba8) {
+    if (!c) return 1;
+    if (!out_host) return c->fail(std::string(fn) + ": out_host is null");
+    if (!check_target(c, t) || !bind_device(c)) return 1;
+    DeviceBuffer& staging = rgba8 ? c->staging8 : c->staging;
+    const size_t bytes = pe_target_pixels(t) * (rgba8 ? 4 : 16);
+    if (!cuda_ok(c, staging.ensure(bytes), "cudaMalloc(staging)")) return 1;
+    if (render_impl(c, t, staging.dev, nullptr, nullptr, rgba8)) return 1;
+    if (!cuda_ok(c, cudaMemcpyAsync(out_host, staging.dev, bytes, cudaMemcpyDeviceToHost, c->stream), "D2H copy")) return 1;
+    return cuda_ok(c, cudaStreamSynchronize(c->stream), fn) ? 0 : 1;
 }
 
 }  // namespace
@@ -783,45 +859,18 @@ int pe_probe_ray(pe_ctx* c, const float a[3], const float b[3], float pos_out[3]
 
 int pe_render_adaptive(pe_ctx* c, const pe_target* t, int threshold, int rgba8, void* out_device, void* refined_count_device,
                        void* stream) {
-    if (!c) return 1;
-    if (!out_device) return c->fail("pe_render_adaptive: out_device is null");
-    if (!check_target(c, t) || !bind_device(c)) return 1;
-    if (t->n_strips == 0) return 0;   // nothing of this frame belongs to the caller
-    if (t->strip_first != 0 || t->n_strips != 1 || t->strip_rows < t->height)
-        return c->fail("pe_render_adaptive: only whole-frame targets ({w, h, h, 0, 1, 1, layout}) are supported -- use "
-                       "pe_render_adaptive_strips for strip targets");
-    return render_adaptive_impl(c, t, threshold, rgba8 != 0, out_device, refined_count_device, stream_of(c, stream), 0);
+    return render_adaptive_checked(c, "pe_render_adaptive", t, threshold, rgba8, out_device, refined_count_device, stream, 0, true);
 }
 
 int pe_render_adaptive_strips(pe_ctx* c, const pe_target* t, int threshold, int rgba8, void* out_device,
                               void* refined_count_device, void* stream) {
-    if (!c) return 1;
-    if (!out_device) return c->fail("pe_render_adaptive_strips: out_device is null");
-    if (!check_target(c, t) || !bind_device(c)) return 1;
-    if (t->n_strips == 0) return 0;   // nothing of this frame belongs to the caller
-    return render_adaptive_impl(c, t, threshold, rgba8 != 0, out_device, refined_count_device, stream_of(c, stream), 0);
+    return render_adaptive_checked(c, "pe_render_adaptive_strips", t, threshold, rgba8, out_device, refined_count_device, stream, 0);
 }
 
-int pe_render_host(pe_ctx* c, const pe_target* t, float* out_host) {
-    if (!c) return 1;
-    if (!out_host) return c->fail("pe_render_host: out_host is null");
-    if (!check_target(c, t) || !bind_device(c)) return 1;
-    size_t bytes = pe_target_pixels(t) * 16;
-    if (!cuda_ok(c, c->staging.ensure(bytes), "cudaMalloc(staging)")) return 1;
-    if (pe_render(c, t, c->staging.dev, nullptr, nullptr)) return 1;
-    if (!cuda_ok(c, cudaMemcpyAsync(out_host, c->staging.dev, bytes, cudaMemcpyDeviceToHost, c->stream), "D2H copy")) return 1;
-    return cuda_ok(c, cudaStreamSynchronize(c->stream), "pe_render_host") ? 0 : 1;
-}
+int pe_render_host(pe_ctx* c, const pe_target* t, float* out_host) { return render_host(c, "pe_render_host", t, out_host, false); }
 
 int pe_render_host_rgba8(pe_ctx* c, const pe_target* t, uint8_t* out_host) {
-    if (!c) return 1;
-    if (!out_host) return c->fail("pe_render_host_rgba8: out_host is null");
-    if (!check_target(c, t) || !bind_device(c)) return 1;
-    size_t n = pe_target_pixels(t);
-    if (!cuda_ok(c, c->staging8.ensure(n * 4), "cudaMalloc(staging)")) return 1;
-    if (render_impl(c, t, c->staging8.dev, nullptr, nullptr, true)) return 1;
-    if (!cuda_ok(c, cudaMemcpyAsync(out_host, c->staging8.dev, n * 4, cudaMemcpyDeviceToHost, c->stream), "D2H copy")) return 1;
-    return cuda_ok(c, cudaStreamSynchronize(c->stream), "pe_render_host_rgba8") ? 0 : 1;
+    return render_host(c, "pe_render_host_rgba8", t, out_host, true);
 }
 
 // ---- pipelined readback: frame i's D2H copy (copy stream) overlaps frame i+1's kernel (render stream) ----
@@ -904,11 +953,7 @@ int pe_internal_submit_host_strips_adaptive(pe_ctx* c, const pe_target* t, uint8
 }
 
 int pe_internal_render_adaptive(pe_ctx* c, const pe_target* t, int threshold, int rgba8, void* out_device, void* stream, int instance) {
-    if (!c) return 1;
-    if (!out_device) return c->fail("adaptive anti-aliasing: out_device is null");
-    if (!check_target(c, t) || !bind_device(c)) return 1;
-    if (t->n_strips == 0) return 0;
-    return render_adaptive_impl(c, t, threshold, rgba8 != 0, out_device, nullptr, stream_of(c, stream), instance);
+    return render_adaptive_checked(c, "adaptive anti-aliasing", t, threshold, rgba8, out_device, nullptr, stream, instance);
 }
 
 int pe_internal_copy_strips(pe_ctx* c, const pe_target* t, void* frame_device, const void* strips_device, size_t bytes_per_pixel,
@@ -976,11 +1021,8 @@ int pe_deinterleave_strips(pe_ctx* c, const void* gathered, void* frame, int wid
         return c->fail("pe_deinterleave_strips: strips_per_rank " + std::to_string(strips_per_rank) +
                        " is below ceil(ceil(height / strip_rows) / n_ranks) = " + std::to_string(need));
     if (!bind_device(c)) return 1;
-    const cudaStream_t s = stream_of(c, stream);
-    if (!cuda_ok(c, (cudaError_t)launch_deinterleave(gathered, frame, width, height, strip_rows, n_ranks, strips_per_rank,
-                                                    c->sm_count, s), "deinterleave")) return 1;
-    c->launches++;
-    return 0;
+    return launched(c, launch_deinterleave(gathered, frame, width, height, strip_rows, n_ranks, strips_per_rank, c->sm_count,
+                                           stream_of(c, stream)), "deinterleave") ? 0 : 1;
 }
 
 int pe_device_malloc(pe_ctx* c, size_t bytes, void** out) {
@@ -1093,10 +1135,9 @@ int pe_frames_differ(pe_ctx* c, const void* a, const void* b, size_t bytes, void
     if (!cuda_ok(c, c->diff_word.ensure(16), "cudaMalloc(difference word)")) return 1;
     void* diff = c->diff_word.dev;
     if (!cuda_ok(c, cudaMemsetAsync(diff, 0, 16, s), "pe_frames_differ") ||
-        !cuda_ok(c, (cudaError_t)launch_count_diff(a, b, bytes / 16, (unsigned*)diff, c->sm_count, s), "pe_frames_differ") ||
+        !launched(c, launch_count_diff(a, b, bytes / 16, (unsigned*)diff, c->sm_count, s), "pe_frames_differ") ||
         !cuda_ok(c, cudaMemcpyAsync(words_out, diff, 4, cudaMemcpyDeviceToHost, s), "pe_frames_differ") ||
         !cuda_ok(c, cudaStreamSynchronize(s), "pe_frames_differ")) return 1;
-    c->launches++;
     return 0;
 }
 
@@ -1111,10 +1152,7 @@ int pe_memcpy_d2h(pe_ctx* c, void* dst, const void* src, size_t bytes, void* str
 int pe_signal_u32(pe_ctx* c, void* const* device_ptrs, int n, uint32_t value, void* stream) {
     if (!c || !device_ptrs) return 1;
     if (!bind_device(c)) return 1;
-    const cudaStream_t s = stream_of(c, stream);
-    if (!cuda_ok(c, (cudaError_t)launch_signal(device_ptrs, n, value, s), "signal")) return 1;
-    c->launches++;
-    return 0;
+    return launched(c, launch_signal(device_ptrs, n, value, stream_of(c, stream)), "signal") ? 0 : 1;
 }
 
 int pe_stream_wait_geq_u32(pe_ctx* c, void* local_device_ptr, uint32_t value, void* stream) {
@@ -1157,288 +1195,6 @@ int pe_ipc_close(pe_ctx* c, void* p) {
     if (!c || !p) return 1;
     if (!bind_device(c)) return 1;
     return cuda_ok(c, cudaIpcCloseMemHandle(p), "cudaIpcCloseMemHandle") ? 0 : 1;
-}
-
-// ------------------------------------------------------------------------------ post-processing
-int pe_average_frames_rgba8(pe_ctx* c, const void* const* frames, int n_frames, void* out, size_t n_pixels, void* stream) {
-    if (!c) return 1;
-    if (!frames || !out || n_frames < 1 || n_frames > 64) return c->fail("pe_average_frames_rgba8: bad arguments (1 <= n_frames <= 64)");
-    for (int i = 0; i < n_frames; i++)
-        if (!frames[i]) return c->fail("pe_average_frames_rgba8: frame " + std::to_string(i) + " is null");
-    bool aligned = (uintptr_t(out) & 3) == 0;
-    for (int i = 0; i < n_frames; i++) aligned = aligned && (uintptr_t(frames[i]) & 3) == 0;
-    if (!aligned) return c->fail("pe_average_frames_rgba8: the frames and the output must be 4-byte aligned");
-    if (!bind_device(c)) return 1;
-    const cudaStream_t s = stream_of(c, stream);
-    if (!cuda_ok(c, (cudaError_t)launch_average_rgba8(frames, n_frames, out, n_pixels, c->sm_count, s), "average")) return 1;
-    c->launches++;
-    return 0;
-}
-
-int pe_quantize_rgba8(pe_ctx* c, const void* in, void* out, size_t n_pixels, void* stream) {
-    if (!c) return 1;
-    if (!in || !out) return c->fail("pe_quantize_rgba8: bad arguments");
-    if ((uintptr_t(in) & 15) || (uintptr_t(out) & 3)) return c->fail("pe_quantize_rgba8: the float frame must be 16-byte and the output 4-byte aligned");
-    if (!bind_device(c)) return 1;
-    const cudaStream_t s = stream_of(c, stream);
-    if (!cuda_ok(c, (cudaError_t)launch_quantize_rgba8(in, out, n_pixels, c->sm_count, s), "quantize")) return 1;
-    c->launches++;
-    return 0;
-}
-
-int pe_average_frames_rgba16(pe_ctx* c, const void* const* frames, int n_frames, void* out, size_t n_pixels, void* stream) {
-    if (!c) return 1;
-    if (!frames || !out || n_frames < 1 || n_frames > 64) return c->fail("pe_average_frames_rgba16: bad arguments (1 <= n_frames <= 64)");
-    bool aligned = (uintptr_t(out) & 7) == 0;
-    for (int i = 0; i < n_frames; i++) aligned = aligned && frames[i] && (uintptr_t(frames[i]) & 7) == 0;
-    if (!aligned) return c->fail("pe_average_frames_rgba16: the frames and the output must be 8-byte aligned");
-    if (!bind_device(c)) return 1;
-    const cudaStream_t s = stream_of(c, stream);
-    if (!cuda_ok(c, (cudaError_t)launch_average_rgba16(frames, n_frames, out, n_pixels, c->sm_count, s), "average")) return 1;
-    c->launches++;
-    return 0;
-}
-
-int pe_quantize_rgba16(pe_ctx* c, const void* in, void* out, size_t n_pixels, void* stream) {
-    if (!c) return 1;
-    if (!in || !out) return c->fail("pe_quantize_rgba16: bad arguments");
-    if ((uintptr_t(in) & 15) || (uintptr_t(out) & 7)) return c->fail("pe_quantize_rgba16: the float frame must be 16-byte and the output 8-byte aligned");
-    if (!bind_device(c)) return 1;
-    const cudaStream_t s = stream_of(c, stream);
-    if (!cuda_ok(c, (cudaError_t)launch_quantize_rgba16(in, out, n_pixels, c->sm_count, s), "quantize")) return 1;
-    c->launches++;
-    return 0;
-}
-
-// ------------------------------------------------------------------------------ PNG encoding (pe_png.cu)
-size_t pe_png_bound(int width, int height) { return png_bound(width, height, 4); }
-size_t pe_png_bound_rgba16(int width, int height) { return png_bound(width, height, 8); }
-
-}  // extern "C"
-
-namespace {
-
-// pe_encode_png_rgba8 / _rgba16 (`bpp` 4 / 8 bytes per pixel; the frame must be aligned to one pixel word)
-int encode_png(pe_ctx* c, const char* name, int bpp, const void* rgba, int width, int height, void* png, size_t capacity, void* size_device,
-               void* stream) {
-    const std::string fn = name;
-    if (!rgba || !png || !size_device) return c->fail(fn + ": null argument");
-    if (width < 1 || height < 1) return c->fail(fn + ": width and height must be at least 1");
-    const size_t bound = png_bound(width, height, bpp);
-    if (!bound) return c->fail(fn + ": frame too large (its PNG could exceed 2^31 - 1 bytes)");
-    const char* bound_fn = bpp == 4 ? "pe_png_bound" : "pe_png_bound_rgba16";
-    if (capacity < bound) return c->fail(fn + ": capacity " + std::to_string(capacity) + " is below " + bound_fn + " = " + std::to_string(bound));
-    if (uintptr_t(rgba) & uintptr_t(bpp - 1)) return c->fail(fn + ": the frame must be " + std::to_string(bpp) + "-byte aligned");
-    if (!bind_device(c)) return 1;
-    if (!cuda_ok(c, c->png_work.ensure(png_workspace_bytes(width, height, bpp)), "cudaMalloc(PNG work space)")) return 1;
-    if (!cuda_ok(c, (cudaError_t)launch_png_encode(rgba, width, height, bpp, c->png_work.dev, png, size_device, stream_of(c, stream)), name))
-        return 1;
-    c->launches += 5;
-    return 0;
-}
-
-// pe_encode_png_host / _host_rgba16: the device form into the context's own file buffer, then read back
-int encode_png_host(pe_ctx* c, const char* name, const char* device_name, int bpp, const void* rgba, int width, int height, uint8_t* png_host,
-                    size_t capacity, size_t* size_out) {
-    const std::string fn = name;
-    if (!rgba || !png_host || !size_out) return c->fail(fn + ": null argument");
-    if (width < 1 || height < 1) return c->fail(fn + ": width and height must be at least 1");
-    const size_t bound = png_bound(width, height, bpp);
-    if (!bound) return c->fail(fn + ": frame too large (its PNG could exceed 2^31 - 1 bytes)");
-    const char* bound_fn = bpp == 4 ? "pe_png_bound" : "pe_png_bound_rgba16";
-    if (capacity < bound) return c->fail(fn + ": capacity " + std::to_string(capacity) + " is below " + bound_fn + " = " + std::to_string(bound));
-    if (!bind_device(c)) return 1;
-    if (!cuda_ok(c, c->png_file.ensure(bound), "cudaMalloc(PNG file)") || !cuda_ok(c, c->png_size.ensure(8), "cudaMalloc(PNG length)")) return 1;
-    if (encode_png(c, device_name, bpp, rgba, width, height, c->png_file.dev, c->png_file.bytes, c->png_size.dev, nullptr)) return 1;
-    uint64_t n = 0;
-    if (!cuda_ok(c, cudaMemcpyAsync(&n, c->png_size.dev, 8, cudaMemcpyDeviceToHost, c->stream), name) ||
-        !cuda_ok(c, cudaStreamSynchronize(c->stream), name) ||
-        !cuda_ok(c, cudaMemcpyAsync(png_host, c->png_file.dev, size_t(n), cudaMemcpyDeviceToHost, c->stream), name) ||
-        !cuda_ok(c, cudaStreamSynchronize(c->stream), name)) return 1;
-    *size_out = size_t(n);
-    return 0;
-}
-
-}  // namespace
-
-extern "C" {
-
-int pe_encode_png_rgba8(pe_ctx* c, const void* rgba8, int width, int height, void* png, size_t capacity, void* size_device, void* stream) {
-    return c ? encode_png(c, "pe_encode_png_rgba8", 4, rgba8, width, height, png, capacity, size_device, stream) : 1;
-}
-
-int pe_encode_png_host(pe_ctx* c, const void* rgba8, int width, int height, uint8_t* png_host, size_t capacity, size_t* size_out) {
-    return c ? encode_png_host(c, "pe_encode_png_host", "pe_encode_png_rgba8", 4, rgba8, width, height, png_host, capacity, size_out) : 1;
-}
-
-int pe_encode_png_rgba16(pe_ctx* c, const void* rgba16, int width, int height, void* png, size_t capacity, void* size_device, void* stream) {
-    return c ? encode_png(c, "pe_encode_png_rgba16", 8, rgba16, width, height, png, capacity, size_device, stream) : 1;
-}
-
-int pe_encode_png_host_rgba16(pe_ctx* c, const void* rgba16, int width, int height, uint8_t* png_host, size_t capacity, size_t* size_out) {
-    return c ? encode_png_host(c, "pe_encode_png_host_rgba16", "pe_encode_png_rgba16", 8, rgba16, width, height, png_host, capacity, size_out) : 1;
-}
-
-// ------------------------------------------------------------------------------ GIF frame blocks (pe_gif.cu)
-size_t pe_gif_frame_bound(int width, int height) { return gif_frame_bound(width, height); }
-
-int pe_gif_header(int width, int height, int loop, uint8_t* out, size_t capacity) {
-    if (!out || !gif_frame_bound(width, height) || (loop != 0 && loop != 1)) return 0;
-    const uint8_t lsd[13] = {'G', 'I', 'F', '8', '9', 'a', uint8_t(width), uint8_t(width >> 8), uint8_t(height), uint8_t(height >> 8), 0x70, 0, 0};
-    const uint8_t netscape[19] = {0x21, 0xFF, 0x0B, 'N', 'E', 'T', 'S', 'C', 'A', 'P', 'E', '2', '.', '0', 0x03, 0x01, 0x00, 0x00, 0x00};
-    const size_t n = loop ? 32 : 13;
-    if (capacity < n) return 0;
-    std::memcpy(out, lsd, 13);
-    if (loop) std::memcpy(out + 13, netscape, 19);
-    return int(n);
-}
-
-}  // extern "C"
-
-namespace {
-
-// The checks every GIF entry point makes before anything is allocated or launched
-bool check_gif(pe_ctx* c, const std::string& fn, int width, int height, int delay_cs, size_t capacity) {
-    if (!gif_frame_bound(width, height))
-        return !c->fail(fn + ": invalid size " + std::to_string(width) + " x " + std::to_string(height) + " (1 <= width, height <= 65535)");
-    if (delay_cs < 0 || delay_cs > 65535) return !c->fail(fn + ": delay " + std::to_string(delay_cs) + " cs is outside 0 .. 65535");
-    const size_t bound = gif_frame_bound(width, height);
-    if (capacity < bound) return !c->fail(fn + ": capacity " + std::to_string(capacity) + " is below pe_gif_frame_bound = " + std::to_string(bound));
-    return true;
-}
-
-int encode_gif(pe_ctx* c, const void* rgba, int width, int height, int delay_cs, void* out, size_t capacity, void* size_device, void* stream) {
-    const std::string fn = "pe_encode_gif_frame";
-    if (!rgba || !out || !size_device) return c->fail(fn + ": null argument");
-    if (!check_gif(c, fn, width, height, delay_cs, capacity)) return 1;
-    if (uintptr_t(rgba) & 3) return c->fail(fn + ": the frame must be 4-byte aligned");
-    if (!bind_device(c)) return 1;
-    if (!cuda_ok(c, c->gif_work.ensure(gif_workspace_bytes(width, height)), "cudaMalloc(GIF work space)")) return 1;
-    if (!cuda_ok(c, (cudaError_t)launch_gif_encode(rgba, width, height, delay_cs, c->gif_work.dev, out, size_device, stream_of(c, stream)), fn.c_str()))
-        return 1;
-    c->launches += 6;
-    return 0;
-}
-
-}  // namespace
-
-extern "C" {
-
-int pe_encode_gif_frame(pe_ctx* c, const void* rgba8, int width, int height, int delay_cs, void* out, size_t capacity, void* size_device,
-                        void* stream) {
-    return c ? encode_gif(c, rgba8, width, height, delay_cs, out, capacity, size_device, stream) : 1;
-}
-
-int pe_encode_gif_frame_host(pe_ctx* c, const void* rgba8, int width, int height, int delay_cs, uint8_t* out_host, size_t capacity,
-                             size_t* size_out) {
-    if (!c) return 1;
-    const std::string fn = "pe_encode_gif_frame_host";
-    if (!rgba8 || !out_host || !size_out) return c->fail(fn + ": null argument");
-    if (!check_gif(c, fn, width, height, delay_cs, capacity)) return 1;
-    if (uintptr_t(rgba8) & 3) return c->fail(fn + ": the frame must be 4-byte aligned");
-    if (!bind_device(c)) return 1;
-    const size_t bound = gif_frame_bound(width, height);
-    if (!cuda_ok(c, c->gif_block.ensure(bound), "cudaMalloc(GIF block)") || !cuda_ok(c, c->gif_size.ensure(8), "cudaMalloc(GIF length)")) return 1;
-    if (encode_gif(c, rgba8, width, height, delay_cs, c->gif_block.dev, c->gif_block.bytes, c->gif_size.dev, nullptr)) return 1;
-    uint64_t n = 0;
-    if (!cuda_ok(c, cudaMemcpyAsync(&n, c->gif_size.dev, 8, cudaMemcpyDeviceToHost, c->stream), fn.c_str()) ||
-        !cuda_ok(c, cudaStreamSynchronize(c->stream), fn.c_str()) ||
-        !cuda_ok(c, cudaMemcpyAsync(out_host, c->gif_block.dev, size_t(n), cudaMemcpyDeviceToHost, c->stream), fn.c_str()) ||
-        !cuda_ok(c, cudaStreamSynchronize(c->stream), fn.c_str())) return 1;
-    *size_out = size_t(n);
-    return 0;
-}
-
-// ------------------------------------------------------------------------------ Y'CbCr 4:2:0, 10 bits (pe_yuv.cu)
-size_t pe_yuv420p10_bytes(int width, int height) { return yuv420p10_bytes(width, height); }
-
-int pe_rgba_to_yuv420p10(pe_ctx* c, const void* rgba, int bits, int width, int height, void* yuv, void* stream) {
-    if (!c) return 1;
-    if (!rgba || !yuv) return c->fail("pe_rgba_to_yuv420p10: null argument");
-    if (bits != 8 && bits != 16) return c->fail("pe_rgba_to_yuv420p10: bits must be 8 or 16, got " + std::to_string(bits));
-    if (!yuv420p10_bytes(width, height))
-        return c->fail("pe_rgba_to_yuv420p10: invalid size " + std::to_string(width) + " x " + std::to_string(height) + " (1 <= width, height; at most 2^31 - 1 pixels)");
-    const uintptr_t word = bits == 16 ? 7 : 3;
-    if ((uintptr_t(rgba) & word) || (uintptr_t(yuv) & 1))
-        return c->fail("pe_rgba_to_yuv420p10: the frame must be " + std::to_string(word + 1) + "-byte and the planes 2-byte aligned");
-    if (!bind_device(c)) return 1;
-    if (!cuda_ok(c, (cudaError_t)launch_rgba_to_yuv420p10(rgba, bits, width, height, yuv, stream_of(c, stream)), "pe_rgba_to_yuv420p10")) return 1;
-    c->launches++;
-    return 0;
-}
-
-// ------------------------------------------------------------------------------ Y'CbCr 4:2:0 -> RGBA8 (pe_yuv.cu)
-size_t pe_yuv420_bytes(int width, int height, int bits) { return yuv420_bytes(width, height, bits); }
-
-}  // extern "C"
-
-namespace {
-
-// The format and the size of a conversion, checked before anything is copied or launched.
-bool check_yuv420(pe_ctx* c, const std::string& fn, const pe_yuv_format* f, int width, int height) {
-    if (!f) return !c->fail(fn + ": null format");
-    if (f->bits != 8 && f->bits != 10) return !c->fail(fn + ": bits must be 8 or 10, got " + std::to_string(f->bits));
-    if (f->matrix != PE_YUV_BT709 && f->matrix != PE_YUV_BT601) return !c->fail(fn + ": matrix must be PE_YUV_BT709 or PE_YUV_BT601");
-    if (f->full_range != 0 && f->full_range != 1) return !c->fail(fn + ": full_range must be 0 or 1");
-    if (f->siting != PE_YUV_SITING_LEFT && f->siting != PE_YUV_SITING_CENTER)
-        return !c->fail(fn + ": siting must be PE_YUV_SITING_LEFT or PE_YUV_SITING_CENTER");
-    if (!yuv420_bytes(width, height, f->bits))
-        return !c->fail(fn + ": invalid size " + std::to_string(width) + " x " + std::to_string(height) + " (1 <= width, height; at most 2^31 - 1 pixels)");
-    return true;
-}
-
-int yuv420_launch(pe_ctx* c, const void* yuv, const pe_yuv_format* f, int width, int height, void* rgba, cudaStream_t s, const char* fn) {
-    if (!cuda_ok(c, (cudaError_t)launch_yuv420_to_rgba8(yuv, f->bits, f->matrix, f->full_range, f->siting, width, height, rgba, s), fn)) return 1;
-    c->launches++;
-    return 0;
-}
-
-}  // namespace
-
-extern "C" {
-
-int pe_yuv420_to_rgba8(pe_ctx* c, const void* yuv, const pe_yuv_format* format, int width, int height, void* rgba8, void* stream) {
-    if (!c) return 1;
-    const std::string fn = "pe_yuv420_to_rgba8";
-    if (!yuv || !rgba8) return c->fail(fn + ": null argument");
-    if (!check_yuv420(c, fn, format, width, height)) return 1;
-    if ((uintptr_t(yuv) & uintptr_t(format->bits == 10 ? 1 : 0)) || (uintptr_t(rgba8) & 3))
-        return c->fail(fn + ": the planes must be " + std::string(format->bits == 10 ? "2" : "1") + "-byte and the image 4-byte aligned");
-    if (!bind_device(c)) return 1;
-    return yuv420_launch(c, yuv, format, width, height, rgba8, stream_of(c, stream), "pe_yuv420_to_rgba8");
-}
-
-int pe_set_texture_yuv420(pe_ctx* c, const char* name, const void* yuv_host, const pe_yuv_format* format, int width, int height) {
-    if (!c) return 1;
-    const std::string fn = "pe_set_texture_yuv420";
-    if (!name || !yuv_host) return c->fail(fn + ": null argument");
-    if (!check_yuv420(c, fn, format, width, height)) return 1;
-    ensure_layout(c);
-    auto it = c->layout.tex_slot.find(name);
-    if (it == c->layout.tex_slot.end()) return c->fail(std::string("unknown texture `") + name + "`", 2);
-    if (!bind_device(c)) return 1;
-    DeviceBuffer& t = c->textures[name];
-    const size_t bytes = size_t(width) * size_t(height) * 4, planes = yuv420_bytes(width, height, format->bits);
-    uint8_t* rec = c->cblock.data() + c->layout.off_tex + size_t(it->second) * 16;
-    // As pe_set_texture: a render queued on any stream may still read the image, so wait for the device before touching it.
-    // If that wait fails the old image stays allocated and bound.
-    if (t.dev && !cuda_ok(c, cudaDeviceSynchronize(), "pe_set_texture_yuv420: waiting for queued renders")) return 1;
-    if (t.bytes != bytes) {            // another size: free the old image; until the new one is in place the sampler is unbound
-        t.release();
-        std::memset(rec, 0, 16);
-        if (!cuda_ok(c, t.ensure(bytes), "cudaMalloc(texture)")) return 1;
-    }
-    if (!cuda_ok(c, c->yuv_upload.ensure(planes), "cudaMalloc(texture planes)") ||
-        !cuda_ok(c, cudaMemcpyAsync(c->yuv_upload.dev, yuv_host, planes, cudaMemcpyHostToDevice, c->stream), "cudaMemcpy(texture planes)") ||
-        yuv420_launch(c, c->yuv_upload.dev, format, width, height, t.dev, c->stream, "pe_set_texture_yuv420") ||
-        !cuda_ok(c, cudaStreamSynchronize(c->stream), "pe_set_texture_yuv420")) {
-        std::memset(rec, 0, 16);       // the image may be half written: unbind it, keep the memory (it is freed with the context)
-        return 1;
-    }
-    std::memcpy(rec, &t.dev, 8);
-    std::memcpy(rec + 8, &width, 4);
-    std::memcpy(rec + 12, &height, 4);
-    return 0;
 }
 
 }  // extern "C"

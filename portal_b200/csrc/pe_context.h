@@ -1,5 +1,6 @@
-// The context behind the C ABI's opaque `pe_ctx`, shared by pe_api.cpp (entry points, uniform block, launches) and
-// pe_program.cpp (NVRTC, the cubin cache, variant selection, module load and unload).  Not part of the C ABI.
+// The context behind the C ABI's opaque `pe_ctx`, shared by pe_api.cpp (entry points, uniform block, launches),
+// pe_frames.cpp (post-processing and encoding of frames) and pe_program.cpp (NVRTC, the cubin cache, variant selection,
+// module load and unload).  Not part of the C ABI.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -103,12 +104,14 @@ struct pe_ctx {
     // refill cursor, and the one-sample RGBA8 halo rows above and below the target's strips
     struct AdaptiveBuffers { pe_host::DeviceBuffer refine_list, refine_count, halo_above, halo_below; };
     AdaptiveBuffers adaptive[2];
-    // pe_encode_png_rgba8's work space: filtered stream, per-segment deflate output, segment sizes / offsets / checksums; and
-    // pe_encode_png_host's device copy of the file and its length
-    pe_host::DeviceBuffer png_work, png_file, png_size;
+    // pe_encode_png_rgba8's work space: filtered stream, per-segment deflate output, segment sizes / offsets / checksums
+    pe_host::DeviceBuffer png_work;
     // pe_encode_gif_frame's work space: occupancy bitmap, histogram, palette, index stream, per-segment LZW output, segment
-    // bit lengths / offsets; and pe_encode_gif_frame_host's device copy of the block and its length
-    pe_host::DeviceBuffer gif_work, gif_block, gif_size;
+    // bit lengths / offsets
+    pe_host::DeviceBuffer gif_work;
+    // the host forms of the encoders (pe_encode_png_host*, pe_encode_gif_frame_host): the device copy of the encoding and its
+    // length
+    pe_host::DeviceBuffer encoded, encoded_size;
     // pe_set_texture_yuv420's device copy of the Y'CbCr planes it converts
     pe_host::DeviceBuffer yuv_upload;
     // adaptive de-specialisation: a slot whose value differed between renders more than kMaxRespecialisations times is read
@@ -139,8 +142,19 @@ struct pe_ctx {
 
 namespace pe_host {
 
-// pe_api.cpp: build the layout and the default uniform block on first use.
+// pe_api.cpp.  True when `e` is cudaSuccess; otherwise the context's error becomes "`what`: <CUDA's message>".
+bool cuda_ok(pe_ctx* c, cudaError_t e, const char* what);
+// As cuda_ok for the error a helper-kernel launcher (pe_kernels.h) returned; on success its `kernels` launches are counted.
+bool launched(pe_ctx* c, int e, const char* what, int kernels = 1);
+// Make the context's device current; fails on a compile-only context.
+bool bind_device(pe_ctx* c);
+// The caller's stream, or the context's own for nullptr.
+cudaStream_t stream_of(pe_ctx* c, void* stream);
+// Build the layout and the default uniform block on first use.
 void ensure_layout(pe_ctx* c);
+
+// pe_frames.cpp: the format and the size of a Y'CbCr 4:2:0 conversion, checked before anything is copied or launched.
+bool check_yuv420(pe_ctx* c, const std::string& fn, const pe_yuv_format* f, int width, int height);
 
 // pe_program.cpp.  Make the variant for the current uniforms current (generate / compile / load instance 0 as needed).
 // Beyond what the context's options ask for, a call may need the probe or the refine kernel.  `counted`: the uniforms are

@@ -98,6 +98,7 @@ def test_png16_bound_and_argument_checks_without_a_device():
             (lambda: enc(a, 4, 4, a, 8192, a, None), "no CPU rendering path"),
             (lambda: host(None, 4, 4, buf, 8192, C.byref(ln)), "null argument"),
             (lambda: host(a, 40, 40, buf, 8192, C.byref(ln)), "below pe_png_bound_rgba16"),
+            (lambda: host(a + 4, 4, 4, buf, 8192, C.byref(ln)), "8-byte aligned"),
             (lambda: host(a, 4, 4, buf, 8192, C.byref(ln)), "no CPU rendering path"),
             (lambda: lib.pe_quantize_rgba16(ctx, a + 8, a, 4, None), "aligned"),
             (lambda: lib.pe_quantize_rgba16(ctx, a, a + 4, 4, None), "aligned"),
@@ -105,6 +106,7 @@ def test_png16_bound_and_argument_checks_without_a_device():
             (lambda: lib.pe_average_frames_rgba16(ctx, frames, 0, a, 4, None), "n_frames"),
             (lambda: lib.pe_average_frames_rgba16(ctx, frames, 65, a, 4, None), "n_frames"),
             (lambda: lib.pe_average_frames_rgba16(ctx, frames, 2, a + 4, 4, None), "aligned"),
+            (lambda: lib.pe_average_frames_rgba16(ctx, (C.c_void_p * 2)(a, None), 2, a, 4, None), "frame 1 is null"),
             (lambda: lib.pe_average_frames_rgba16(ctx, frames, 64, a, 4, None), "no CPU rendering path"),
         ]
         for k, (call, want) in enumerate(cases):

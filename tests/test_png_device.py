@@ -85,6 +85,7 @@ def test_png_bound_and_argument_checks_without_a_device():
             (lambda: host(a, 4, 4, buf, 4096, None), "null argument"),
             (lambda: host(a, 4, 0, buf, 4096, C.byref(ln)), "at least 1"),
             (lambda: host(a, 40, 40, buf, 4096, C.byref(ln)), "below pe_png_bound"),
+            (lambda: host(a + 2, 4, 4, buf, 4096, C.byref(ln)), "4-byte aligned"),
             (lambda: enc(a, 4, 4, a, 4096, a, None), "no CPU rendering path"),
             (lambda: host(a, 4, 4, buf, 4096, C.byref(ln)), "no CPU rendering path"),
         ]

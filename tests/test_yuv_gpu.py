@@ -47,6 +47,7 @@ def _convert_guarded(torch, ctx, frame, bits, w, h, off):
     lib = capi.lib()
     n = lib.pe_yuv420p10_bytes(w, h) // 2
     buf = torch.full((n + off + 64,), GUARD, dtype=torch.int16, device="cuda")
+    torch.cuda.synchronize()            # the conversion runs on the context's own stream, unordered with torch's fill
     assert lib.pe_rgba_to_yuv420p10(ctx, C.c_void_p(frame.data_ptr()), bits, w, h, C.c_void_p(buf.data_ptr() + 2 * off), None) == 0, \
         lib.pe_last_error(ctx)
     torch.cuda.synchronize()
