@@ -98,28 +98,39 @@ static bool ends_with(const std::string& s, const char* suffix) {
     return s.size() >= n && s.compare(s.size() - n, n, suffix) == 0;
 }
 
-// YUV4MPEG2 (the raw input ffmpeg and x265 read): the stream header with the tags ffmpeg's own muxer writes for full-range
-// yuv420p10le, then per frame "FRAME\n" and the Y, Cb, Cr planes as little-endian uint16.  Y4M cannot carry the matrix
-// (BT.709): the encode command states it (README.md, DESIGN.md section 5.4).
-static_assert(__BYTE_ORDER__ == __ORDER_LITTLE_ENDIAN__, "the planes are written as read back, in host byte order");
-static bool write_y4m_header(FILE* f, int width, int height, int fps) {
-    return std::fprintf(f, "YUV4MPEG2 W%d H%d F%d:1 Ip A1:1 C420p10 XYSCSS=420P10 XCOLORRANGE=FULL\n", width, height, fps) > 0;
-}
-static bool write_y4m_frame(FILE* f, const std::vector<uint8_t>& planes) {
-    return std::fputs("FRAME\n", f) >= 0 && std::fwrite(planes.data(), 1, planes.size(), f) == planes.size();
+// How a frame becomes output, decided once from the extension (of --output, or --frame-format) and --bit-depth: what
+// ph_player_render delivers (the container, rendered at `bits`), how those bytes become a file, and what messages call them
+enum FrameFile { AS_RETURNED, PPM, Y4M, GIF };
+struct FrameFormat {
+    FrameFile file = PPM;
+    int container = PH_OUT_PIXELS, bits = 8;
+    std::string ext;            // `render`'s files: DIR/<animation>/frame_<i><ext>, or the stream DIR/<animation><ext>
+    const char* name = "";      // the stream's name in messages
+    const char* what = "";      // what one ph_player_render call returns, in messages
+    bool stream() const { return file == Y4M || file == GIF; }   // `render`: one file per animation, not per frame
+};
+static FrameFormat frame_format(const std::string& ext, int bits) {
+    if (ext == ".png") return {AS_RETURNED, PH_OUT_PNG, bits, ext, "PNG", "PNG"};   // Image::export_png (main.rs:2939-2943)
+    if (ext == ".y4m") return {Y4M, PH_OUT_YUV420P10, bits, ext, "Y4M", "Y4M stream"};
+    if (ext == ".gif") return {GIF, PH_OUT_GIF, bits, ext, "GIF", "GIF frame"};
+    return {ends_with(ext, ".rgba") ? AS_RETURNED : PPM, PH_OUT_PIXELS, bits, ext, "image", "image"};
 }
 
-// GIF: pe_gif_header (with the loop block for an animation), then the frame blocks as ph_player_render returns them, then the
-// trailer
-static bool write_gif_header(FILE* f, int width, int height, bool loop) {
+// A stream: the header, each frame as ph_player_render returns it, the trailer.  Y4M: the tags ffmpeg's own muxer writes for
+// full-range yuv420p10le, "FRAME\n" and the Y, Cb, Cr planes as little-endian uint16 per frame, no trailer; it cannot carry the
+// matrix (BT.709): the encode command states it (README.md, DESIGN.md section 5.4).  GIF: pe_gif_header, the blocks, the trailer.
+static_assert(__BYTE_ORDER__ == __ORDER_LITTLE_ENDIAN__, "the planes are written as read back, in host byte order");
+static bool write_stream_header(FILE* f, const FrameFormat& fmt, int width, int height, int fps, bool loop) {
+    if (fmt.file == Y4M)
+        return std::fprintf(f, "YUV4MPEG2 W%d H%d F%d:1 Ip A1:1 C420p10 XYSCSS=420P10 XCOLORRANGE=FULL\n", width, height, fps) > 0;
     uint8_t h[64];
     const int n = pe_gif_header(width, height, loop ? 1 : 0, h, sizeof h);
     return n > 0 && std::fwrite(h, 1, size_t(n), f) == size_t(n);
 }
-static bool write_gif_block(FILE* f, const std::vector<uint8_t>& block) {
-    return std::fwrite(block.data(), 1, block.size(), f) == block.size();
+static bool write_stream_frame(FILE* f, const FrameFormat& fmt, const uint8_t* data, size_t len) {
+    return (fmt.file != Y4M || std::fputs("FRAME\n", f) >= 0) && std::fwrite(data, 1, len, f) == len;
 }
-static bool write_gif_trailer(FILE* f) { return std::fputc(0x3B, f) != EOF; }
+static bool write_stream_trailer(FILE* f, const FrameFormat& fmt) { return fmt.file != GIF || std::fputc(0x3B, f) != EOF; }
 
 // Centiseconds frame i of a GIF stream at `fps` shows for: round(100 (i + 1) / fps) - round(100 i / fps), halves up, so that
 // the first n frames last round(100 n / fps)
@@ -128,26 +139,10 @@ static int gif_delay(int i, int fps) {
     return int(r(i + 1) - r(i));
 }
 
-// How a frame becomes output, decided once from --output / --frame-format and --bit-depth: what ph_player_render delivers (the
-// container, rendered at `bits`) and how those bytes become a file
-enum FrameFile { AS_RETURNED, PPM, Y4M, GIF };
-struct FrameFormat {
-    FrameFile file;
-    int container, bits;
-};
-
-// One frame as ph_player_render returned it (`len` bytes of `px`) -> the file `path`: the bytes as they are (PNG; raw RGBA8, or
-// RGBA16 in host byte order, which is little-endian), a P6 PPM with alpha dropped (maxval 255, or 65535 with big-endian samples,
-// as the format defines), a one-frame Y4M stream at 25 fps, or a one-frame GIF (no loop block)
+// One frame as ph_player_render returned it (`len` bytes of `px`) -> the frame file `path`: the bytes as they are (PNG; raw
+// RGBA8, or RGBA16 in host byte order, which is little-endian), or a P6 PPM with alpha dropped (maxval 255, or 65535 with
+// big-endian samples, as the format defines)
 static bool write_frame(const std::string& path, const FrameFormat& fmt, const std::vector<uint8_t>& px, size_t len, int width, int height) {
-    if (fmt.file == Y4M || fmt.file == GIF) {
-        FILE* f = std::fopen(path.c_str(), "wb");
-        if (!f) return false;
-        const bool ok = fmt.file == Y4M ? write_y4m_header(f, width, height, 25) && write_y4m_frame(f, px)
-                                        : write_gif_header(f, width, height, false) &&
-                                              std::fwrite(px.data(), 1, len, f) == len && write_gif_trailer(f);
-        return std::fclose(f) == 0 && ok;
-    }
     std::ofstream out(path, std::ios::binary);
     if (!out) return false;
     if (fmt.file == AS_RETURNED) {
@@ -316,7 +311,159 @@ static bool parse_devices(const std::string& list, std::vector<int>& devices, st
     }
 }
 
-// One worker: a context, a scene parsed from the scene text, a player and the video runtimes, all its own
+// The command line
+struct Options {
+    bool frame_cmd = false;                  // render-frame; else render
+    std::string scene_path, output = "frame.ppm", out_dir = "video";
+    int width = 0, height = 0, depth = 0, aa = 0, fps = 60, motion_blur = 1, max_frames = -1;
+    bool stereo = false, skip_existing = true, adaptive = false;
+    int adaptive_threshold = 0, bits = 8, video_matrix = PE_YUV_BT709;
+    double time = 0.0;
+    std::vector<std::string> textures, videos, animations;
+    std::string stage, animation, camera, starts_with, assets;
+    bool all_animations = true;              // no --animations list: every animation, filtered by --starts-with
+    std::vector<int> devices;                // one worker per entry
+    FrameFormat fmt;
+    bool to_stdout = false;                  // `render` to a stream with --out-dir -
+    FILE* status = stdout;                   // stderr when stdout carries the stream
+};
+
+// Fills `o`; non-zero: the exit code of a refusal, reported at the first bad option, then for --devices
+static int parse_options(int argc, char** argv, Options& o) {
+    o.frame_cmd = argc >= 3 && std::strcmp(argv[1], "render-frame") == 0;
+    const bool anim_cmd = argc >= 3 && std::strcmp(argv[1], "render") == 0;
+    if (!o.frame_cmd && !anim_cmd) {
+        std::fprintf(stderr, "usage: %s render-frame <scene.ron> [--width W] [--height H] [--render-depth D] [--aa-count N] [--time T] "
+                             "[--stage NAME] [--animation NAME] [--camera NAME] [--device K] [--texture name=file.png|name=file.rgba:WxH] [--assets DIR] [--output out.png|.ppm|.rgba|.y4m|.gif] [--adaptive-aa T] [--bit-depth 8|16] [--video name=clip.y4m] [--video-matrix bt709|bt601]\n"
+                             "       %s render <scene.ron> [a,b | --animations a,b | --starts-with PREFIX] [--fps N] [--motion-blur-frames M] [--width W] [--height H] "
+                             "[--render-depth D] [--aa-count N] [--stereo-image] [--no-skip-existing] [--out-dir DIR] [--max-frames K] [--frame-format ppm|png|rgba|y4m|gif] [--adaptive-aa T] [--bit-depth 8|16] [--video name=clip.y4m] [--video-matrix bt709|bt601] [--device K | --devices K,K,...]\n", argv[0], argv[0]);
+        return 2;
+    }
+    o.scene_path = argv[2];
+    // defaults of RenderFrameCliOptions (main.rs:2744-2754) / RenderCliOptions (main.rs:2764-2803)
+    o.width = o.frame_cmd ? 1920 : 3840, o.height = o.frame_cmd ? 1080 : 2160, o.depth = o.frame_cmd ? 100 : 150, o.aa = o.frame_cmd ? 1 : 4;
+    int device = 0, first_option = 3;
+    bool device_given = false, devices_given = false;
+    std::string frame_ext = ".ppm", devices_list, animations;
+    if (anim_cmd && argc > 3 && std::strncmp(argv[3], "--", 2) != 0) animations = argv[first_option++];   // `render <scene> [animations]`
+    for (int i = first_option; i < argc; i++) {
+        std::string a = argv[i];
+        auto next = [&]() -> const char* { return i + 1 < argc ? argv[++i] : ""; };
+        if (a == "--width") o.width = std::atoi(next());
+        else if (a == "--height") o.height = std::atoi(next());
+        else if (a == "--render-depth" || a == "--render_depth") o.depth = std::atoi(next());
+        else if (a == "--aa-count" || a == "--aa_count") o.aa = std::atoi(next());
+        else if (a == "--time") o.time = std::atof(next());
+        else if (a == "--device") { device = std::atoi(next()); device_given = true; }
+        else if (a == "--devices") { devices_list = next(); devices_given = true; }
+        else if (a == "--stage") o.stage = next();
+        else if (a == "--animation") o.animation = next();
+        else if (a == "--camera") o.camera = next();
+        else if (a == "--animations") animations = next();
+        else if (a == "--starts-with" || a == "--filter-starts-with" || a == "--starts_with" || a == "--filter_starts_with") o.starts_with = next();
+        else if (a == "--fps") o.fps = std::atoi(next());
+        else if (a == "--motion-blur-frames" || a == "--motion_blur_frames") o.motion_blur = std::atoi(next());
+        else if (a == "--out-dir") o.out_dir = next();
+        else if (a == "--max-frames") o.max_frames = std::atoi(next());
+        else if (a == "--stereo-image" || a == "--stereoimage" || a == "--stereo_image") o.stereo = true;
+        else if (a == "--no-skip-existing" || a == "--no_skip_existing") o.skip_existing = false;
+        else if (a == "--output") o.output = next();
+        else if (a == "--texture") o.textures.push_back(next());
+        else if (a == "--video") o.videos.push_back(next());
+        else if (a == "--video-matrix" || a == "--video_matrix") {
+            const std::string v = next();
+            if (v != "bt709" && v != "bt601") { std::fprintf(stderr, "--video-matrix must be bt709 or bt601, got `%s`\n", v.c_str()); return 2; }
+            o.video_matrix = v == "bt601" ? PE_YUV_BT601 : PE_YUV_BT709;
+        }
+        else if (a == "--assets") o.assets = next();
+        else if (a == "--frame-format") frame_ext = std::string(".") + next();          // render: ppm (default) | png | rgba | y4m | gif
+        else if (a == "--adaptive-aa" || a == "--adaptive_aa") {
+            const char* v = next();
+            char* end = nullptr;
+            const long t = std::strtol(v, &end, 10);
+            if (!*v || *end) { std::fprintf(stderr, "--adaptive-aa needs an integer threshold, got `%s`\n", v); return 2; }
+            o.adaptive = true;
+            o.adaptive_threshold = int(std::max(-1L, std::min(t, 255L)));
+        }
+        else if (a == "--bit-depth" || a == "--bit_depth") {
+            const std::string v = next();
+            if (v != "8" && v != "16") { std::fprintf(stderr, "--bit-depth must be 8 or 16, got `%s`\n", v.c_str()); return 2; }
+            o.bits = std::atoi(v.c_str());
+        }
+        else { std::fprintf(stderr, "unknown option %s\n", a.c_str()); return 2; }
+    }
+    o.devices = {device};
+    if (devices_given) {
+        std::string why;
+        if (device_given) { std::fprintf(stderr, "--devices and --device exclude each other\n"); return 2; }
+        if (!parse_devices(devices_list, o.devices, why)) { std::fprintf(stderr, "--devices %s\n", why.c_str()); return 2; }
+        if (o.frame_cmd && o.devices.size() > 1) { std::fprintf(stderr, "render-frame renders one frame on one device: --devices takes one entry here, got `%s`\n", devices_list.c_str()); return 2; }
+    }
+    std::stringstream ss(animations);
+    for (std::string item; std::getline(ss, item, ',');) if (!item.empty()) o.animations.push_back(item);
+    o.all_animations = animations.empty();
+    const size_t dot = o.output.rfind('.');   // the frame's format: from the output's name (render-frame) or --frame-format (render)
+    o.fmt = frame_format(!o.frame_cmd ? frame_ext : dot == std::string::npos ? std::string() : o.output.substr(dot), o.bits);
+    o.to_stdout = anim_cmd && o.fmt.stream() && o.out_dir == "-";
+    o.status = o.to_stdout ? stderr : stdout;
+    return 0;
+}
+
+// The scene's animations in file order
+static std::vector<std::string> animation_names(ph_scene* scene) {
+    std::vector<std::string> names;
+    const char* nm = nullptr;
+    for (int a = 0; a < ph_scene_animation_count(scene); a++)
+        if (ph_scene_animation(scene, a, &nm, nullptr) == 0) names.push_back(nm);
+    return names;
+}
+// The duration of the last animation named `name`; 0 when there is none
+static double animation_duration(ph_scene* scene, const std::string& name) {
+    double duration = 0.0, d = 0.0;
+    const char* nm = nullptr;
+    for (int a = 0; a < ph_scene_animation_count(scene); a++)
+        if (ph_scene_animation(scene, a, &nm, &d) == 0 && name == nm) duration = d;
+    return duration;
+}
+static bool has_video(ph_scene* scene, const std::string& name) {
+    const char *nm = nullptr, *path = nullptr, *uniform = nullptr;
+    for (int k = 0; ph_scene_video(scene, k, &nm, &path, &uniform) == 0; k++)
+        if (name == nm) return true;
+    return false;
+}
+// render: --animations a,b -> render_named_animations (main.rs:1876-1930); otherwise render_all_animations (:1932-1974): every
+// animation in file order is initialised and updated once, and rendered unless --starts-with filters it out
+static bool is_rendered(const Options& o, const std::string& name) {
+    return !o.all_animations || o.starts_with.empty() || name.compare(0, o.starts_with.size(), o.starts_with) == 0;
+}
+
+// The refusals that need the scene's animation list, before any context exists: --out-dir - and GIF's limits
+static int check_output(const Options& o, const std::vector<std::string>& names) {
+    const size_t selected = size_t(std::count_if(names.begin(), names.end(), [&](const std::string& nm) { return is_rendered(o, nm); }));
+    if (o.to_stdout && selected != 1) { std::fprintf(stderr, "--out-dir - writes one %s stream to stdout: select exactly one animation (%zu selected)\n", o.fmt.name, selected); return 2; }
+    if (o.fmt.file != GIF) return 0;
+    if (o.bits != 8) { std::fprintf(stderr, "GIF frames are 8-bit: --bit-depth 16 cannot be written as GIF\n"); return 2; }
+    if (!o.frame_cmd && o.fps > 50) { std::fprintf(stderr, "--fps %d is above 50: GIF delays are whole centiseconds and browsers show a delay below 2 cs as 10 cs; use --fps 50, 33 or 25\n", o.fps); return 2; }
+    if (o.fps < 1 && !o.frame_cmd) { std::fprintf(stderr, "--fps must be at least 1 for GIF, got %d\n", o.fps); return 2; }
+    const bool doubled = o.stereo && !o.frame_cmd;
+    const long long gif_w = doubled ? 2LL * o.width : o.width;
+    if (gif_w >= 1 && o.height >= 1 && gif_w <= 65535 && o.height <= 65535) return 0;
+    std::fprintf(stderr, "a GIF frame is 1 .. 65535 pixels wide and high, got %lld x %d%s\n", gif_w, o.height, doubled ? " (stereo doubles the width)" : "");
+    return 2;
+}
+// --video name=clip.y4m: every clip is opened (and refused) before a context exists, into `clips` by video name
+static int open_given_clips(const Options& o, ph_scene* scene, std::map<std::string, VideoRuntime>& clips) {
+    for (const std::string& g : o.videos) {
+        const size_t eq = g.find('=');
+        const std::string name = eq == std::string::npos ? std::string() : g.substr(0, eq), path = eq == std::string::npos ? g : g.substr(eq + 1);
+        if (!has_video(scene, name)) { std::fprintf(stderr, "--video %s: the scene has no video named `%s`\n", g.c_str(), name.c_str()); return 1; }
+        std::string why;
+        if (!open_clip(clips[name], path, o.video_matrix, why)) { std::fprintf(stderr, "--video %s: %s\n", g.c_str(), why.c_str()); return 1; }
+    }
+    return 0;
+}
+
+// One worker: a context, a scene parsed from the scene text, a player and the video runtimes, all its own, released together
 struct Worker {
     pe_ctx* ctx = nullptr;
     ph_scene* scene = nullptr;
@@ -325,10 +472,23 @@ struct Worker {
     std::vector<uint8_t> px;                          // the frame as ph_player_render returns it
     size_t len = 0;                                   // its bytes
     std::vector<std::vector<uint8_t>> free_planes;   // `render` to a stream: the frame buffers the main thread does not hold
+    Worker() = default;
+    Worker(const Worker&) = delete;              // nor movable: see video_state
+    Worker& operator=(const Worker&) = delete;
+    ~Worker() {
+        for (VideoRuntime& v : video_state.videos) {
+            if (v.planes) pe_host_free(ctx, v.planes);
+            ph_y4m_close(v.clip);
+        }
+        ph_player_free(player);
+        pe_destroy(ctx);
+        ph_scene_free(scene);
+    }
 };
 
 // What `render` does with one entry of the animation list, decided before any worker starts
 struct AnimationPlan {
+    std::string name;
     bool rendered = false;           // false: --starts-with filters it out (it is still initialised and updated once)
     double duration = 0.0;           // the f32 duration render_animation takes
     int count = 1, todo = 0;         // frames of the animation, frames to render (--max-frames)
@@ -386,427 +546,265 @@ struct Shared {
     }
 };
 
+// A worker's set-up, everything up to the first frame, in steps that return the exit code of a failure they report
+// The player, and render-frame's --stage, --animation and --camera (main.rs:2900-2926)
+static int start_player(const Options& o, Worker& wk) {
+    wk.player = ph_player_new(wk.scene);
+    if (o.adaptive) ph_player_set_adaptive_aa(wk.player, 1, o.adaptive_threshold);
+    const struct { const std::string& name; int (*select)(ph_player*, const char*); const char* what; } picks[] = {
+        {o.stage, ph_player_init_stage, "stage"}, {o.animation, ph_player_init_animation, "animation"}, {o.camera, ph_player_select_camera, "camera"}};
+    for (const auto& s : picks)
+        if (o.frame_cmd && !s.name.empty() && s.select(wk.player, s.name.c_str())) { std::fprintf(stderr, "Scene `%s` has no %s named `%s`\n", o.scene_path.c_str(), s.what, s.name.c_str()); return 1; }
+    return 0;
+}
+static int build_program(Worker& wk) {
+    if (!ph_scene_build_program(wk.scene, wk.ctx) && !ph_scene_upload_uniforms(wk.scene, wk.ctx)) return 0;
+    std::fprintf(stderr, "%s\n", ph_scene_last_error(wk.scene));
+    return 1;
+}
+// --texture name=file.png | name=file.rgba:WxH, then every other texture of the scene from its stored path (reload_textures,
+// main.rs:1066-1085), where a failure is reported and the render goes on
+static int set_textures(const Options& o, Worker& wk, bool first, std::map<std::string, DecodedPng>& decoded) {
+    std::set<std::string> given;
+    std::string why;
+    for (const std::string& t : o.textures) {
+        size_t eq = t.find('='), colon = t.rfind(':'), x = t.rfind('x');
+        given.insert(t.substr(0, eq));
+        if (eq != std::string::npos && ends_with(t, ".png")) {
+            if (!set_texture_decoded(wk.ctx, t.substr(0, eq), decode_png_once(decoded, t.substr(eq + 1)), why)) { std::fprintf(stderr, "texture %s: %s\n", t.c_str(), why.c_str()); return 1; }
+            continue;
+        }
+        if (eq == std::string::npos || colon == std::string::npos || x == std::string::npos || x < colon) { std::fprintf(stderr, "bad --texture %s\n", t.c_str()); return 2; }
+        int tw = std::atoi(t.substr(colon + 1, x - colon - 1).c_str()), th = std::atoi(t.substr(x + 1).c_str());
+        bool tok = false;
+        std::string bytes = slurp(t.substr(eq + 1, colon - eq - 1), tok);
+        if (!tok || bytes.size() != size_t(tw) * size_t(th) * 4) { std::fprintf(stderr, "texture %s: cannot read / wrong size\n", t.c_str()); return 1; }
+        if (pe_set_texture(wk.ctx, t.substr(0, eq).c_str(), reinterpret_cast<const uint8_t*>(bytes.data()), tw, th)) { std::fprintf(stderr, "%s\n", pe_last_error(wk.ctx)); return 1; }
+    }
+    for (int k = 0;; k++) {
+        const char *name = nullptr, *path = nullptr;
+        if (ph_scene_texture(wk.scene, k, &name, &path)) break;
+        if (given.count(name)) continue;
+        const std::string file = o.assets.empty() || (path[0] == '/') ? std::string(path) : o.assets + "/" + path;
+        if (!set_texture_decoded(wk.ctx, name, decode_png_once(decoded, file), why) && first)
+            std::fprintf(stderr, "texture `%s`: %s (the sampler stays unbound)\n", name, why.c_str());
+    }
+    return 0;
+}
+// The source of video `name` (stored path `path`) in the order above, into `v`, and `source` for the status line: empty when
+// there is none.  The first worker takes over the --video clips opened before, leaving null handles in `given_clips`; the
+// others open their own.  False: a --video clip cannot be opened again (reported).
+static bool video_source(const Options& o, const char* name, const char* path, bool first, std::map<std::string, VideoRuntime>& given_clips, VideoRuntime& v, std::string& source) {
+    std::string why;
+    const auto it = given_clips.find(name);
+    if (it != given_clips.end()) {
+        const std::string given_path = videos_path_of(o.videos, name);
+        if (first && it->second.clip) {
+            v = it->second;
+            it->second.clip = nullptr;
+        } else if (!open_clip(v, given_path, o.video_matrix, why, true)) { std::fprintf(stderr, "--video %s=%s: %s\n", name, given_path.c_str(), why.c_str()); return false; }
+        source = clip_description(given_path, v);
+    } else if (!(v.frames = video_frame_files(o.assets, path)).empty()) {
+        source = std::to_string(v.frames.size()) + " PNG frames in " + v.frames[0].substr(0, v.frames[0].rfind('/'));
+    } else {
+        char rel[1024];
+        const int n = ph_video_frames_dir(path, rel, sizeof rel);
+        const std::string stem = n > 0 ? std::string(rel).substr(std::string(rel).find('/') + 1) : std::string();
+        const std::string clip = (o.assets.empty() ? std::string() : o.assets + "/") + "video_y4m/" + stem + ".y4m";
+        if (stem.empty() || !file_exists(clip)) return true;
+        if (!open_clip(v, clip, o.video_matrix, why, !first)) { if (first) std::fprintf(stderr, "video `%s`: %s (the sampler is not updated)\n", name, why.c_str()); return true; }
+        source = clip_description(clip, v);
+    }
+    return true;
+}
+// VideoRuntime::from_scene (main.rs:820-858): the videos that have a path, a uniform and a source, played by the update hook
+static int set_videos(const Options& o, Worker& wk, bool first, std::map<std::string, VideoRuntime>& given_clips) {
+    VideoState& video_state = wk.video_state = {wk.scene, wk.ctx, {}};
+    for (int k = 0;; k++) {
+        const char *name = nullptr, *path = nullptr, *uniform = nullptr;
+        if (ph_scene_video(wk.scene, k, &name, &path, &uniform)) break;
+        if (!path[0] || !uniform[0]) continue;
+        VideoRuntime v;
+        std::string source;
+        if (!video_source(o, name, path, first, given_clips, v, source)) return 1;
+        if (source.empty()) continue;
+        v.video = k;
+        v.name = name;
+        video_state.videos.push_back(v);
+        if (v.clip && pe_host_malloc(wk.ctx, v.planes_bytes, &video_state.videos.back().planes)) { std::fprintf(stderr, "%s\n", pe_last_error(wk.ctx)); return 1; }
+        if (first) std::fprintf(o.status, "video `%s`: %s\n", name, source.c_str());
+    }
+    if (first)                        // the clips it did not take: a video without a path or a uniform plays nothing
+        for (auto& kv : given_clips) { ph_y4m_close(kv.second.clip); kv.second.clip = nullptr; }
+    if (!video_state.videos.empty()) ph_player_set_update_hook(wk.player, update_videos, &video_state);
+    return 0;
+}
+// Only the first worker reports what it finds (textures, videos): the others find the same
+static int set_up(const Options& o, Worker& wk, bool first, std::map<std::string, DecodedPng>& decoded, std::map<std::string, VideoRuntime>& given_clips) {
+    if (const int rc = start_player(o, wk)) return rc;
+    if (const int rc = build_program(wk)) return rc;
+    if (const int rc = set_textures(o, wk, first, decoded)) return rc;
+    if (pe_scene_compile(wk.ctx)) { std::fprintf(stderr, "%s\n", pe_last_error(wk.ctx)); return 1; }
+    ph_player_attach(wk.player, wk.ctx);  // camera teleportation goes through pe_probe_ray
+    if (const int rc = set_videos(o, wk, first, given_clips)) return rc;
+    if (o.stereo) ph_player_set_stereo(wk.player, 1, 0.07, 0);         // `render --stereo-image` (main.rs:2809-2816, 2842)
+    return 0;
+}
+
+// render-frame (main.rs:2928-2946)
+static int render_frame(const Options& o, Worker& wk, const ph_frame_params& p, size_t frame_bytes) {
+    wk.px.resize(frame_bytes);
+    if (ph_player_update(wk.player, o.time) ||
+        ph_player_render(wk.player, wk.ctx, &p, nullptr, o.fmt.container, o.fmt.bits, wk.px.data(), wk.px.size(), &wk.len)) { std::fprintf(stderr, "%s\n", ph_player_last_error(wk.player)); return 1; }
+    FILE* f = o.fmt.stream() ? std::fopen(o.output.c_str(), "wb") : nullptr;    // a one-frame stream: 25 fps, no GIF loop block
+    const bool ok = !o.fmt.stream() ? write_frame(o.output, o.fmt, wk.px, wk.len, p.width, p.height)
+                                    : f && write_stream_header(f, o.fmt, p.width, p.height, 25, false) && write_stream_frame(f, o.fmt, wk.px.data(), wk.len) && write_stream_trailer(f, o.fmt);
+    if ((f && std::fclose(f) != 0) || !ok) { std::fprintf(stderr, "cannot write %s\n", o.output.c_str()); return 1; }
+    std::printf("Rendered `%s` to `%s`\n", o.scene_path.c_str(), o.output.c_str());
+    return 0;
+}
+// The plan: every skip decision from one snapshot of the output, taken now, plus what the animations before each one will
+// write (a name listed twice), so that the decisions are the sequential loop's and no worker's write can change another's
+static std::vector<AnimationPlan> plan_animations(const Options& o, ph_scene* scene, const std::vector<std::string>& names) {
+    std::vector<AnimationPlan> plan(names.size());
+    std::set<std::string> to_write;
+    auto skip = [&](const std::string& file) {                          // main.rs:1771-1779 (a stream), 1789-1793 (frames)
+        const bool exists = o.skip_existing && (file_exists(file) || to_write.count(file));
+        if (!exists) to_write.insert(file);
+        return exists;
+    };
+    for (size_t k = 0; k < names.size(); k++) {
+        AnimationPlan& a = plan[k];
+        a.name = names[k];
+        a.rendered = is_rendered(o, a.name);
+        const float duration32 = float(animation_duration(scene, a.name));   // render_animation takes f32
+        a.duration = double(duration32);
+        a.count = int(duration32 * float(o.fps));                            // main.rs:1785
+        if (a.count < 1) a.count = 1;
+        a.todo = o.max_frames >= 0 && o.max_frames < a.count ? o.max_frames : a.count;
+        a.skip_frame.assign(size_t(a.todo), 0);
+        if (!a.rendered || o.to_stdout) continue;
+        const std::string dir = o.out_dir + "/" + a.name;
+        if (o.fmt.stream()) a.skip_stream = skip(dir + o.fmt.ext);
+        else
+            for (int i = 0; i < a.todo; i++) a.skip_frame[size_t(i)] = skip(dir + "/frame_" + std::to_string(i) + o.fmt.ext);
+    }
+    return plan;
+}
+// One worker's run through every animation: it renders frame i when i mod N is `me` and advances through the others
+static void run_worker(const Options& o, const std::vector<AnimationPlan>& plan, std::vector<Worker>& workers, size_t me, const ph_frame_params& p, size_t frame_bytes, Shared& sh) {
+    Worker& wk = workers[me];
+    for (size_t k = 0; k < plan.size(); k++) {
+        const AnimationPlan& a = plan[k];
+        if (sh.stopped()) return;
+        if (ph_player_init_animation(wk.player, a.name.c_str())) { sh.fail("Scene `" + o.scene_path + "` has no animation named `" + a.name + "`"); return; }
+        if (ph_player_update(wk.player, 0.0)) { sh.fail(ph_player_last_error(wk.player)); return; }
+        if (!a.rendered) continue;
+        if (me == 0) sh.post(k, -1, {});
+        if (a.skip_stream) continue;
+        const std::string dir = o.out_dir + "/" + a.name;
+        if (!o.fmt.stream() && !make_dirs(dir)) { sh.fail("cannot create " + dir); return; }
+        for (int i = 0; i < a.todo; i++) {
+            if (sh.stopped()) return;
+            if (a.skip_frame[size_t(i)]) continue;                 // neither rendered nor advanced, as the sequential loop
+            if (size_t(i) % workers.size() != me) {
+                if (ph_player_advance_motion_blur_frame(wk.player, i, a.count, o.motion_blur, a.duration)) { sh.fail(ph_player_last_error(wk.player)); return; }
+                continue;
+            }
+            std::vector<uint8_t> planes;                           // a stream: the frame goes to the main thread
+            if (o.fmt.stream() && !sh.take_buffer(wk, planes)) return;
+            if (o.fmt.stream()) planes.resize(frame_bytes);          // a GIF block came back cut to its length
+            std::vector<uint8_t>& buf = o.fmt.stream() ? planes : wk.px;
+            const ph_motion_blur mb = {i, a.count, o.motion_blur, a.duration};
+            if ((o.fmt.file == GIF && ph_player_set_gif_delay(wk.player, gif_delay(i, o.fps))) ||
+                ph_player_render(wk.player, wk.ctx, &p, &mb, o.fmt.container, o.fmt.bits, buf.data(), buf.size(), &wk.len)) { sh.fail(ph_player_last_error(wk.player)); return; }
+            const std::string name = dir + "/frame_" + std::to_string(i) + o.fmt.ext;
+            if (o.fmt.stream()) planes.resize(wk.len);
+            else if (!write_frame(name, o.fmt, wk.px, wk.len, p.width, p.height)) { sh.fail("cannot write " + name); return; }
+            sh.post(k, i, std::move(planes));
+        }
+    }
+}
+// The main thread's run: status lines and streams, in frame order, up to the first failure.  A stream is written under a
+// temporary name and renamed when complete, so that an interrupted run leaves no stream for skip-existing to take as done.
+static void write_in_order(const Options& o, const std::vector<AnimationPlan>& plan, std::vector<Worker>& workers, const ph_frame_params& p, Shared& sh) {
+    std::vector<uint8_t> planes;
+    for (size_t k = 0; k < plan.size(); k++) {
+        const AnimationPlan& a = plan[k];
+        if (!a.rendered) continue;
+        if (!sh.take(k, -1, planes)) return;
+        std::fprintf(o.status, "Rendering animation %s, %zu/%zu\n", a.name.c_str(), k + 1, plan.size());
+        if (a.skip_stream) { std::fprintf(o.status, "Skip `%s`, because it's already exists\n", a.name.c_str()); continue; }
+        const std::string file = o.out_dir + "/" + a.name + o.fmt.ext, part = file + ".part";
+        FILE* f = nullptr;
+        bool ok = true, stopped = false;
+        if (o.fmt.stream()) {
+            if (!o.to_stdout && !make_dirs(o.out_dir)) { sh.fail("cannot create " + o.out_dir); return; }
+            f = o.to_stdout ? stdout : std::fopen(part.c_str(), "wb");
+            ok = f && write_stream_header(f, o.fmt, p.width, p.height, o.fps, true);
+        }
+        for (int i = 0; i < a.todo && ok; i++) {
+            if (a.skip_frame[size_t(i)]) continue;
+            if (!sh.take(k, i, planes)) { stopped = true; break; }
+            if (o.fmt.stream()) {
+                ok = write_stream_frame(f, o.fmt, planes.data(), planes.size());
+                sh.give_back(workers[size_t(i) % workers.size()], planes);
+            }
+            std::fprintf(o.status, "\r%d/%d done      ", i + 1, a.count);
+            std::fflush(o.status);
+        }
+        if (o.fmt.stream()) {
+            if (ok && !stopped) ok = write_stream_trailer(f, o.fmt);
+            if (f) ok = (o.to_stdout ? std::fflush(f) : std::fclose(f)) == 0 && ok;
+            if (!stopped && (!ok || (!o.to_stdout && std::rename(part.c_str(), file.c_str()) != 0))) { sh.fail(std::string("cannot write ") + (o.to_stdout ? "the stream to stdout" : file.c_str())); return; }
+        }
+        if (stopped) return;                                           // a stream keeps its .part name
+        std::fprintf(o.status, "\n");
+    }
+}
+// render (render_animation, main.rs:1757-1830), one thread per worker
+static int render_animations(const Options& o, ph_scene* scene, const std::vector<std::string>& names, std::vector<Worker>& workers, const ph_frame_params& p, size_t frame_bytes) {
+    const std::vector<AnimationPlan> plan = plan_animations(o, scene, names);
+    for (Worker& wk : workers) {       // a stream: two buffers per worker, which travel to the main thread and back
+        if (o.fmt.stream()) wk.free_planes.assign(2, std::vector<uint8_t>(frame_bytes));
+        else wk.px.resize(frame_bytes);
+    }
+    Shared sh;
+    std::vector<std::thread> threads;
+    for (size_t w = 0; w < workers.size(); w++) threads.emplace_back([&, w] { run_worker(o, plan, workers, w, p, frame_bytes, sh); });
+    write_in_order(o, plan, workers, p, sh);
+    for (std::thread& t : threads) t.join();
+    if (sh.stop) std::fprintf(stderr, "%s\n", sh.error.c_str());
+    return sh.stop ? 1 : 0;
+}
+
 int main(int argc, char** argv) {
-    const bool frame_cmd = argc >= 3 && std::strcmp(argv[1], "render-frame") == 0;
-    const bool anim_cmd = argc >= 3 && std::strcmp(argv[1], "render") == 0;
-    if (!frame_cmd && !anim_cmd) {
-        std::fprintf(stderr, "usage: %s render-frame <scene.ron> [--width W] [--height H] [--render-depth D] [--aa-count N] [--time T] "
-                             "[--stage NAME] [--animation NAME] [--camera NAME] [--device K] [--texture name=file.png|name=file.rgba:WxH] [--assets DIR] [--output out.png|.ppm|.rgba|.y4m|.gif] [--adaptive-aa T] [--bit-depth 8|16] [--video name=clip.y4m] [--video-matrix bt709|bt601]\n"
-                             "       %s render <scene.ron> [a,b | --animations a,b | --starts-with PREFIX] [--fps N] [--motion-blur-frames M] [--width W] [--height H] "
-                             "[--render-depth D] [--aa-count N] [--stereo-image] [--no-skip-existing] [--out-dir DIR] [--max-frames K] [--frame-format ppm|png|rgba|y4m|gif] [--adaptive-aa T] [--bit-depth 8|16] [--video name=clip.y4m] [--video-matrix bt709|bt601] [--device K | --devices K,K,...]\n", argv[0], argv[0]);
-        return 2;
-    }
-    std::string scene_path = argv[2], output = "frame.ppm", out_dir = "video";
-    // defaults of RenderFrameCliOptions (main.rs:2744-2754) / RenderCliOptions (main.rs:2764-2803)
-    int width = frame_cmd ? 1920 : 3840, height = frame_cmd ? 1080 : 2160, depth = frame_cmd ? 100 : 150, aa = frame_cmd ? 1 : 4, device = 0;
-    int fps = 60, motion_blur = 1, max_frames = -1;
-    bool stereo = false, skip_existing = true, adaptive = false, device_given = false, devices_given = false;
-    int adaptive_threshold = 0, bits = 8;
-    double time = 0.0;
-    std::vector<std::string> textures, videos;
-    int video_matrix = PE_YUV_BT709;
-    std::string stage, animation, camera, animations, starts_with, assets, frame_ext = ".ppm", devices_list;
-    int first_option = 3;
-    if (anim_cmd && argc > 3 && std::strncmp(argv[3], "--", 2) != 0) animations = argv[first_option++];   // `render <scene> [animations]`
-    for (int i = first_option; i < argc; i++) {
-        std::string a = argv[i];
-        auto next = [&]() -> const char* { return i + 1 < argc ? argv[++i] : ""; };
-        if (a == "--width") width = std::atoi(next());
-        else if (a == "--height") height = std::atoi(next());
-        else if (a == "--render-depth" || a == "--render_depth") depth = std::atoi(next());
-        else if (a == "--aa-count" || a == "--aa_count") aa = std::atoi(next());
-        else if (a == "--time") time = std::atof(next());
-        else if (a == "--device") { device = std::atoi(next()); device_given = true; }
-        else if (a == "--devices") { devices_list = next(); devices_given = true; }
-        else if (a == "--stage") stage = next();
-        else if (a == "--animation") animation = next();
-        else if (a == "--camera") camera = next();
-        else if (a == "--animations") animations = next();
-        else if (a == "--starts-with" || a == "--filter-starts-with" || a == "--starts_with" || a == "--filter_starts_with") starts_with = next();
-        else if (a == "--fps") fps = std::atoi(next());
-        else if (a == "--motion-blur-frames" || a == "--motion_blur_frames") motion_blur = std::atoi(next());
-        else if (a == "--out-dir") out_dir = next();
-        else if (a == "--max-frames") max_frames = std::atoi(next());
-        else if (a == "--stereo-image" || a == "--stereoimage" || a == "--stereo_image") stereo = true;
-        else if (a == "--no-skip-existing" || a == "--no_skip_existing") skip_existing = false;
-        else if (a == "--output") output = next();
-        else if (a == "--texture") textures.push_back(next());
-        else if (a == "--video") videos.push_back(next());
-        else if (a == "--video-matrix" || a == "--video_matrix") {
-            const std::string v = next();
-            if (v != "bt709" && v != "bt601") { std::fprintf(stderr, "--video-matrix must be bt709 or bt601, got `%s`\n", v.c_str()); return 2; }
-            video_matrix = v == "bt601" ? PE_YUV_BT601 : PE_YUV_BT709;
-        }
-        else if (a == "--assets") assets = next();
-        else if (a == "--frame-format") frame_ext = std::string(".") + next();          // render: ppm (default) | png | rgba | y4m | gif
-        else if (a == "--adaptive-aa" || a == "--adaptive_aa") {
-            const char* v = next();
-            char* end = nullptr;
-            const long t = std::strtol(v, &end, 10);
-            if (!*v || *end) { std::fprintf(stderr, "--adaptive-aa needs an integer threshold, got `%s`\n", v); return 2; }
-            adaptive = true;
-            adaptive_threshold = int(std::max(-1L, std::min(t, 255L)));
-        }
-        else if (a == "--bit-depth" || a == "--bit_depth") {
-            const std::string v = next();
-            if (v != "8" && v != "16") { std::fprintf(stderr, "--bit-depth must be 8 or 16, got `%s`\n", v.c_str()); return 2; }
-            bits = std::atoi(v.c_str());
-        }
-        else { std::fprintf(stderr, "unknown option %s\n", a.c_str()); return 2; }
-    }
-    std::vector<int> devices = {device};         // one worker per entry
-    if (devices_given) {
-        std::string why;
-        if (device_given) { std::fprintf(stderr, "--devices and --device exclude each other\n"); return 2; }
-        if (!parse_devices(devices_list, devices, why)) { std::fprintf(stderr, "--devices %s\n", why.c_str()); return 2; }
-        if (frame_cmd && devices.size() > 1) {
-            std::fprintf(stderr, "render-frame renders one frame on one device: --devices takes one entry here, got `%s`\n", devices_list.c_str());
-            return 2;
-        }
-    }
+    Options o;
+    if (const int rc = parse_options(argc, argv, o)) return rc;
     bool ok = false;
-    std::string text = slurp(scene_path, ok);
-    if (!ok) { std::fprintf(stderr, "cannot read %s\n", scene_path.c_str()); return 1; }
+    const std::string text = slurp(o.scene_path, ok);
+    if (!ok) { std::fprintf(stderr, "cannot read %s\n", o.scene_path.c_str()); return 1; }
     char err[2048] = {0};
     ph_scene* scene = ph_scene_load_ron(text.data(), text.size(), err, sizeof err);
-    if (!scene) { std::fprintf(stderr, "Failed to parse scene `%s`: %s\n", scene_path.c_str(), err); return 1; }
-    // render: --animations a,b -> render_named_animations (main.rs:1876-1930); otherwise render_all_animations (:1932-1974): every
-    // animation in file order is initialised and updated once, and rendered unless --starts-with filters it out
-    std::vector<std::string> names;
-    const bool all = animations.empty();
-    size_t selected = 0;
-    if (anim_cmd) {
-        if (all) {
-            for (int a = 0; a < ph_scene_animation_count(scene); a++) {
-                const char* nm = nullptr;
-                if (ph_scene_animation(scene, a, &nm, nullptr) == 0) names.push_back(nm);
-            }
-        } else {
-            std::stringstream ss(animations);
-            for (std::string item; std::getline(ss, item, ',');) if (!item.empty()) names.push_back(item);
-        }
-        for (const std::string& nm : names) selected += !all || starts_with.empty() || nm.compare(0, starts_with.size(), starts_with) == 0;
-    }
-    // the frame's format: from the output's name (render-frame) or --frame-format (render), at --bit-depth
-    auto format_is = [&](const char* ext) { return frame_cmd ? ends_with(output, ext) : frame_ext == ext; };
-    const FrameFormat fmt = format_is(".png")   ? FrameFormat{AS_RETURNED, PH_OUT_PNG, bits}   // Image::export_png (main.rs:2939-2943)
-                            : format_is(".y4m") ? FrameFormat{Y4M, PH_OUT_YUV420P10, bits}
-                            : format_is(".gif") ? FrameFormat{GIF, PH_OUT_GIF, bits}
-                                                : FrameFormat{ends_with(frame_cmd ? output : frame_ext, ".rgba") ? AS_RETURNED : PPM, PH_OUT_PIXELS, bits};
-    const bool stream = anim_cmd && (fmt.file == Y4M || fmt.file == GIF);    // one file per animation, not per frame
-    const std::string stream_ext = fmt.file == GIF ? ".gif" : ".y4m";
-    const bool to_stdout = stream && out_dir == "-";
-    if (to_stdout && selected != 1) {
-        std::fprintf(stderr, "--out-dir - writes one %s stream to stdout: select exactly one animation (%zu selected)\n", fmt.file == GIF ? "GIF" : "Y4M", selected);
-        return 2;
-    }
-    if (fmt.file == GIF) {                          // refused before any context exists
-        if (bits != 8) { std::fprintf(stderr, "GIF frames are 8-bit: --bit-depth 16 cannot be written as GIF\n"); return 2; }
-        if (anim_cmd && fps > 50) {
-            std::fprintf(stderr, "--fps %d is above 50: GIF delays are whole centiseconds and browsers show a delay below 2 cs as 10 cs; use --fps 50, 33 or 25\n", fps);
-            return 2;
-        }
-        if (fps < 1 && anim_cmd) { std::fprintf(stderr, "--fps must be at least 1 for GIF, got %d\n", fps); return 2; }
-        const long long gif_w = stereo && anim_cmd ? 2LL * width : width;
-        if (gif_w < 1 || height < 1 || gif_w > 65535 || height > 65535) {
-            std::fprintf(stderr, "a GIF frame is 1 .. 65535 pixels wide and high, got %lld x %d%s\n", gif_w, height, stereo && anim_cmd ? " (stereo doubles the width)" : "");
-            return 2;
-        }
-    }
-    FILE* status = to_stdout ? stderr : stdout;     // stdout carries the stream
-    // --video name=clip.y4m: every clip is opened (and refused) before a context exists
+    if (!scene) { std::fprintf(stderr, "Failed to parse scene `%s`: %s\n", o.scene_path.c_str(), err); return 1; }
+    const std::vector<std::string> names = o.frame_cmd ? std::vector<std::string>() : o.all_animations ? animation_names(scene) : o.animations;
+    if (const int rc = check_output(o, names)) return rc;
     std::map<std::string, VideoRuntime> given_clips;
-    for (const std::string& g : videos) {
-        const size_t eq = g.find('=');
-        const std::string name = eq == std::string::npos ? std::string() : g.substr(0, eq), path = eq == std::string::npos ? g : g.substr(eq + 1);
-        bool known = false;
-        for (int k = 0;; k++) {
-            const char *nm = nullptr, *vp = nullptr, *un = nullptr;
-            if (ph_scene_video(scene, k, &nm, &vp, &un)) break;
-            known = known || name == nm;
-        }
-        if (!known) { std::fprintf(stderr, "--video %s: the scene has no video named `%s`\n", g.c_str(), name.c_str()); return 1; }
-        std::string why;
-        if (!open_clip(given_clips[name], path, video_matrix, why)) { std::fprintf(stderr, "--video %s: %s\n", g.c_str(), why.c_str()); return 1; }
-    }
-    std::vector<Worker> workers(devices.size());
+    if (const int rc = open_given_clips(o, scene, given_clips)) return rc;
+    std::vector<Worker> workers(o.devices.size());
     for (size_t w = 0; w < workers.size(); w++) {    // every device is opened before any work
-        workers[w].ctx = pe_create(devices[w]);
+        workers[w].ctx = pe_create(o.devices[w]);
         if (!workers[w].ctx) { std::fprintf(stderr, "pe_create: %s\n", pe_last_error(nullptr)); return 1; }
         workers[w].scene = w == 0 ? scene : ph_scene_load_ron(text.data(), text.size(), err, sizeof err);
     }
-    // Everything up to the first frame, for one worker.  Only the first reports what it finds (textures, videos): the others
-    // find the same.
-    std::map<std::string, DecodedPng> decoded;
-    std::set<std::string> given_video_names;
-    for (auto& kv : given_clips) given_video_names.insert(kv.first);
-    auto set_up = [&](Worker& wk, bool first) -> int {
-        pe_ctx* ctx = wk.ctx;
-        ph_scene* sc = wk.scene;
-        ph_player* player = wk.player = ph_player_new(sc);
-        if (adaptive) ph_player_set_adaptive_aa(player, 1, adaptive_threshold);
-        if (frame_cmd) {  // main.rs:2900-2926
-            if (!stage.empty() && ph_player_init_stage(player, stage.c_str())) {
-                std::fprintf(stderr, "Scene `%s` has no stage named `%s`\n", scene_path.c_str(), stage.c_str());
-                return 1;
-            }
-            if (!animation.empty() && ph_player_init_animation(player, animation.c_str())) {
-                std::fprintf(stderr, "Scene `%s` has no animation named `%s`\n", scene_path.c_str(), animation.c_str());
-                return 1;
-            }
-            if (!camera.empty() && ph_player_select_camera(player, camera.c_str())) {
-                std::fprintf(stderr, "Scene `%s` has no camera named `%s`\n", scene_path.c_str(), camera.c_str());
-                return 1;
-            }
-        }
-        if (ph_scene_build_program(sc, ctx) || ph_scene_upload_uniforms(sc, ctx)) {
-            std::fprintf(stderr, "%s\n", ph_scene_last_error(sc));
-            return 1;
-        }
-        std::map<std::string, bool> given;
-        for (const std::string& t : textures) {  // name=file.png | name=file.rgba:WxH
-            size_t eq = t.find('='), colon = t.rfind(':'), x = t.rfind('x');
-            if (eq != std::string::npos && ends_with(t, ".png")) {
-                std::string why;
-                if (!set_texture_decoded(ctx, t.substr(0, eq), decode_png_once(decoded, t.substr(eq + 1)), why)) { std::fprintf(stderr, "texture %s: %s\n", t.c_str(), why.c_str()); return 1; }
-                given[t.substr(0, eq)] = true;
-                continue;
-            }
-            if (eq == std::string::npos || colon == std::string::npos || x == std::string::npos || x < colon) { std::fprintf(stderr, "bad --texture %s\n", t.c_str()); return 2; }
-            given[t.substr(0, eq)] = true;
-            int tw = std::atoi(t.substr(colon + 1, x - colon - 1).c_str()), th = std::atoi(t.substr(x + 1).c_str());
-            bool tok = false;
-            std::string bytes = slurp(t.substr(eq + 1, colon - eq - 1), tok);
-            if (!tok || bytes.size() != size_t(tw) * size_t(th) * 4) { std::fprintf(stderr, "texture %s: cannot read / wrong size\n", t.c_str()); return 1; }
-            if (pe_set_texture(ctx, t.substr(0, eq).c_str(), reinterpret_cast<const uint8_t*>(bytes.data()), tw, th)) { std::fprintf(stderr, "%s\n", pe_last_error(ctx)); return 1; }
-        }
-        // reload_textures (main.rs:1066-1085): every texture of the scene from its stored path; a failure is reported, the render goes on
-        for (int k = 0;; k++) {
-            const char *name = nullptr, *path = nullptr;
-            if (ph_scene_texture(sc, k, &name, &path)) break;
-            if (given.count(name)) continue;
-            const std::string file = assets.empty() || (path[0] == '/') ? std::string(path) : assets + "/" + path;
-            std::string why;
-            if (!set_texture_decoded(ctx, name, decode_png_once(decoded, file), why) && first)
-                std::fprintf(stderr, "texture `%s`: %s (the sampler stays unbound)\n", name, why.c_str());
-        }
-        if (pe_scene_compile(ctx)) { std::fprintf(stderr, "%s\n", pe_last_error(ctx)); return 1; }
-        ph_player_attach(player, ctx);  // camera teleportation goes through pe_probe_ray
-        // VideoRuntime::from_scene (main.rs:820-858): videos that have a path, a uniform and frames on disk
-        VideoState& video_state = wk.video_state;
-        video_state.scene = sc;
-        video_state.ctx = ctx;
-        for (int k = 0;; k++) {
-            const char *name = nullptr, *path = nullptr, *uniform = nullptr;
-            if (ph_scene_video(sc, k, &name, &path, &uniform)) break;
-            if (!path[0] || !uniform[0]) continue;
-            VideoRuntime v;
-            std::string source;
-            auto it = given_clips.find(name);
-            if (given_video_names.count(name)) {                             // --video
-                const std::string given_path = videos_path_of(videos, name);
-                std::string why;
-                if (first && it != given_clips.end()) {
-                    v = it->second;
-                    given_clips.erase(it);
-                } else if (!open_clip(v, given_path, video_matrix, why, true)) {  // each worker reads with a handle of its own
-                    std::fprintf(stderr, "--video %s=%s: %s\n", name, given_path.c_str(), why.c_str());
-                    return 1;
-                }
-                source = clip_description(given_path, v);
-            } else if (!(v.frames = video_frame_files(assets, path)).empty()) {   // video_png/<stem>/
-                source = std::to_string(v.frames.size()) + " PNG frames in " + v.frames[0].substr(0, v.frames[0].rfind('/'));
-            } else {                                                         // <assets>/video_y4m/<stem>.y4m
-                char rel[1024];
-                const int n = ph_video_frames_dir(path, rel, sizeof rel);
-                const std::string stem = n > 0 ? std::string(rel).substr(std::string(rel).find('/') + 1) : std::string();
-                const std::string clip = (assets.empty() ? std::string() : assets + "/") + "video_y4m/" + stem + ".y4m";
-                std::string why;
-                if (stem.empty() || !file_exists(clip)) continue;
-                if (!open_clip(v, clip, video_matrix, why, !first)) {
-                    if (first) std::fprintf(stderr, "video `%s`: %s (the sampler is not updated)\n", name, why.c_str());
-                    continue;
-                }
-                source = clip_description(clip, v);
-            }
-            v.video = k;
-            v.name = name;
-            if (v.clip && pe_host_malloc(ctx, v.planes_bytes, &v.planes)) { std::fprintf(stderr, "%s\n", pe_last_error(ctx)); return 1; }
-            if (first) std::fprintf(status, "video `%s`: %s\n", name, source.c_str());
-            video_state.videos.push_back(v);
-        }
-        if (first)
-            for (auto& kv : given_clips) ph_y4m_close(kv.second.clip);   // a video without a path or a uniform plays nothing
-        if (!video_state.videos.empty()) ph_player_set_update_hook(player, update_videos, &video_state);
-        if (stereo) ph_player_set_stereo(player, 1, 0.07, 0);         // `render --stereo-image` (main.rs:2809-2816, 2842)
-        return 0;
-    };
+    std::map<std::string, DecodedPng> decoded;       // the scene's textures, decoded once for every worker
     for (size_t w = 0; w < workers.size(); w++) {
-        if (!workers[w].scene) { std::fprintf(stderr, "Failed to parse scene `%s`: %s\n", scene_path.c_str(), err); return 1; }
-        if (const int rc = set_up(workers[w], w == 0)) return rc;
+        if (!workers[w].scene) { std::fprintf(stderr, "Failed to parse scene `%s`: %s\n", o.scene_path.c_str(), err); return 1; }
+        if (const int rc = set_up(o, workers[w], w == 0, decoded, given_clips)) return rc;
     }
-    if (stereo) width *= 2;         // side-by-side eyes, doubled width
-    // one buffer per worker for the frame (`render` to a stream: two, which travel to the main thread and back)
-    const size_t frame_bytes = ph_output_bytes(fmt.container, fmt.bits, width, height);
-    if (!frame_bytes) {
-        static const char* const what[] = {"image", "PNG", "Y4M stream", "GIF frame"};
-        std::fprintf(stderr, "no %s for a %d x %d frame\n", what[fmt.container], width, height);
-        return 1;
-    }
-    for (Worker& wk : workers) {
-        if (stream) wk.free_planes.assign(2, std::vector<uint8_t>(frame_bytes));
-        else wk.px.resize(frame_bytes);
-    }
-    ph_frame_params p = {width, height, depth, aa, 0, 0, {0, 0, 0}, 0, 0, 0};
-    int exit_code = 0;
-    if (frame_cmd) {
-        Worker& wk = workers[0];
-        if (ph_player_update(wk.player, time) ||                                                          // main.rs:2928-2929
-            ph_player_render(wk.player, wk.ctx, &p, nullptr, fmt.container, fmt.bits, wk.px.data(), wk.px.size(), &wk.len)) {
-            std::fprintf(stderr, "%s\n", ph_player_last_error(wk.player));
-            return 1;
-        }
-        if (!write_frame(output, fmt, wk.px, wk.len, width, height)) { std::fprintf(stderr, "cannot write %s\n", output.c_str()); return 1; }
-        std::printf("Rendered `%s` to `%s`\n", scene_path.c_str(), output.c_str());
-    } else {
-        // The plan: every skip decision from one snapshot of the output, taken now, plus what the animations before each one
-        // will write (a name listed twice), so that the decisions are the sequential loop's and no worker's write can change
-        // another's
-        std::vector<AnimationPlan> plan(names.size());
-        std::set<std::string> to_write;
-        for (size_t k = 0; k < names.size(); k++) {
-            AnimationPlan& a = plan[k];
-            for (int i = 0; i < ph_scene_animation_count(scene); i++) {
-                const char* nm = nullptr;
-                double d = 0.0;
-                if (ph_scene_animation(scene, i, &nm, &d) == 0 && names[k] == nm) a.duration = d;
-            }
-            a.rendered = !(all && !starts_with.empty() && names[k].compare(0, starts_with.size(), starts_with) != 0);
-            const float duration32 = float(a.duration);                                        // render_animation takes f32
-            a.duration = double(duration32);
-            a.count = int(duration32 * float(fps));                                             // main.rs:1785
-            if (a.count < 1) a.count = 1;
-            a.todo = max_frames >= 0 && max_frames < a.count ? max_frames : a.count;
-            a.skip_frame.assign(size_t(a.todo), 0);
-            if (!a.rendered || to_stdout) continue;
-            if (stream) {
-                const std::string file = out_dir + "/" + names[k] + stream_ext;
-                a.skip_stream = skip_existing && (file_exists(file) || to_write.count(file));         // main.rs:1771-1779
-                if (!a.skip_stream) to_write.insert(file);
-                continue;
-            }
-            for (int i = 0; i < a.todo; i++) {
-                const std::string f = out_dir + "/" + names[k] + "/frame_" + std::to_string(i) + frame_ext;
-                a.skip_frame[size_t(i)] = skip_existing && (file_exists(f) || to_write.count(f));   // resumes like main.rs:1789-1793
-                if (!a.skip_frame[size_t(i)]) to_write.insert(f);
-            }
-        }
-        Shared sh;
-        // A worker runs the whole loop.  It renders frame i of an animation when i mod N is its number and advances through
-        // the others, so its player's state at every frame is the sequential one (camera teleportation carries over).
-        auto run_worker = [&](size_t me) {
-            Worker& wk = workers[me];
-            for (size_t k = 0; k < names.size(); k++) {
-                if (sh.stopped()) return;
-                if (ph_player_init_animation(wk.player, names[k].c_str())) {
-                    sh.fail("Scene `" + scene_path + "` has no animation named `" + names[k] + "`");
-                    return;
-                }
-                if (ph_player_update(wk.player, 0.0)) { sh.fail(ph_player_last_error(wk.player)); return; }
-                const AnimationPlan& a = plan[k];
-                if (!a.rendered) continue;
-                if (me == 0) sh.post(k, -1, {});
-                if (stream && a.skip_stream) continue;
-                const std::string dir = out_dir + "/" + names[k];
-                if (!stream && !make_dirs(dir)) { sh.fail("cannot create " + dir); return; }
-                for (int i = 0; i < a.todo; i++) {
-                    if (sh.stopped()) return;
-                    if (a.skip_frame[size_t(i)]) continue;                 // neither rendered nor advanced, as the sequential loop
-                    if (size_t(i) % workers.size() != me) {
-                        if (ph_player_advance_motion_blur_frame(wk.player, i, a.count, motion_blur, a.duration)) { sh.fail(ph_player_last_error(wk.player)); return; }
-                        continue;
-                    }
-                    std::vector<uint8_t> planes;                           // a stream: the frame goes to the main thread
-                    if (stream && !sh.take_buffer(wk, planes)) return;
-                    if (stream) planes.resize(frame_bytes);                // a GIF block came back cut to its length
-                    std::vector<uint8_t>& buf = stream ? planes : wk.px;
-                    const ph_motion_blur mb = {i, a.count, motion_blur, a.duration};
-                    if ((fmt.file == GIF && ph_player_set_gif_delay(wk.player, gif_delay(i, fps))) ||
-                        ph_player_render(wk.player, wk.ctx, &p, &mb, fmt.container, fmt.bits, buf.data(), buf.size(), &wk.len)) {
-                        sh.fail(ph_player_last_error(wk.player));
-                        return;
-                    }
-                    if (fmt.file == GIF) planes.resize(wk.len);
-                    if (!stream) {
-                        const std::string name = dir + "/frame_" + std::to_string(i) + frame_ext;
-                        if (!write_frame(name, fmt, wk.px, wk.len, width, height)) { sh.fail("cannot write " + name); return; }
-                    }
-                    sh.post(k, i, std::move(planes));
-                }
-            }
-        };
-        std::vector<std::thread> threads;
-        for (size_t w = 0; w < workers.size(); w++) threads.emplace_back(run_worker, w);
-        // The main thread: status lines and Y4M / GIF streams, in frame order
-        std::vector<uint8_t> planes;
-        for (size_t k = 0; k < names.size(); k++) {
-            const AnimationPlan& a = plan[k];
-            if (!a.rendered) continue;
-            if (!sh.take(k, -1, planes)) break;
-            std::fprintf(status, "Rendering animation %s, %zu/%zu\n", names[k].c_str(), k + 1, names.size());
-            bool stopped = false;
-            if (stream) {
-                // one stream per animation, written under a temporary name and renamed when complete, so that an interrupted
-                // run leaves no stream for skip-existing to take as done
-                const std::string file = out_dir + "/" + names[k] + stream_ext, part = file + ".part";
-                if (a.skip_stream) {
-                    std::fprintf(status, "Skip `%s`, because it's already exists\n", names[k].c_str());
-                    continue;
-                }
-                if (!to_stdout && !make_dirs(out_dir)) { sh.fail("cannot create " + out_dir); break; }
-                FILE* f = to_stdout ? stdout : std::fopen(part.c_str(), "wb");
-                bool ok_stream = f && (fmt.file == GIF ? write_gif_header(f, width, height, true) : write_y4m_header(f, width, height, fps));
-                for (int i = 0; i < a.todo && ok_stream; i++) {
-                    if (!sh.take(k, i, planes)) { stopped = true; break; }
-                    ok_stream = fmt.file == GIF ? write_gif_block(f, planes) : write_y4m_frame(f, planes);
-                    sh.give_back(workers[size_t(i) % workers.size()], planes);
-                    std::fprintf(status, "\r%d/%d done      ", i + 1, a.count);
-                    std::fflush(status);
-                }
-                if (ok_stream && !stopped && fmt.file == GIF) ok_stream = write_gif_trailer(f);
-                if (f) ok_stream = (to_stdout ? std::fflush(f) : std::fclose(f)) == 0 && ok_stream;
-                if (stopped) break;                                        // the stream keeps its .part name
-                if (!ok_stream || (!to_stdout && std::rename(part.c_str(), file.c_str()) != 0)) {
-                    sh.fail(std::string("cannot write ") + (to_stdout ? "the stream to stdout" : file.c_str()));
-                    break;
-                }
-                std::fprintf(status, "\n");
-                continue;
-            }
-            for (int i = 0; i < a.todo && !stopped; i++) {
-                if (a.skip_frame[size_t(i)]) continue;
-                if (!sh.take(k, i, planes)) { stopped = true; break; }
-                std::fprintf(status, "\r%d/%d done      ", i + 1, a.count);
-                std::fflush(status);
-            }
-            if (stopped) break;
-            std::fprintf(status, "\n");
-        }
-        for (std::thread& t : threads) t.join();
-        if (sh.stop) {
-            std::fprintf(stderr, "%s\n", sh.error.c_str());
-            exit_code = 1;
-        }
-    }
-    for (Worker& wk : workers) {
-        for (VideoRuntime& v : wk.video_state.videos) {
-            if (v.planes) pe_host_free(wk.ctx, v.planes);
-            ph_y4m_close(v.clip);
-        }
-        ph_player_free(wk.player);
-        pe_destroy(wk.ctx);
-        ph_scene_free(wk.scene);
-    }
-    return exit_code;
+    const int width = o.stereo ? 2 * o.width : o.width;      // side-by-side eyes, doubled width
+    const size_t frame_bytes = ph_output_bytes(o.fmt.container, o.fmt.bits, width, o.height);
+    if (!frame_bytes) { std::fprintf(stderr, "no %s for a %d x %d frame\n", o.fmt.what, width, o.height); return 1; }
+    const ph_frame_params p = {width, o.height, o.depth, o.aa, 0, 0, {0, 0, 0}, 0, 0, 0};
+    return o.frame_cmd ? render_frame(o, workers[0], p, frame_bytes) : render_animations(o, scene, names, workers, p, frame_bytes);
 }
-
