@@ -365,6 +365,25 @@ PE_API int pe_encode_gif_frame_host(pe_ctx* ctx, const void* rgba8_device, int w
  * below that length.  The file ends with the trailer, the single byte 0x3B, after the last frame block. */
 PE_API int pe_gif_header(int width, int height, int loop, uint8_t* out, size_t capacity);
 
+/* ---- JPEG files encoded on the device (no counterpart in the reference) ---------------------------------------------------
+ * DESIGN.md section 5.7, restated sequentially in tests/host_harness/jpeg_spec.cpp.  One file is a pure function of the RGBA8
+ * frame (alpha ignored) and the quality (1 .. 100): baseline sequential JFIF, Y'CbCr 4:2:0 (JFIF / BT.601 full range, the frame
+ * padded to a multiple of 16 by repeating its last column and row, chroma averaged over 2 x 2), the quantisation tables of
+ * T.81 Annex K.1 scaled by the IJG quality rule, an integer FDCT, Huffman tables optimised for the frame (T.81 Annex K.2) and
+ * one restart interval per MCU row.  The bytes do not depend on the GPU, the stream or scheduling.  The work space is the
+ * context's own (never a pe_scratch_buffer slot); one context encodes on one stream at a time. */
+/* Upper bound of the file for a width x height frame; 0 unless 1 <= width, height <= 65535. */
+PE_API size_t pe_jpeg_bound(int width, int height);
+/* JPEG file of a row-major RGBA8 frame in device memory (4-byte aligned), encoded on the device.  Asynchronous on `stream`
+ * (NULL: the context's stream): a memset and eight kernel launches.  Writes the file into jpeg_device (capacity >=
+ * pe_jpeg_bound) and its length into *size_device (uint64).  A bad size, alignment, capacity, a quality outside 1 .. 100 or a
+ * context without a device are refused before any launch.  The frame is only read. */
+PE_API int pe_encode_jpeg_rgba8(pe_ctx* ctx, const void* rgba8_device, int width, int height, int quality, void* jpeg_device,
+                                size_t capacity, void* size_device, void* stream);
+/* Synchronous form on the context's stream: the file lands in host memory; *size_out = its length. */
+PE_API int pe_encode_jpeg_host(pe_ctx* ctx, const void* rgba8_device, int width, int height, int quality, uint8_t* jpeg_host,
+                               size_t capacity, size_t* size_out);
+
 /* ---- 16 bits per channel (opt-in; no counterpart in the reference, whose frames are 8-bit) ---------------------------------
  * For a 10-bit video encode: the float frame of pe_render (or pe_render_adaptive with rgba8 = 0) quantised to unorm16 instead
  * of unorm8.  An RGBA16 pixel is four uint16 (r, g, b, a) in host byte order, 8 B.  Same argument rules as the RGBA8 forms. */

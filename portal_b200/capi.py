@@ -36,7 +36,7 @@ class PhMotionBlur(C.Structure):
                 ("duration_seconds", C.c_double)]
 
 
-PH_OUT_PIXELS, PH_OUT_PNG, PH_OUT_YUV420P10, PH_OUT_GIF = 0, 1, 2, 3
+PH_OUT_PIXELS, PH_OUT_PNG, PH_OUT_YUV420P10, PH_OUT_GIF, PH_OUT_JPEG = 0, 1, 2, 3, 4
 
 PE_YUV_BT709, PE_YUV_BT601 = 0, 1
 PE_YUV_SITING_LEFT, PE_YUV_SITING_CENTER = 0, 1
@@ -147,6 +147,9 @@ def lib() -> C.CDLL:
         "pe_encode_gif_frame": (i32, [vp, vp, i32, i32, i32, vp, C.c_size_t, vp, vp]),
         "pe_encode_gif_frame_host": (i32, [vp, vp, i32, i32, i32, vp, C.c_size_t, C.POINTER(C.c_size_t)]),
         "pe_gif_header": (i32, [i32, i32, i32, vp, C.c_size_t]),
+        "pe_jpeg_bound": (C.c_size_t, [i32, i32]),
+        "pe_encode_jpeg_rgba8": (i32, [vp, vp, i32, i32, i32, vp, C.c_size_t, vp, vp]),
+        "pe_encode_jpeg_host": (i32, [vp, vp, i32, i32, i32, vp, C.c_size_t, C.POINTER(C.c_size_t)]),
         "pe_yuv420p10_bytes": (C.c_size_t, [i32, i32]),
         "pe_rgba_to_yuv420p10": (i32, [vp, vp, i32, i32, i32, vp, vp]),
         "pe_yuv420_bytes": (C.c_size_t, [i32, i32, i32]),
@@ -222,6 +225,7 @@ def lib() -> C.CDLL:
         "ph_player_advance_motion_blur_frame": (i32, [vp, i32, i32, i32, C.c_double]),
         "ph_player_set_adaptive_aa": (i32, [vp, i32, i32]),
         "ph_player_set_gif_delay": (i32, [vp, i32]),
+        "ph_player_set_jpeg_quality": (i32, [vp, i32]),
         "ph_y4m_open": (vp, [cp, i32, cp, C.c_size_t]),
         "ph_y4m_info": (i32, [vp, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(PeYuvFormat),
                               C.POINTER(C.c_int64)]),
@@ -277,21 +281,32 @@ def encode_gif_frame(ctx, rgba8, delay_cs: int = 0) -> bytes:
     """GIF frame block (DESIGN.md section 5.6) of a CUDA uint8 tensor [h, w, 4] (contiguous) encoded on the device by
     pe_encode_gif_frame on context `ctx`, ordered after the work already queued on the current torch stream.  A file is
     gif_header(w, h, loop) + the blocks + b"\\x3b"."""
+    return _encode_on_stream(ctx, rgba8, "GIF frame", "pe_gif_frame_bound", "pe_encode_gif_frame", int(delay_cs))
+
+
+def encode_jpeg(ctx, rgba8, quality: int = 90) -> bytes:
+    """JPEG file (DESIGN.md section 5.7) of a CUDA uint8 tensor [h, w, 4] (contiguous; alpha ignored) at `quality` 1 .. 100,
+    encoded on the device by pe_encode_jpeg_rgba8 on context `ctx`, ordered after the work already queued on the current torch
+    stream."""
+    return _encode_on_stream(ctx, rgba8, "JPEG", "pe_jpeg_bound", "pe_encode_jpeg_rgba8", int(quality))
+
+
+def _encode_on_stream(ctx, rgba8, what: str, bound: str, encode: str, arg: int) -> bytes:
     import torch
     if rgba8.dim() != 3 or rgba8.shape[2] != 4 or not rgba8.is_cuda or rgba8.dtype != torch.uint8 or not rgba8.is_contiguous():
         raise ValueError("frame must be a contiguous CUDA uint8 tensor [h, w, 4]")
     L = lib()
     h, w = int(rgba8.shape[0]), int(rgba8.shape[1])
-    cap = L.pe_gif_frame_bound(w, h)
+    cap = getattr(L, bound)(w, h)
     if cap == 0:
-        raise PortalB200Error(f"pe_gif_frame_bound: no GIF frame for a {w} x {h} frame")
+        raise PortalB200Error(f"{bound}: no {what} for a {w} x {h} frame")
     out = torch.empty(cap, dtype=torch.uint8, device=rgba8.device)
     size = torch.empty(1, dtype=torch.int64, device=rgba8.device)
     # the read-backs go on the same stream handle (0, torch's default stream, names the context's stream)
     stream = C.c_void_p(torch.cuda.current_stream(rgba8.device).cuda_stream)
     n = C.c_uint64()
-    if (L.pe_encode_gif_frame(ctx, C.c_void_p(rgba8.data_ptr()), w, h, int(delay_cs), C.c_void_p(out.data_ptr()), cap,
-                              C.c_void_p(size.data_ptr()), stream)
+    if (getattr(L, encode)(ctx, C.c_void_p(rgba8.data_ptr()), w, h, arg, C.c_void_p(out.data_ptr()), cap,
+                           C.c_void_p(size.data_ptr()), stream)
             or L.pe_memcpy_d2h(ctx, C.addressof(n), C.c_void_p(size.data_ptr()), 8, stream)):
         raise PortalB200Error(L.pe_last_error(ctx).decode(errors="replace"))
     host = (C.c_uint8 * max(1, n.value))()

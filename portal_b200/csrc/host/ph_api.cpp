@@ -30,6 +30,7 @@ struct ph_player {
     void* hook_user = nullptr;
     bool adaptive_aa = false;           // ph_player_set_adaptive_aa: frames go through pe_render_adaptive
     int gif_delay = 0;                  // ph_player_set_gif_delay: the GCE delay of PH_OUT_GIF blocks, centiseconds
+    int jpeg_quality = 90;              // ph_player_set_jpeg_quality: the quality of PH_OUT_JPEG files
     int adaptive_threshold = 8;
     explicit ph_player(ph_scene* sc) : s(sc), player(sc->scene) {}
 };
@@ -624,6 +625,13 @@ int ph_player_set_gif_delay(ph_player* pl, int delay_cs) {
     return 0;
 }
 
+int ph_player_set_jpeg_quality(ph_player* pl, int quality) {
+    if (!pl) return 1;
+    if (quality < 1 || quality > 100) return pfail(pl, "ph_player_set_jpeg_quality: quality " + std::to_string(quality) + " is outside 1 .. 100");
+    pl->jpeg_quality = quality;
+    return 0;
+}
+
 int ph_player_advance_motion_blur_frame(ph_player* pl, int frame_index, int frame_count, int motion_blur_frames, double duration_seconds) {
     if (!pl) return 1;
     std::vector<double> times;
@@ -642,6 +650,7 @@ size_t ph_output_bytes(int container, int bits, int width, int height) {
         case PH_OUT_PNG: return bits == 8 ? pe_png_bound(width, height) : bits == 16 ? pe_png_bound_rgba16(width, height) : 0;
         case PH_OUT_YUV420P10: return bits == 8 || bits == 16 ? pe_yuv420p10_bytes(width, height) : 0;
         case PH_OUT_GIF: return bits == 8 ? pe_gif_frame_bound(width, height) : 0;
+        case PH_OUT_JPEG: return bits == 8 ? pe_jpeg_bound(width, height) : 0;
     }
     return 0;
 }
@@ -650,9 +659,11 @@ size_t ph_output_bytes(int container, int bits, int width, int height) {
 int ph_player_render(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, const ph_motion_blur* mb, int container, int bits,
                      void* out_host, size_t capacity, size_t* len) {
     if (!pl || !ctx || !p || !out_host || !len) return 1;
-    if (container != PH_OUT_PIXELS && container != PH_OUT_PNG && container != PH_OUT_YUV420P10 && container != PH_OUT_GIF)
+    if (container != PH_OUT_PIXELS && container != PH_OUT_PNG && container != PH_OUT_YUV420P10 && container != PH_OUT_GIF &&
+        container != PH_OUT_JPEG)
         return pfail(pl, "ph_player_render: unknown container " + std::to_string(container));
     if (container == PH_OUT_GIF && bits != 8) return pfail(pl, "ph_player_render: GIF frames are 8-bit (bits must be 8)");
+    if (container == PH_OUT_JPEG && bits != 8) return pfail(pl, "ph_player_render: JPEG frames are 8-bit (bits must be 8)");
     if (container != PH_OUT_PIXELS && bits != 8 && bits != 16) return pfail(pl, "ph_player_render: bits must be 8 or 16 for PNG and Y'CbCr");
     if (bits != 8 && bits != 16 && bits != 32) return pfail(pl, "ph_player_render: bits must be 8, 16 or 32");
     if (bits == 32 && mb) return pfail(pl, "ph_player_render: motion blur needs bits 8 or 16 (its sub-frames are averaged as integers)");
@@ -692,6 +703,11 @@ int ph_player_render(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, const
     if (container == PH_OUT_GIF) {
         if (pe_encode_gif_frame_host(ctx, frame, p->width, p->height, pl->gif_delay, static_cast<uint8_t*>(out_host), capacity, len))
             return pfail(pl, std::string("GIF encoding failed: ") + pe_last_error(ctx));
+        return 0;
+    }
+    if (container == PH_OUT_JPEG) {
+        if (pe_encode_jpeg_host(ctx, frame, p->width, p->height, pl->jpeg_quality, static_cast<uint8_t*>(out_host), capacity, len))
+            return pfail(pl, std::string("JPEG encoding failed: ") + pe_last_error(ctx));
         return 0;
     }
     if (container == PH_OUT_YUV420P10) {

@@ -4,11 +4,12 @@
 //   portal_b200_render render-frame <scene.ron> [--width W] [--height H] [--render-depth D] [--aa-count N]
 //                      [--time T] [--stage NAME] [--animation NAME] [--camera NAME] [--device K]
 //                      [--texture name=file.png | name=file.rgba:WxH ...] [--assets DIR] [--output out.png|.ppm|.rgba]
-//                      [--adaptive-aa T] [--bit-depth 8|16]                   (also --output out.y4m | out.gif)
+//                      [--adaptive-aa T] [--bit-depth 8|16]                   (also --output out.y4m | out.gif | out.jpg)
+//                      [--jpeg-quality Q]
 //                      [--video name=clip.y4m ...] [--video-matrix bt709|bt601]
 //   portal_b200_render render <scene.ron> [--animations a,b,... | --starts-with PREFIX] [--fps N] [--motion-blur-frames M] [--width W]
 //                      [--height H] [--render-depth D] [--aa-count N] [--stereo-image] [--no-skip-existing] [--out-dir DIR] [--max-frames K]
-//                      [--frame-format ppm|png|rgba|y4m|gif] [--assets DIR] [--adaptive-aa T] [--bit-depth 8|16]
+//                      [--frame-format ppm|png|rgba|y4m|gif|jpg] [--jpeg-quality Q] [--assets DIR] [--adaptive-aa T] [--bit-depth 8|16]
 //                      [--video name=clip.y4m ...] [--video-matrix bt709|bt601]
 //                      (`portal render`, main.rs:2808-2873 -> render_named_animations :1876-1930 ->
 //                       render_animation :1757-1830; frames are written as DIR/<animation>/frame_<i>.<format>, or as one
@@ -39,6 +40,12 @@
 // (halves up), so that n frames last round(100 n / fps) cs; --fps above 50 is refused, as browsers show a delay below 2 cs
 // as 10 cs.  render-frame writes a one-frame file without the loop block, delay 0.  GIF is 8-bit: --bit-depth 16 is refused,
 // and so is a frame wider or taller than 65535 pixels.
+//
+// --frame-format jpg / --output *.jpg or *.jpeg (not in the reference): every RGBA8 frame encoded on the device into a
+// baseline JPEG file (pe_encode_jpeg_rgba8; DESIGN.md section 5.7: Y'CbCr 4:2:0, Huffman tables optimised per frame, one
+// restart interval per MCU row) at --jpeg-quality Q (1 .. 100, 90 by default).  A JPEG is a frame file like a PNG:
+// render-frame writes one, `render` writes DIR/<animation>/frame_<i>.jpg.  JPEG is 8-bit: --bit-depth 16 is refused, and so
+// are a frame wider or taller than 65535 pixels and --jpeg-quality with any other format.
 //
 // Output: the RGBA8 frame the reference hands to export_png (main.rs:2939-2943) as a PNG when the name ends in .png (encoded
 // on the device: pe_encode_png_rgba8), as raw RGBA8 for .rgba, else as a binary PPM (P6, alpha dropped).  Every format is one
@@ -113,6 +120,7 @@ static FrameFormat frame_format(const std::string& ext, int bits) {
     if (ext == ".png") return {AS_RETURNED, PH_OUT_PNG, bits, ext, "PNG", "PNG"};   // Image::export_png (main.rs:2939-2943)
     if (ext == ".y4m") return {Y4M, PH_OUT_YUV420P10, bits, ext, "Y4M", "Y4M stream"};
     if (ext == ".gif") return {GIF, PH_OUT_GIF, bits, ext, "GIF", "GIF frame"};
+    if (ext == ".jpg" || ext == ".jpeg") return {AS_RETURNED, PH_OUT_JPEG, bits, ext, "JPEG", "JPEG"};
     return {ends_with(ext, ".rgba") ? AS_RETURNED : PPM, PH_OUT_PIXELS, bits, ext, "image", "image"};
 }
 
@@ -318,6 +326,7 @@ struct Options {
     int width = 0, height = 0, depth = 0, aa = 0, fps = 60, motion_blur = 1, max_frames = -1;
     bool stereo = false, skip_existing = true, adaptive = false;
     int adaptive_threshold = 0, bits = 8, video_matrix = PE_YUV_BT709;
+    int jpeg_quality = 90;                   // --jpeg-quality
     double time = 0.0;
     std::vector<std::string> textures, videos, animations;
     std::string stage, animation, camera, starts_with, assets;
@@ -334,16 +343,16 @@ static int parse_options(int argc, char** argv, Options& o) {
     const bool anim_cmd = argc >= 3 && std::strcmp(argv[1], "render") == 0;
     if (!o.frame_cmd && !anim_cmd) {
         std::fprintf(stderr, "usage: %s render-frame <scene.ron> [--width W] [--height H] [--render-depth D] [--aa-count N] [--time T] "
-                             "[--stage NAME] [--animation NAME] [--camera NAME] [--device K] [--texture name=file.png|name=file.rgba:WxH] [--assets DIR] [--output out.png|.ppm|.rgba|.y4m|.gif] [--adaptive-aa T] [--bit-depth 8|16] [--video name=clip.y4m] [--video-matrix bt709|bt601]\n"
+                             "[--stage NAME] [--animation NAME] [--camera NAME] [--device K] [--texture name=file.png|name=file.rgba:WxH] [--assets DIR] [--output out.png|.ppm|.rgba|.y4m|.gif|.jpg] [--jpeg-quality Q] [--adaptive-aa T] [--bit-depth 8|16] [--video name=clip.y4m] [--video-matrix bt709|bt601]\n"
                              "       %s render <scene.ron> [a,b | --animations a,b | --starts-with PREFIX] [--fps N] [--motion-blur-frames M] [--width W] [--height H] "
-                             "[--render-depth D] [--aa-count N] [--stereo-image] [--no-skip-existing] [--out-dir DIR] [--max-frames K] [--frame-format ppm|png|rgba|y4m|gif] [--adaptive-aa T] [--bit-depth 8|16] [--video name=clip.y4m] [--video-matrix bt709|bt601] [--device K | --devices K,K,...]\n", argv[0], argv[0]);
+                             "[--render-depth D] [--aa-count N] [--stereo-image] [--no-skip-existing] [--out-dir DIR] [--max-frames K] [--frame-format ppm|png|rgba|y4m|gif|jpg] [--jpeg-quality Q] [--adaptive-aa T] [--bit-depth 8|16] [--video name=clip.y4m] [--video-matrix bt709|bt601] [--device K | --devices K,K,...]\n", argv[0], argv[0]);
         return 2;
     }
     o.scene_path = argv[2];
     // defaults of RenderFrameCliOptions (main.rs:2744-2754) / RenderCliOptions (main.rs:2764-2803)
     o.width = o.frame_cmd ? 1920 : 3840, o.height = o.frame_cmd ? 1080 : 2160, o.depth = o.frame_cmd ? 100 : 150, o.aa = o.frame_cmd ? 1 : 4;
     int device = 0, first_option = 3;
-    bool device_given = false, devices_given = false;
+    bool device_given = false, devices_given = false, quality_given = false;
     std::string frame_ext = ".ppm", devices_list, animations;
     if (anim_cmd && argc > 3 && std::strncmp(argv[3], "--", 2) != 0) animations = argv[first_option++];   // `render <scene> [animations]`
     for (int i = first_option; i < argc; i++) {
@@ -376,7 +385,15 @@ static int parse_options(int argc, char** argv, Options& o) {
             o.video_matrix = v == "bt601" ? PE_YUV_BT601 : PE_YUV_BT709;
         }
         else if (a == "--assets") o.assets = next();
-        else if (a == "--frame-format") frame_ext = std::string(".") + next();          // render: ppm (default) | png | rgba | y4m | gif
+        else if (a == "--frame-format") frame_ext = std::string(".") + next();          // render: ppm (default) | png | rgba | y4m | gif | jpg
+        else if (a == "--jpeg-quality" || a == "--jpeg_quality") {
+            const char* v = next();
+            char* end = nullptr;
+            const long q = std::strtol(v, &end, 10);
+            if (!*v || *end || q < 1 || q > 100) { std::fprintf(stderr, "--jpeg-quality must be an integer in 1 .. 100, got `%s`\n", v); return 2; }
+            o.jpeg_quality = int(q);
+            quality_given = true;
+        }
         else if (a == "--adaptive-aa" || a == "--adaptive_aa") {
             const char* v = next();
             char* end = nullptr;
@@ -404,6 +421,7 @@ static int parse_options(int argc, char** argv, Options& o) {
     o.all_animations = animations.empty();
     const size_t dot = o.output.rfind('.');   // the frame's format: from the output's name (render-frame) or --frame-format (render)
     o.fmt = frame_format(!o.frame_cmd ? frame_ext : dot == std::string::npos ? std::string() : o.output.substr(dot), o.bits);
+    if (quality_given && o.fmt.container != PH_OUT_JPEG) { std::fprintf(stderr, "--jpeg-quality applies to JPEG frames only (.jpg / .jpeg)\n"); return 2; }
     o.to_stdout = anim_cmd && o.fmt.stream() && o.out_dir == "-";
     o.status = o.to_stdout ? stderr : stdout;
     return 0;
@@ -437,18 +455,24 @@ static bool is_rendered(const Options& o, const std::string& name) {
     return !o.all_animations || o.starts_with.empty() || name.compare(0, o.starts_with.size(), o.starts_with) == 0;
 }
 
-// The refusals that need the scene's animation list, before any context exists: --out-dir - and GIF's limits
+// The refusals that need the scene's animation list, before any context exists: --out-dir -, and GIF's and JPEG's limits
 static int check_output(const Options& o, const std::vector<std::string>& names) {
     const size_t selected = size_t(std::count_if(names.begin(), names.end(), [&](const std::string& nm) { return is_rendered(o, nm); }));
     if (o.to_stdout && selected != 1) { std::fprintf(stderr, "--out-dir - writes one %s stream to stdout: select exactly one animation (%zu selected)\n", o.fmt.name, selected); return 2; }
+    const bool doubled = o.stereo && !o.frame_cmd;
+    const long long frame_w = doubled ? 2LL * o.width : o.width;
+    if (o.fmt.container == PH_OUT_JPEG) {
+        if (o.bits != 8) { std::fprintf(stderr, "JPEG frames are 8-bit: --bit-depth 16 cannot be written as JPEG\n"); return 2; }
+        if (frame_w >= 1 && o.height >= 1 && frame_w <= 65535 && o.height <= 65535) return 0;
+        std::fprintf(stderr, "a JPEG frame is 1 .. 65535 pixels wide and high, got %lld x %d%s\n", frame_w, o.height, doubled ? " (stereo doubles the width)" : "");
+        return 2;
+    }
     if (o.fmt.file != GIF) return 0;
     if (o.bits != 8) { std::fprintf(stderr, "GIF frames are 8-bit: --bit-depth 16 cannot be written as GIF\n"); return 2; }
     if (!o.frame_cmd && o.fps > 50) { std::fprintf(stderr, "--fps %d is above 50: GIF delays are whole centiseconds and browsers show a delay below 2 cs as 10 cs; use --fps 50, 33 or 25\n", o.fps); return 2; }
     if (o.fps < 1 && !o.frame_cmd) { std::fprintf(stderr, "--fps must be at least 1 for GIF, got %d\n", o.fps); return 2; }
-    const bool doubled = o.stereo && !o.frame_cmd;
-    const long long gif_w = doubled ? 2LL * o.width : o.width;
-    if (gif_w >= 1 && o.height >= 1 && gif_w <= 65535 && o.height <= 65535) return 0;
-    std::fprintf(stderr, "a GIF frame is 1 .. 65535 pixels wide and high, got %lld x %d%s\n", gif_w, o.height, doubled ? " (stereo doubles the width)" : "");
+    if (frame_w >= 1 && o.height >= 1 && frame_w <= 65535 && o.height <= 65535) return 0;
+    std::fprintf(stderr, "a GIF frame is 1 .. 65535 pixels wide and high, got %lld x %d%s\n", frame_w, o.height, doubled ? " (stereo doubles the width)" : "");
     return 2;
 }
 // --video name=clip.y4m: every clip is opened (and refused) before a context exists, into `clips` by video name
@@ -551,6 +575,7 @@ struct Shared {
 static int start_player(const Options& o, Worker& wk) {
     wk.player = ph_player_new(wk.scene);
     if (o.adaptive) ph_player_set_adaptive_aa(wk.player, 1, o.adaptive_threshold);
+    ph_player_set_jpeg_quality(wk.player, o.jpeg_quality);
     const struct { const std::string& name; int (*select)(ph_player*, const char*); const char* what; } picks[] = {
         {o.stage, ph_player_init_stage, "stage"}, {o.animation, ph_player_init_animation, "animation"}, {o.camera, ph_player_select_camera, "camera"}};
     for (const auto& s : picks)

@@ -109,8 +109,11 @@ struct pe_ctx {
     // pe_encode_gif_frame's work space: occupancy bitmap, histogram, palette, index stream, per-segment LZW output, segment
     // bit lengths / offsets
     pe_host::DeviceBuffer gif_work;
-    // the host forms of the encoders (pe_encode_png_host*, pe_encode_gif_frame_host): the device copy of the encoding and its
-    // length
+    // pe_encode_jpeg_rgba8's work space: coefficients, symbol histograms, Huffman codes, block offsets, per-row bit streams,
+    // bit lengths, 0xFF counts and file offsets
+    pe_host::DeviceBuffer jpeg_work;
+    // the host forms of the encoders (pe_encode_png_host*, pe_encode_gif_frame_host, pe_encode_jpeg_host): the device copy of
+    // the encoding and its length
     pe_host::DeviceBuffer encoded, encoded_size;
     // pe_set_texture_yuv420's device copy of the Y'CbCr planes it converts
     pe_host::DeviceBuffer yuv_upload;

@@ -1,6 +1,6 @@
 // portal_b200 C ABI (include/portal_b200.h): what happens to a frame after it is rendered -- motion-blur averages,
-// quantisation, PNG and GIF encoding, Y'CbCr 4:2:0 conversion both ways -- through the helper kernels of pe_kernels.cu,
-// pe_png.cu, pe_gif.cu and pe_yuv.cu.  pe_set_texture_yuv420 converts into a sampler's image and lives with the other
+// quantisation, PNG, GIF and JPEG encoding, Y'CbCr 4:2:0 conversion both ways -- through the helper kernels of pe_kernels.cu,
+// pe_png.cu, pe_gif.cu, pe_jpeg.cu and pe_yuv.cu.  pe_set_texture_yuv420 converts into a sampler's image and lives with the other
 // texture upload in pe_api.cpp.
 #include <cstring>
 #include <string>
@@ -114,6 +114,23 @@ int run_gif(pe_ctx* c, const char* fn, const void* frame, int width, int height,
     return launched(c, launch_gif_encode(frame, width, height, delay_cs, c->gif_work.dev, out, size_device, s), fn, 6) ? 0 : 1;
 }
 
+// The checks both forms of pe_encode_jpeg_rgba8 make before anything is allocated or launched
+bool check_jpeg(pe_ctx* c, const std::string& fn, const void* frame, int width, int height, int quality, size_t capacity) {
+    if (!frame) return !c->fail(fn + ": null argument");
+    if (!jpeg_bound(width, height))
+        return !c->fail(fn + ": invalid size " + std::to_string(width) + " x " + std::to_string(height) + " (1 <= width, height <= 65535)");
+    if (quality < 1 || quality > 100) return !c->fail(fn + ": quality " + std::to_string(quality) + " is outside 1 .. 100");
+    const size_t bound = jpeg_bound(width, height);
+    if (capacity < bound) return !c->fail(fn + ": capacity " + std::to_string(capacity) + " is below pe_jpeg_bound = " + std::to_string(bound));
+    if (uintptr_t(frame) & 3) return !c->fail(fn + ": the frame must be 4-byte aligned");
+    return true;
+}
+
+int run_jpeg(pe_ctx* c, const char* fn, const void* frame, int width, int height, int quality, void* jpeg, void* size_device, cudaStream_t s) {
+    if (!cuda_ok(c, c->jpeg_work.ensure(jpeg_workspace_bytes(width, height)), "cudaMalloc(JPEG work space)")) return 1;
+    return launched(c, launch_jpeg_encode(frame, width, height, quality, c->jpeg_work.dev, jpeg, size_device, s), fn, 8) ? 0 : 1;
+}
+
 }  // namespace
 
 bool pe_host::check_yuv420(pe_ctx* c, const std::string& fn, const pe_yuv_format* f, int width, int height) {
@@ -198,6 +215,29 @@ int pe_encode_gif_frame_host(pe_ctx* c, const void* rgba8, int width, int height
     if (!check_gif(c, fn, rgba8, width, height, delay_cs, capacity)) return 1;
     return encode_to_host(c, fn, gif_frame_bound(width, height), out_host, size_out, [&](void* block, void* size_device) {
         return run_gif(c, fn, rgba8, width, height, delay_cs, block, size_device, c->stream);
+    });
+}
+
+// ------------------------------------------------------------------------------ JPEG files (pe_jpeg.cu)
+size_t pe_jpeg_bound(int width, int height) { return jpeg_bound(width, height); }
+
+int pe_encode_jpeg_rgba8(pe_ctx* c, const void* rgba8, int width, int height, int quality, void* jpeg, size_t capacity, void* size_device,
+                         void* stream) {
+    if (!c) return 1;
+    const char* fn = "pe_encode_jpeg_rgba8";
+    if (!jpeg || !size_device) return c->fail(std::string(fn) + ": null argument");
+    if (!check_jpeg(c, fn, rgba8, width, height, quality, capacity) || !bind_device(c)) return 1;
+    return run_jpeg(c, fn, rgba8, width, height, quality, jpeg, size_device, stream_of(c, stream));
+}
+
+int pe_encode_jpeg_host(pe_ctx* c, const void* rgba8, int width, int height, int quality, uint8_t* jpeg_host, size_t capacity,
+                        size_t* size_out) {
+    if (!c) return 1;
+    const char* fn = "pe_encode_jpeg_host";
+    if (!jpeg_host || !size_out) return c->fail(std::string(fn) + ": null argument");
+    if (!check_jpeg(c, fn, rgba8, width, height, quality, capacity)) return 1;
+    return encode_to_host(c, fn, jpeg_bound(width, height), jpeg_host, size_out, [&](void* jpeg, void* size_device) {
+        return run_jpeg(c, fn, rgba8, width, height, quality, jpeg, size_device, c->stream);
     });
 }
 

@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>
+#include <stdint.h>
 
 namespace pe_host {
 
@@ -48,6 +49,20 @@ size_t gif_workspace_bytes(int width, int height);
 // Enqueue a memset and the six kernels: RGBA8 frame -> frame block at `block` (capacity >= gif_frame_bound) with the GCE delay
 // `delay` (centiseconds), its length in *(uint64*)size_out.
 int launch_gif_encode(const void* rgba, int width, int height, int delay, void* work, void* block, void* size_out, cudaStream_t s);
+
+// JPEG files on the device (pe_jpeg.cu; the encoding is tests/host_harness/jpeg_spec.cpp, DESIGN.md section 5.7): one restart
+// interval per MCU row.  The per-block kernels are grid-stride loops over at most kJpegGridCap CTAs of 256 threads; the scans
+// run kJpegScanThreads values per pass.
+constexpr int kJpegGridCap = 132 * 16, kJpegScanThreads = 1024;
+// Upper bound of the file for a width x height frame; 0 unless 1 <= width, height <= 65535.
+size_t jpeg_bound(int width, int height);
+// Bytes of device work space launch_jpeg_encode needs for a width x height frame (256-byte aligned base).
+size_t jpeg_workspace_bytes(int width, int height);
+// The luma and chroma quantisation tables (natural order) at `quality` 1 .. 100.
+void jpeg_quant_tables(int quality, uint8_t q[2][64]);
+// Enqueue a memset and the eight kernels: RGBA8 frame (4-byte aligned) -> JPEG file at `jpeg` (capacity >= jpeg_bound) at
+// `quality`, its length in *(uint64*)size_out.
+int launch_jpeg_encode(const void* rgba, int width, int height, int quality, void* work, void* jpeg, void* size_out, cudaStream_t s);
 
 // RGB -> Y'CbCr 4:2:0 at 10 bits (pe_yuv.cu; DESIGN.md section 5.4).  Bytes of the Y, Cb, Cr planes of a width x height frame,
 // 0 when the size is invalid or the frame has more than 2^31 - 1 pixels.

@@ -308,6 +308,20 @@ class HostPlayer:
         mb = (frame_index, frame_count, motion_blur_frames, float(duration_seconds))
         return self._render(capi.PH_OUT_GIF, 8, width, height, depth, aa_count, motion_blur=mb).tobytes()
 
+    def set_jpeg_quality(self, quality: int):
+        """The quality (1 .. 100; 90 by default) of the next JPEG frames."""
+        self._check(self._lib.ph_player_set_jpeg_quality(self._p, int(quality)))
+
+    def render_frame_jpeg(self, width, height, depth, aa_count=1, aa_start=0) -> bytes:
+        """The frame of render_frame (rgba8=True) as a JPEG file encoded on the device (DESIGN.md section 5.7)."""
+        return self._render(capi.PH_OUT_JPEG, 8, width, height, depth, aa_count, aa_start).tobytes()
+
+    def render_motion_blur_frame_jpeg(self, width, height, depth, frame_index, frame_count, motion_blur_frames, duration_seconds,
+                                      aa_count=1) -> bytes:
+        """render_motion_blur_frame as a JPEG file."""
+        mb = (frame_index, frame_count, motion_blur_frames, float(duration_seconds))
+        return self._render(capi.PH_OUT_JPEG, 8, width, height, depth, aa_count, motion_blur=mb).tobytes()
+
 
 class HostRenderer:
     """SceneRenderer::new + render_frame over the C API only (no scene IR involved)."""
