@@ -403,6 +403,32 @@ PE_API int pe_encode_png_rgba16(pe_ctx* ctx, const void* rgba16_device, int widt
 PE_API int pe_encode_png_host_rgba16(pe_ctx* ctx, const void* rgba16_device, int width, int height, uint8_t* png_host,
                                      size_t capacity, size_t* size_out);
 
+/* ---- Animated PNG (APNG) frames encoded on the device (no counterpart in the reference) --------------------------------
+ * DESIGN.md section 5.8.  A frame block is a pure function of the pixels, `bits`, the frame index k and the delay, built from
+ * the still file S that pe_encode_png_rgba8 / _rgba16 writes for the same pixels.  fcTL(s) is the frame control chunk with
+ * sequence number s, the full width and height at offset 0, 0, delay_num / delay_den seconds, dispose_op 0 (none) and blend_op
+ * 0 (source).  Frame 0 is fcTL(0) || S[33 : |S| - 12], S's own IDAT chunks.  Frame k >= 1 is fcTL(2k - 1) || one fdAT chunk
+ * of sequence number 2k and S's whole zlib stream, so that every sequence number depends on k alone and frames rendered
+ * apart concatenate into one valid file.  A file is pe_apng_header, the blocks in order, and the 12 bytes of IEND
+ * (00 00 00 00 'I' 'E' 'N' 'D' AE 42 60 82).  The bytes do not depend on the GPU, the stream or scheduling.  The work space
+ * is the context's own (never a pe_scratch_buffer slot); one context encodes on one stream at a time. */
+/* Upper bound of the frame block at `bits` 8 or 16: 0 for another depth, or when the PNG bound at that depth is 0. */
+PE_API size_t pe_apng_frame_bound(int width, int height, int bits);
+/* Frame block k = `index` (0 .. 2^30 - 1) of a row-major RGBA8 (`bits` 8, 4-byte aligned) or RGBA16 (`bits` 16, host byte
+ * order, 8-byte aligned) frame in device memory, encoded on the device.  Asynchronous on `stream` (NULL: the context's
+ * stream): six kernel launches, eight for k >= 1.  Writes the block into out_device (capacity >= pe_apng_frame_bound) and its
+ * length into *size_device (uint64).  A bad size, alignment, capacity, bits, index, a delay outside 0 .. 65535 or a context
+ * without a device are refused before any launch.  The frame is only read. */
+PE_API int pe_encode_apng_frame(pe_ctx* ctx, const void* pixels_device, int width, int height, int bits, int index, int delay_num,
+                                int delay_den, void* out_device, size_t capacity, void* size_device, void* stream);
+/* Synchronous form on the context's stream: the block lands in host memory; *size_out = its length. */
+PE_API int pe_encode_apng_frame_host(pe_ctx* ctx, const void* pixels_device, int width, int height, int bits, int index,
+                                     int delay_num, int delay_den, uint8_t* out_host, size_t capacity, size_t* size_out);
+/* The file's header, host only: the PNG signature, IHDR exactly as the still encoder writes it at `bits` (8 or 16, RGBA) and
+ * acTL(num_frames, num_plays; 0 plays: loop forever).  Returns 53, or 0 for a bad size or depth, num_frames outside
+ * 1 .. 2^30, num_plays above 2^31 - 1 or a capacity below 53. */
+PE_API int pe_apng_header(int width, int height, int bits, uint32_t num_frames, uint32_t num_plays, uint8_t* out, size_t capacity);
+
 /* ---- Y'CbCr 4:2:0 at 10 bits (the yuv420p10le the reference's ffmpeg `zscale` step makes from its frames, on the device) ----
  * DESIGN.md section 5.4, restated in tests/helpers/yuv_spec.py: BT.709 matrix, full range, no change of transfer; exact
  * rationals rounded once, round(x) = floor(x + 1/2).  Y = round(1023 (2126 R + 7152 G + 722 B) / (10000 M)) at every pixel

@@ -179,7 +179,8 @@ PE_API int ph_scene_camera_name(ph_scene* s, int k, const char** name);
  *   Y'CbCr 4:2:0 planes at 10 bits (pe_rgba_to_yuv420p10, DESIGN.md section 5.4: Y, then Cb, then Cr) or, at 8 bits only,
  *   one GIF frame block (pe_encode_gif_frame, DESIGN.md section 5.6, with the delay of ph_player_set_gif_delay; a file is
  *   pe_gif_header, the blocks and the trailer 0x3B) or a JPEG file (pe_encode_jpeg_rgba8, DESIGN.md section 5.7, at the quality
- *   of ph_player_set_jpeg_quality);
+ *   of ph_player_set_jpeg_quality); or, at 8 or 16 bits, one APNG frame block (pe_encode_apng_frame, DESIGN.md section 5.8,
+ *   with the index and delay of ph_player_set_apng_frame; a file is pe_apng_header, the blocks and IEND);
  * - read it back into out_host (capacity >= ph_output_bytes), *len bytes.  Pixels and planes are in host byte order.
  * Any other combination, bad motion-blur arguments or a short capacity are refused before any launch.
  * Scratch slots (pe_scratch_buffer) of the context, with M sub-frames (0 without motion blur): slot 0 holds the frame, slots
@@ -187,7 +188,7 @@ PE_API int ph_scene_camera_name(ph_scene* s, int k, const char** name);
  * Y'CbCr planes.  At 16 bits that is 8 (M + 1) + 16 bytes per pixel before the planes, 17.8 GB at 7680 x 4320 with M = 64.
  * A single frame of RGBA8 or float pixels without adaptive anti-aliasing is rendered straight into host memory
  * (pe_render_host_rgba8 / pe_render_host) and uses no slot. */
-enum { PH_OUT_PIXELS = 0, PH_OUT_PNG = 1, PH_OUT_YUV420P10 = 2, PH_OUT_GIF = 3, PH_OUT_JPEG = 4 };
+enum { PH_OUT_PIXELS = 0, PH_OUT_PNG = 1, PH_OUT_YUV420P10 = 2, PH_OUT_GIF = 3, PH_OUT_JPEG = 4, PH_OUT_APNG = 5 };
 /* One output frame of render_animation (src/main.rs:1786-1817): sub-frame j of frame `frame_index` (of `frame_count`) calls
  * update(t_j * duration_seconds), t_j = frame_index/frame_count + j/motion_blur_frames/frame_count * 0.5 -- time mapping,
  * camera interpolation, teleportation and the update hook --, renders with `_aa_start` = j, and the sub-frames are averaged
@@ -198,8 +199,8 @@ typedef struct ph_motion_blur {
     double duration_seconds;
 } ph_motion_blur;
 /* The capacity a `container` of a width x height frame at `bits` needs: w * h * bits / 2 (pixels), pe_png_bound /
- * pe_png_bound_rgba16 (PNG), pe_yuv420p10_bytes (Y'CbCr), pe_gif_frame_bound (GIF, bits 8), pe_jpeg_bound (JPEG, bits 8); 0 when
- * there is no such output. */
+ * pe_png_bound_rgba16 (PNG), pe_yuv420p10_bytes (Y'CbCr), pe_gif_frame_bound (GIF, bits 8), pe_jpeg_bound (JPEG, bits 8),
+ * pe_apng_frame_bound (APNG, bits 8 or 16); 0 when there is no such output. */
 PE_API size_t ph_output_bytes(int container, int bits, int width, int height);
 PE_API int ph_player_render(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, const ph_motion_blur* mb, int container,
                             int bits, void* out_host, size_t capacity, size_t* len);
@@ -218,6 +219,9 @@ PE_API int ph_player_advance_motion_blur_frame(ph_player* pl, int frame_index, i
 PE_API int ph_player_set_adaptive_aa(ph_player* pl, int on, int threshold);
 /* The Graphic Control Extension delay, in centiseconds (0 .. 65535; 0 by default), of the player's next PH_OUT_GIF blocks. */
 PE_API int ph_player_set_gif_delay(ph_player* pl, int delay_cs);
+/* The frame index (0 .. 2^30 - 1) and the fcTL delay delay_num / delay_den seconds (each 0 .. 65535; 0 / 1 by default) of the
+ * player's next PH_OUT_APNG blocks. */
+PE_API int ph_player_set_apng_frame(ph_player* pl, int index, int delay_num, int delay_den);
 /* The quality (1 .. 100; 90 by default) of the player's next PH_OUT_JPEG files. */
 PE_API int ph_player_set_jpeg_quality(ph_player* pl, int quality);
 

@@ -36,7 +36,7 @@ class PhMotionBlur(C.Structure):
                 ("duration_seconds", C.c_double)]
 
 
-PH_OUT_PIXELS, PH_OUT_PNG, PH_OUT_YUV420P10, PH_OUT_GIF, PH_OUT_JPEG = 0, 1, 2, 3, 4
+PH_OUT_PIXELS, PH_OUT_PNG, PH_OUT_YUV420P10, PH_OUT_GIF, PH_OUT_JPEG, PH_OUT_APNG = 0, 1, 2, 3, 4, 5
 
 PE_YUV_BT709, PE_YUV_BT601 = 0, 1
 PE_YUV_SITING_LEFT, PE_YUV_SITING_CENTER = 0, 1
@@ -148,6 +148,10 @@ def lib() -> C.CDLL:
         "pe_encode_gif_frame_host": (i32, [vp, vp, i32, i32, i32, vp, C.c_size_t, C.POINTER(C.c_size_t)]),
         "pe_gif_header": (i32, [i32, i32, i32, vp, C.c_size_t]),
         "pe_jpeg_bound": (C.c_size_t, [i32, i32]),
+        "pe_apng_frame_bound": (C.c_size_t, [i32, i32, i32]),
+        "pe_encode_apng_frame": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, vp, C.c_size_t, vp, vp]),
+        "pe_encode_apng_frame_host": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, vp, C.c_size_t, C.POINTER(C.c_size_t)]),
+        "pe_apng_header": (i32, [i32, i32, i32, C.c_uint32, C.c_uint32, vp, C.c_size_t]),
         "pe_encode_jpeg_rgba8": (i32, [vp, vp, i32, i32, i32, vp, C.c_size_t, vp, vp]),
         "pe_encode_jpeg_host": (i32, [vp, vp, i32, i32, i32, vp, C.c_size_t, C.POINTER(C.c_size_t)]),
         "pe_yuv420p10_bytes": (C.c_size_t, [i32, i32]),
@@ -226,6 +230,7 @@ def lib() -> C.CDLL:
         "ph_player_set_adaptive_aa": (i32, [vp, i32, i32]),
         "ph_player_set_gif_delay": (i32, [vp, i32]),
         "ph_player_set_jpeg_quality": (i32, [vp, i32]),
+        "ph_player_set_apng_frame": (i32, [vp, i32, i32, i32]),
         "ph_y4m_open": (vp, [cp, i32, cp, C.c_size_t]),
         "ph_y4m_info": (i32, [vp, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(PeYuvFormat),
                               C.POINTER(C.c_int64)]),
@@ -313,6 +318,48 @@ def _encode_on_stream(ctx, rgba8, what: str, bound: str, encode: str, arg: int) 
     if L.pe_memcpy_d2h(ctx, host, C.c_void_p(out.data_ptr()), n.value, stream):
         raise PortalB200Error(L.pe_last_error(ctx).decode(errors="replace"))
     return bytes(host[:n.value])
+
+
+def encode_apng_frame(ctx, pixels, index: int = 0, delay_num: int = 0, delay_den: int = 1) -> bytes:
+    """APNG frame block `index` (DESIGN.md section 5.8) of a CUDA uint8 (8-bit) or uint16 (16-bit, host byte order) tensor
+    [h, w, 4] (contiguous) with the delay delay_num / delay_den seconds, encoded on the device by pe_encode_apng_frame on
+    context `ctx`, ordered after the work already queued on the current torch stream.  A file is
+    apng_header(w, h, bits, n) + blocks 0 .. n - 1 + IEND."""
+    import torch
+    if (pixels.dim() != 3 or pixels.shape[2] != 4 or not pixels.is_cuda or pixels.dtype not in (torch.uint8, torch.uint16)
+            or not pixels.is_contiguous()):
+        raise ValueError("frame must be a contiguous CUDA uint8 or uint16 tensor [h, w, 4]")
+    L = lib()
+    bits = 8 if pixels.dtype == torch.uint8 else 16
+    h, w = int(pixels.shape[0]), int(pixels.shape[1])
+    cap = L.pe_apng_frame_bound(w, h, bits)
+    if cap == 0:
+        raise PortalB200Error(f"pe_apng_frame_bound: no APNG frame for a {w} x {h} frame at {bits} bits")
+    out = torch.empty(cap, dtype=torch.uint8, device=pixels.device)
+    size = torch.empty(1, dtype=torch.int64, device=pixels.device)
+    # the read-backs go on the same stream handle (0, torch's default stream, names the context's stream)
+    stream = C.c_void_p(torch.cuda.current_stream(pixels.device).cuda_stream)
+    n = C.c_uint64()
+    if (L.pe_encode_apng_frame(ctx, C.c_void_p(pixels.data_ptr()), w, h, bits, int(index), int(delay_num), int(delay_den),
+                               C.c_void_p(out.data_ptr()), cap, C.c_void_p(size.data_ptr()), stream)
+            or L.pe_memcpy_d2h(ctx, C.addressof(n), C.c_void_p(size.data_ptr()), 8, stream)):
+        raise PortalB200Error(L.pe_last_error(ctx).decode(errors="replace"))
+    host = (C.c_uint8 * max(1, n.value))()
+    if L.pe_memcpy_d2h(ctx, host, C.c_void_p(out.data_ptr()), n.value, stream):
+        raise PortalB200Error(L.pe_last_error(ctx).decode(errors="replace"))
+    return bytes(host[:n.value])
+
+
+def apng_header(width: int, height: int, bits: int, num_frames: int, num_plays: int = 0) -> bytes:
+    """The APNG file header pe_apng_header writes: the PNG signature, IHDR at `bits` 8 or 16 and acTL."""
+    buf = (C.c_uint8 * 64)()
+    n = lib().pe_apng_header(width, height, bits, num_frames, num_plays, buf, 64)
+    if n == 0:
+        raise PortalB200Error(f"pe_apng_header: no APNG header for a {width} x {height} frame at {bits} bits, {num_frames} frames")
+    return bytes(buf[:n])
+
+
+APNG_TRAILER = b"\x00\x00\x00\x00IEND\xaeB`\x82"
 
 
 def gif_header(width: int, height: int, loop: bool) -> bytes:

@@ -31,6 +31,7 @@ struct ph_player {
     bool adaptive_aa = false;           // ph_player_set_adaptive_aa: frames go through pe_render_adaptive
     int gif_delay = 0;                  // ph_player_set_gif_delay: the GCE delay of PH_OUT_GIF blocks, centiseconds
     int jpeg_quality = 90;              // ph_player_set_jpeg_quality: the quality of PH_OUT_JPEG files
+    int apng_index = 0, apng_delay_num = 0, apng_delay_den = 1;   // ph_player_set_apng_frame: of PH_OUT_APNG blocks
     int adaptive_threshold = 8;
     explicit ph_player(ph_scene* sc) : s(sc), player(sc->scene) {}
 };
@@ -625,6 +626,17 @@ int ph_player_set_gif_delay(ph_player* pl, int delay_cs) {
     return 0;
 }
 
+int ph_player_set_apng_frame(ph_player* pl, int index, int delay_num, int delay_den) {
+    if (!pl) return 1;
+    if (index < 0 || index > (1 << 30) - 1) return pfail(pl, "ph_player_set_apng_frame: frame index " + std::to_string(index) + " is outside 0 .. 2^30 - 1");
+    if (delay_num < 0 || delay_num > 65535 || delay_den < 0 || delay_den > 65535)
+        return pfail(pl, "ph_player_set_apng_frame: delay " + std::to_string(delay_num) + " / " + std::to_string(delay_den) + " is outside 0 .. 65535");
+    pl->apng_index = index;
+    pl->apng_delay_num = delay_num;
+    pl->apng_delay_den = delay_den;
+    return 0;
+}
+
 int ph_player_set_jpeg_quality(ph_player* pl, int quality) {
     if (!pl) return 1;
     if (quality < 1 || quality > 100) return pfail(pl, "ph_player_set_jpeg_quality: quality " + std::to_string(quality) + " is outside 1 .. 100");
@@ -651,6 +663,7 @@ size_t ph_output_bytes(int container, int bits, int width, int height) {
         case PH_OUT_YUV420P10: return bits == 8 || bits == 16 ? pe_yuv420p10_bytes(width, height) : 0;
         case PH_OUT_GIF: return bits == 8 ? pe_gif_frame_bound(width, height) : 0;
         case PH_OUT_JPEG: return bits == 8 ? pe_jpeg_bound(width, height) : 0;
+        case PH_OUT_APNG: return pe_apng_frame_bound(width, height, bits);
     }
     return 0;
 }
@@ -660,11 +673,11 @@ int ph_player_render(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, const
                      void* out_host, size_t capacity, size_t* len) {
     if (!pl || !ctx || !p || !out_host || !len) return 1;
     if (container != PH_OUT_PIXELS && container != PH_OUT_PNG && container != PH_OUT_YUV420P10 && container != PH_OUT_GIF &&
-        container != PH_OUT_JPEG)
+        container != PH_OUT_JPEG && container != PH_OUT_APNG)
         return pfail(pl, "ph_player_render: unknown container " + std::to_string(container));
     if (container == PH_OUT_GIF && bits != 8) return pfail(pl, "ph_player_render: GIF frames are 8-bit (bits must be 8)");
     if (container == PH_OUT_JPEG && bits != 8) return pfail(pl, "ph_player_render: JPEG frames are 8-bit (bits must be 8)");
-    if (container != PH_OUT_PIXELS && bits != 8 && bits != 16) return pfail(pl, "ph_player_render: bits must be 8 or 16 for PNG and Y'CbCr");
+    if (container != PH_OUT_PIXELS && bits != 8 && bits != 16) return pfail(pl, "ph_player_render: bits must be 8 or 16 for PNG, APNG and Y'CbCr");
     if (bits != 8 && bits != 16 && bits != 32) return pfail(pl, "ph_player_render: bits must be 8, 16 or 32");
     if (bits == 32 && mb) return pfail(pl, "ph_player_render: motion blur needs bits 8 or 16 (its sub-frames are averaged as integers)");
     std::vector<double> times;
@@ -698,6 +711,12 @@ int ph_player_render(ph_player* pl, pe_ctx* ctx, const ph_frame_params* p, const
         if (bits == 16 ? pe_encode_png_host_rgba16(ctx, frame, p->width, p->height, static_cast<uint8_t*>(out_host), capacity, len)
                        : pe_encode_png_host(ctx, frame, p->width, p->height, static_cast<uint8_t*>(out_host), capacity, len))
             return pfail(pl, std::string("PNG encoding failed: ") + pe_last_error(ctx));
+        return 0;
+    }
+    if (container == PH_OUT_APNG) {
+        if (pe_encode_apng_frame_host(ctx, frame, p->width, p->height, bits, pl->apng_index, pl->apng_delay_num, pl->apng_delay_den,
+                                      static_cast<uint8_t*>(out_host), capacity, len))
+            return pfail(pl, std::string("APNG encoding failed: ") + pe_last_error(ctx));
         return 0;
     }
     if (container == PH_OUT_GIF) {

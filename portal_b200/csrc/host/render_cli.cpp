@@ -4,16 +4,16 @@
 //   portal_b200_render render-frame <scene.ron> [--width W] [--height H] [--render-depth D] [--aa-count N]
 //                      [--time T] [--stage NAME] [--animation NAME] [--camera NAME] [--device K]
 //                      [--texture name=file.png | name=file.rgba:WxH ...] [--assets DIR] [--output out.png|.ppm|.rgba]
-//                      [--adaptive-aa T] [--bit-depth 8|16]                   (also --output out.y4m | out.gif | out.jpg)
+//                      [--adaptive-aa T] [--bit-depth 8|16]        (also --output out.y4m | out.gif | out.jpg | out.apng)
 //                      [--jpeg-quality Q]
 //                      [--video name=clip.y4m ...] [--video-matrix bt709|bt601]
 //   portal_b200_render render <scene.ron> [--animations a,b,... | --starts-with PREFIX] [--fps N] [--motion-blur-frames M] [--width W]
 //                      [--height H] [--render-depth D] [--aa-count N] [--stereo-image] [--no-skip-existing] [--out-dir DIR] [--max-frames K]
-//                      [--frame-format ppm|png|rgba|y4m|gif|jpg] [--jpeg-quality Q] [--assets DIR] [--adaptive-aa T] [--bit-depth 8|16]
+//                      [--frame-format ppm|png|rgba|y4m|gif|jpg|apng] [--jpeg-quality Q] [--assets DIR] [--adaptive-aa T] [--bit-depth 8|16]
 //                      [--video name=clip.y4m ...] [--video-matrix bt709|bt601]
 //                      (`portal render`, main.rs:2808-2873 -> render_named_animations :1876-1930 ->
 //                       render_animation :1757-1830; frames are written as DIR/<animation>/frame_<i>.<format>, or as one
-//                       stream DIR/<animation>.y4m or DIR/<animation>.gif; the HEVC encode itself is out of scope)
+//                       stream DIR/<animation>.y4m, .gif or .apng; the HEVC encode itself is out of scope)
 //
 // --adaptive-aa T (not in the reference; off by default): every frame / sub-frame is traced with one sample, and with all
 // --aa-count samples only where that frame has an edge (a 3x3 unorm8 range above T, pe_render_adaptive).
@@ -47,6 +47,13 @@
 // render-frame writes one, `render` writes DIR/<animation>/frame_<i>.jpg.  JPEG is 8-bit: --bit-depth 16 is refused, and so
 // are a frame wider or taller than 65535 pixels and --jpeg-quality with any other format.
 //
+// --frame-format apng / --output *.apng (not in the reference): an animated PNG, lossless and at 8 or 16 bits (--bit-depth
+// 16).  Every frame is encoded on the device into one APNG frame block (pe_encode_apng_frame; DESIGN.md section 5.8: the still
+// PNG of the frame, reframed as fcTL + IDAT for frame 0 and fcTL + one fdAT chunk after it).  `render` writes one stream per
+// animation, DIR/<animation>.apng, exactly as a Y4M or GIF stream: the header with acTL(frames rendered, 0 plays: loop
+// forever), the blocks and IEND.  Frame i has index i and shows for exactly 1 / fps seconds; --fps above 65535, the largest
+// fcTL denominator, is refused.  render-frame writes a one-frame file with a delay of 1 / 25 s.
+//
 // Output: the RGBA8 frame the reference hands to export_png (main.rs:2939-2943) as a PNG when the name ends in .png (encoded
 // on the device: pe_encode_png_rgba8), as raw RGBA8 for .rgba, else as a binary PPM (P6, alpha dropped).  Every format is one
 // ph_player_render call per frame.  Textures: every texture of the scene is loaded from its stored path (a PNG, relative to
@@ -68,7 +75,7 @@
 // player, clip handles and pinned buffers, and runs the whole loop: frame i of an animation is rendered by worker i mod N and
 // replayed by every other one (ph_player_advance_motion_blur_frame), so that camera teleportation through portals -- state that
 // carries from frame to frame -- is the sequential one everywhere.  Skip-existing decides from one snapshot of the output taken
-// before the workers start.  Frame files are written by their worker; a Y4M or GIF stream by the main thread, in frame order,
+// before the workers start.  Frame files are written by their worker; a Y4M, GIF or APNG stream by the main thread, in frame order,
 // with at most two frames per worker in flight.  Status lines come in frame order, as from one worker.  The first failure stops every
 // worker at its next frame boundary, exits 1 and renames no stream.  render-frame takes one entry.
 #include <dirent.h>
@@ -107,19 +114,20 @@ static bool ends_with(const std::string& s, const char* suffix) {
 
 // How a frame becomes output, decided once from the extension (of --output, or --frame-format) and --bit-depth: what
 // ph_player_render delivers (the container, rendered at `bits`), how those bytes become a file, and what messages call them
-enum FrameFile { AS_RETURNED, PPM, Y4M, GIF };
+enum FrameFile { AS_RETURNED, PPM, Y4M, GIF, APNG };
 struct FrameFormat {
     FrameFile file = PPM;
     int container = PH_OUT_PIXELS, bits = 8;
     std::string ext;            // `render`'s files: DIR/<animation>/frame_<i><ext>, or the stream DIR/<animation><ext>
     const char* name = "";      // the stream's name in messages
     const char* what = "";      // what one ph_player_render call returns, in messages
-    bool stream() const { return file == Y4M || file == GIF; }   // `render`: one file per animation, not per frame
+    bool stream() const { return file == Y4M || file == GIF || file == APNG; }   // `render`: one file per animation, not per frame
 };
 static FrameFormat frame_format(const std::string& ext, int bits) {
     if (ext == ".png") return {AS_RETURNED, PH_OUT_PNG, bits, ext, "PNG", "PNG"};   // Image::export_png (main.rs:2939-2943)
     if (ext == ".y4m") return {Y4M, PH_OUT_YUV420P10, bits, ext, "Y4M", "Y4M stream"};
     if (ext == ".gif") return {GIF, PH_OUT_GIF, bits, ext, "GIF", "GIF frame"};
+    if (ext == ".apng") return {APNG, PH_OUT_APNG, bits, ext, "APNG", "APNG frame"};
     if (ext == ".jpg" || ext == ".jpeg") return {AS_RETURNED, PH_OUT_JPEG, bits, ext, "JPEG", "JPEG"};
     return {ends_with(ext, ".rgba") ? AS_RETURNED : PPM, PH_OUT_PIXELS, bits, ext, "image", "image"};
 }
@@ -127,18 +135,24 @@ static FrameFormat frame_format(const std::string& ext, int bits) {
 // A stream: the header, each frame as ph_player_render returns it, the trailer.  Y4M: the tags ffmpeg's own muxer writes for
 // full-range yuv420p10le, "FRAME\n" and the Y, Cb, Cr planes as little-endian uint16 per frame, no trailer; it cannot carry the
 // matrix (BT.709): the encode command states it (README.md, DESIGN.md section 5.4).  GIF: pe_gif_header, the blocks, the trailer.
+// APNG: pe_apng_header with the number of frames, the blocks, IEND.
 static_assert(__BYTE_ORDER__ == __ORDER_LITTLE_ENDIAN__, "the planes are written as read back, in host byte order");
-static bool write_stream_header(FILE* f, const FrameFormat& fmt, int width, int height, int fps, bool loop) {
+static bool write_stream_header(FILE* f, const FrameFormat& fmt, int width, int height, int fps, bool loop, int frames) {
     if (fmt.file == Y4M)
         return std::fprintf(f, "YUV4MPEG2 W%d H%d F%d:1 Ip A1:1 C420p10 XYSCSS=420P10 XCOLORRANGE=FULL\n", width, height, fps) > 0;
     uint8_t h[64];
-    const int n = pe_gif_header(width, height, loop ? 1 : 0, h, sizeof h);
+    const int n = fmt.file == APNG ? pe_apng_header(width, height, fmt.bits, uint32_t(frames), 0, h, sizeof h)
+                                   : pe_gif_header(width, height, loop ? 1 : 0, h, sizeof h);
     return n > 0 && std::fwrite(h, 1, size_t(n), f) == size_t(n);
 }
 static bool write_stream_frame(FILE* f, const FrameFormat& fmt, const uint8_t* data, size_t len) {
     return (fmt.file != Y4M || std::fputs("FRAME\n", f) >= 0) && std::fwrite(data, 1, len, f) == len;
 }
-static bool write_stream_trailer(FILE* f, const FrameFormat& fmt) { return fmt.file != GIF || std::fputc(0x3B, f) != EOF; }
+static bool write_stream_trailer(FILE* f, const FrameFormat& fmt) {
+    static const uint8_t iend[12] = {0, 0, 0, 0, 'I', 'E', 'N', 'D', 0xAE, 0x42, 0x60, 0x82};
+    if (fmt.file == APNG) return std::fwrite(iend, 1, 12, f) == 12;
+    return fmt.file != GIF || std::fputc(0x3B, f) != EOF;
+}
 
 // Centiseconds frame i of a GIF stream at `fps` shows for: round(100 (i + 1) / fps) - round(100 i / fps), halves up, so that
 // the first n frames last round(100 n / fps)
@@ -343,9 +357,9 @@ static int parse_options(int argc, char** argv, Options& o) {
     const bool anim_cmd = argc >= 3 && std::strcmp(argv[1], "render") == 0;
     if (!o.frame_cmd && !anim_cmd) {
         std::fprintf(stderr, "usage: %s render-frame <scene.ron> [--width W] [--height H] [--render-depth D] [--aa-count N] [--time T] "
-                             "[--stage NAME] [--animation NAME] [--camera NAME] [--device K] [--texture name=file.png|name=file.rgba:WxH] [--assets DIR] [--output out.png|.ppm|.rgba|.y4m|.gif|.jpg] [--jpeg-quality Q] [--adaptive-aa T] [--bit-depth 8|16] [--video name=clip.y4m] [--video-matrix bt709|bt601]\n"
+                             "[--stage NAME] [--animation NAME] [--camera NAME] [--device K] [--texture name=file.png|name=file.rgba:WxH] [--assets DIR] [--output out.png|.ppm|.rgba|.y4m|.gif|.jpg|.apng] [--jpeg-quality Q] [--adaptive-aa T] [--bit-depth 8|16] [--video name=clip.y4m] [--video-matrix bt709|bt601]\n"
                              "       %s render <scene.ron> [a,b | --animations a,b | --starts-with PREFIX] [--fps N] [--motion-blur-frames M] [--width W] [--height H] "
-                             "[--render-depth D] [--aa-count N] [--stereo-image] [--no-skip-existing] [--out-dir DIR] [--max-frames K] [--frame-format ppm|png|rgba|y4m|gif|jpg] [--jpeg-quality Q] [--adaptive-aa T] [--bit-depth 8|16] [--video name=clip.y4m] [--video-matrix bt709|bt601] [--device K | --devices K,K,...]\n", argv[0], argv[0]);
+                             "[--render-depth D] [--aa-count N] [--stereo-image] [--no-skip-existing] [--out-dir DIR] [--max-frames K] [--frame-format ppm|png|rgba|y4m|gif|jpg|apng] [--jpeg-quality Q] [--adaptive-aa T] [--bit-depth 8|16] [--video name=clip.y4m] [--video-matrix bt709|bt601] [--device K | --devices K,K,...]\n", argv[0], argv[0]);
         return 2;
     }
     o.scene_path = argv[2];
@@ -385,7 +399,7 @@ static int parse_options(int argc, char** argv, Options& o) {
             o.video_matrix = v == "bt601" ? PE_YUV_BT601 : PE_YUV_BT709;
         }
         else if (a == "--assets") o.assets = next();
-        else if (a == "--frame-format") frame_ext = std::string(".") + next();          // render: ppm (default) | png | rgba | y4m | gif | jpg
+        else if (a == "--frame-format") frame_ext = std::string(".") + next();          // render: ppm (default) | png | rgba | y4m | gif | jpg | apng
         else if (a == "--jpeg-quality" || a == "--jpeg_quality") {
             const char* v = next();
             char* end = nullptr;
@@ -455,7 +469,7 @@ static bool is_rendered(const Options& o, const std::string& name) {
     return !o.all_animations || o.starts_with.empty() || name.compare(0, o.starts_with.size(), o.starts_with) == 0;
 }
 
-// The refusals that need the scene's animation list, before any context exists: --out-dir -, and GIF's and JPEG's limits
+// The refusals that need the scene's animation list, before any context exists: --out-dir -, and GIF's, JPEG's and APNG's limits
 static int check_output(const Options& o, const std::vector<std::string>& names) {
     const size_t selected = size_t(std::count_if(names.begin(), names.end(), [&](const std::string& nm) { return is_rendered(o, nm); }));
     if (o.to_stdout && selected != 1) { std::fprintf(stderr, "--out-dir - writes one %s stream to stdout: select exactly one animation (%zu selected)\n", o.fmt.name, selected); return 2; }
@@ -466,6 +480,10 @@ static int check_output(const Options& o, const std::vector<std::string>& names)
         if (frame_w >= 1 && o.height >= 1 && frame_w <= 65535 && o.height <= 65535) return 0;
         std::fprintf(stderr, "a JPEG frame is 1 .. 65535 pixels wide and high, got %lld x %d%s\n", frame_w, o.height, doubled ? " (stereo doubles the width)" : "");
         return 2;
+    }
+    if (o.fmt.file == APNG && !o.frame_cmd) {
+        if (o.fps > 65535) { std::fprintf(stderr, "--fps %d is above 65535: an APNG frame's delay is 1 / fps seconds with a 16-bit denominator\n", o.fps); return 2; }
+        if (o.fps < 1) { std::fprintf(stderr, "--fps must be at least 1 for APNG, got %d\n", o.fps); return 2; }
     }
     if (o.fmt.file != GIF) return 0;
     if (o.bits != 8) { std::fprintf(stderr, "GIF frames are 8-bit: --bit-depth 16 cannot be written as GIF\n"); return 2; }
@@ -516,7 +534,7 @@ struct AnimationPlan {
     bool rendered = false;           // false: --starts-with filters it out (it is still initialised and updated once)
     double duration = 0.0;           // the f32 duration render_animation takes
     int count = 1, todo = 0;         // frames of the animation, frames to render (--max-frames)
-    bool skip_stream = false;        // Y4M or GIF: the stream exists
+    bool skip_stream = false;        // Y4M, GIF or APNG: the stream exists
     std::vector<char> skip_frame;    // frame files: frame i exists
 };
 
@@ -526,7 +544,7 @@ struct Shared {
     std::condition_variable cv;
     bool stop = false;
     std::string error;
-    // (animation, frame) -> the frame's Y4M planes or GIF block (empty for frame files); frame -1: the animation has begun
+    // (animation, frame) -> the frame's Y4M planes, GIF or APNG block (empty for frame files); frame -1: the animation has begun
     std::map<std::pair<size_t, int>, std::vector<uint8_t>> done;
 
     void fail(const std::string& why) {
@@ -679,11 +697,11 @@ static int set_up(const Options& o, Worker& wk, bool first, std::map<std::string
 // render-frame (main.rs:2928-2946)
 static int render_frame(const Options& o, Worker& wk, const ph_frame_params& p, size_t frame_bytes) {
     wk.px.resize(frame_bytes);
-    if (ph_player_update(wk.player, o.time) ||
+    if ((o.fmt.file == APNG && ph_player_set_apng_frame(wk.player, 0, 1, 25)) || ph_player_update(wk.player, o.time) ||
         ph_player_render(wk.player, wk.ctx, &p, nullptr, o.fmt.container, o.fmt.bits, wk.px.data(), wk.px.size(), &wk.len)) { std::fprintf(stderr, "%s\n", ph_player_last_error(wk.player)); return 1; }
     FILE* f = o.fmt.stream() ? std::fopen(o.output.c_str(), "wb") : nullptr;    // a one-frame stream: 25 fps, no GIF loop block
     const bool ok = !o.fmt.stream() ? write_frame(o.output, o.fmt, wk.px, wk.len, p.width, p.height)
-                                    : f && write_stream_header(f, o.fmt, p.width, p.height, 25, false) && write_stream_frame(f, o.fmt, wk.px.data(), wk.len) && write_stream_trailer(f, o.fmt);
+                                    : f && write_stream_header(f, o.fmt, p.width, p.height, 25, false, 1) && write_stream_frame(f, o.fmt, wk.px.data(), wk.len) && write_stream_trailer(f, o.fmt);
     if ((f && std::fclose(f) != 0) || !ok) { std::fprintf(stderr, "cannot write %s\n", o.output.c_str()); return 1; }
     std::printf("Rendered `%s` to `%s`\n", o.scene_path.c_str(), o.output.c_str());
     return 0;
@@ -738,10 +756,11 @@ static void run_worker(const Options& o, const std::vector<AnimationPlan>& plan,
             }
             std::vector<uint8_t> planes;                           // a stream: the frame goes to the main thread
             if (o.fmt.stream() && !sh.take_buffer(wk, planes)) return;
-            if (o.fmt.stream()) planes.resize(frame_bytes);          // a GIF block came back cut to its length
+            if (o.fmt.stream()) planes.resize(frame_bytes);          // a GIF or APNG block came back cut to its length
             std::vector<uint8_t>& buf = o.fmt.stream() ? planes : wk.px;
             const ph_motion_blur mb = {i, a.count, o.motion_blur, a.duration};
             if ((o.fmt.file == GIF && ph_player_set_gif_delay(wk.player, gif_delay(i, o.fps))) ||
+                (o.fmt.file == APNG && ph_player_set_apng_frame(wk.player, i, 1, o.fps)) ||
                 ph_player_render(wk.player, wk.ctx, &p, &mb, o.fmt.container, o.fmt.bits, buf.data(), buf.size(), &wk.len)) { sh.fail(ph_player_last_error(wk.player)); return; }
             const std::string name = dir + "/frame_" + std::to_string(i) + o.fmt.ext;
             if (o.fmt.stream()) planes.resize(wk.len);
@@ -766,7 +785,7 @@ static void write_in_order(const Options& o, const std::vector<AnimationPlan>& p
         if (o.fmt.stream()) {
             if (!o.to_stdout && !make_dirs(o.out_dir)) { sh.fail("cannot create " + o.out_dir); return; }
             f = o.to_stdout ? stdout : std::fopen(part.c_str(), "wb");
-            ok = f && write_stream_header(f, o.fmt, p.width, p.height, o.fps, true);
+            ok = f && write_stream_header(f, o.fmt, p.width, p.height, o.fps, true, a.todo);
         }
         for (int i = 0; i < a.todo && ok; i++) {
             if (a.skip_frame[size_t(i)]) continue;

@@ -106,14 +106,16 @@ struct pe_ctx {
     AdaptiveBuffers adaptive[2];
     // pe_encode_png_rgba8's work space: filtered stream, per-segment deflate output, segment sizes / offsets / checksums
     pe_host::DeviceBuffer png_work;
+    // pe_encode_apng_frame's work space: the PNG work space, the still file, its length and the CRC of each IDAT chunk's payload
+    pe_host::DeviceBuffer apng_work;
     // pe_encode_gif_frame's work space: occupancy bitmap, histogram, palette, index stream, per-segment LZW output, segment
     // bit lengths / offsets
     pe_host::DeviceBuffer gif_work;
     // pe_encode_jpeg_rgba8's work space: coefficients, symbol histograms, Huffman codes, block offsets, per-row bit streams,
     // bit lengths, 0xFF counts and file offsets
     pe_host::DeviceBuffer jpeg_work;
-    // the host forms of the encoders (pe_encode_png_host*, pe_encode_gif_frame_host, pe_encode_jpeg_host): the device copy of
-    // the encoding and its length
+    // the host forms of the encoders (pe_encode_png_host*, pe_encode_apng_frame_host, pe_encode_gif_frame_host,
+    // pe_encode_jpeg_host): the device copy of the encoding and its length
     pe_host::DeviceBuffer encoded, encoded_size;
     // pe_set_texture_yuv420's device copy of the Y'CbCr planes it converts
     pe_host::DeviceBuffer yuv_upload;

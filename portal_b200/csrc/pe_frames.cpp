@@ -1,7 +1,8 @@
 // portal_b200 C ABI (include/portal_b200.h): what happens to a frame after it is rendered -- motion-blur averages,
-// quantisation, PNG, GIF and JPEG encoding, Y'CbCr 4:2:0 conversion both ways -- through the helper kernels of pe_kernels.cu,
+// quantisation, PNG, APNG, GIF and JPEG encoding, Y'CbCr 4:2:0 conversion both ways -- through the helper kernels of pe_kernels.cu,
 // pe_png.cu, pe_gif.cu, pe_jpeg.cu and pe_yuv.cu.  pe_set_texture_yuv420 converts into a sampler's image and lives with the other
 // texture upload in pe_api.cpp.
+#include <cstdint>
 #include <cstring>
 #include <string>
 
@@ -97,6 +98,33 @@ int encode_png_host(pe_ctx* c, const char* fn, int bpp, const void* frame, int w
     });
 }
 
+// The checks both forms of pe_encode_apng_frame make before anything is allocated or launched: bits 8 or 16, the frame index
+// and the delays in range, then the PNG checks with the APNG block's bound
+bool check_apng(pe_ctx* c, const std::string& fn, const void* frame, int width, int height, int bits, int index, int delay_num,
+                int delay_den, size_t capacity) {
+    if (!frame) return !c->fail(fn + ": null argument");
+    if (bits != 8 && bits != 16) return !c->fail(fn + ": bits must be 8 or 16, got " + std::to_string(bits));
+    if (index < 0 || index > kApngMaxIndex)
+        return !c->fail(fn + ": frame index " + std::to_string(index) + " is outside 0 .. 2^30 - 1");
+    if (delay_num < 0 || delay_num > 65535 || delay_den < 0 || delay_den > 65535)
+        return !c->fail(fn + ": delay " + std::to_string(delay_num) + " / " + std::to_string(delay_den) + " is outside 0 .. 65535");
+    if (width < 1 || height < 1) return !c->fail(fn + ": width and height must be at least 1");
+    const int bpp = bits / 2;
+    const size_t bound = apng_frame_bound(width, height, bpp);
+    if (!bound) return !c->fail(fn + ": frame too large (its PNG could exceed 2^31 - 1 bytes)");
+    if (capacity < bound) return !c->fail(fn + ": capacity " + std::to_string(capacity) + " is below pe_apng_frame_bound = " + std::to_string(bound));
+    if (uintptr_t(frame) & uintptr_t(bpp - 1)) return !c->fail(fn + ": the frame must be " + std::to_string(bpp) + "-byte aligned");
+    return true;
+}
+
+int run_apng(pe_ctx* c, const char* fn, const void* frame, int width, int height, int bits, int index, int delay_num, int delay_den,
+             void* out, void* size_device, cudaStream_t s) {
+    const int bpp = bits / 2;
+    if (!cuda_ok(c, c->apng_work.ensure(apng_workspace_bytes(width, height, bpp)), "cudaMalloc(APNG work space)")) return 1;
+    return launched(c, launch_apng_frame(frame, width, height, bpp, index, delay_num, delay_den, c->apng_work.dev, out, size_device, s),
+                    fn, index ? 8 : 6) ? 0 : 1;
+}
+
 // The checks both forms of pe_encode_gif_frame make before anything is allocated or launched
 bool check_gif(pe_ctx* c, const std::string& fn, const void* frame, int width, int height, int delay_cs, size_t capacity) {
     if (!frame) return !c->fail(fn + ": null argument");
@@ -182,6 +210,37 @@ int pe_encode_png_rgba16(pe_ctx* c, const void* rgba16, int width, int height, v
 
 int pe_encode_png_host_rgba16(pe_ctx* c, const void* rgba16, int width, int height, uint8_t* png_host, size_t capacity, size_t* size_out) {
     return encode_png_host(c, "pe_encode_png_host_rgba16", 8, rgba16, width, height, png_host, capacity, size_out);
+}
+
+// ------------------------------------------------------------------------------ APNG frame blocks (pe_png.cu)
+size_t pe_apng_frame_bound(int width, int height, int bits) {
+    return bits == 8 || bits == 16 ? apng_frame_bound(width, height, bits / 2) : 0;
+}
+
+int pe_apng_header(int width, int height, int bits, uint32_t num_frames, uint32_t num_plays, uint8_t* out, size_t capacity) {
+    if (!out || capacity < 53 || !pe_apng_frame_bound(width, height, bits) || num_frames < 1 || num_frames > uint32_t(kApngMaxIndex) + 1 ||
+        num_plays > uint32_t(INT32_MAX)) return 0;
+    return int(apng_header(width, height, bits / 2, num_frames, num_plays, out));
+}
+
+int pe_encode_apng_frame(pe_ctx* c, const void* pixels, int width, int height, int bits, int index, int delay_num, int delay_den,
+                         void* out, size_t capacity, void* size_device, void* stream) {
+    if (!c) return 1;
+    const char* fn = "pe_encode_apng_frame";
+    if (!out || !size_device) return c->fail(std::string(fn) + ": null argument");
+    if (!check_apng(c, fn, pixels, width, height, bits, index, delay_num, delay_den, capacity) || !bind_device(c)) return 1;
+    return run_apng(c, fn, pixels, width, height, bits, index, delay_num, delay_den, out, size_device, stream_of(c, stream));
+}
+
+int pe_encode_apng_frame_host(pe_ctx* c, const void* pixels, int width, int height, int bits, int index, int delay_num, int delay_den,
+                              uint8_t* out_host, size_t capacity, size_t* size_out) {
+    if (!c) return 1;
+    const char* fn = "pe_encode_apng_frame_host";
+    if (!out_host || !size_out) return c->fail(std::string(fn) + ": null argument");
+    if (!check_apng(c, fn, pixels, width, height, bits, index, delay_num, delay_den, capacity)) return 1;
+    return encode_to_host(c, fn, apng_frame_bound(width, height, bits / 2), out_host, size_out, [&](void* block, void* size_device) {
+        return run_apng(c, fn, pixels, width, height, bits, index, delay_num, delay_den, block, size_device, c->stream);
+    });
 }
 
 // ------------------------------------------------------------------------------ GIF frame blocks (pe_gif.cu)

@@ -39,6 +39,21 @@ size_t png_workspace_bytes(int width, int height, int bpp);
 // Enqueue the five kernels: frame -> PNG file at `png` (capacity >= png_bound), its length in *(uint64*)size_out.
 int launch_png_encode(const void* rgba, int width, int height, int bpp, void* work, void* png, void* size_out, cudaStream_t s);
 
+// APNG frame blocks on the device (pe_png.cu; DESIGN.md section 5.8): the still file of launch_png_encode reframed as an fcTL
+// chunk and, for frame 0, its IDAT chunks or, for a later frame, one fdAT chunk of its whole zlib stream.
+// The largest frame index: the sequence numbers 2 k - 1 and 2 k stay below 2^31.
+constexpr int kApngMaxIndex = (1 << 30) - 1;
+// Upper bound of the block for a width x height frame; 0 when png_bound is 0.
+size_t apng_frame_bound(int width, int height, int bpp);
+// Bytes of device work space launch_apng_frame needs (the PNG work space, the still file and the CRC pieces).
+size_t apng_workspace_bytes(int width, int height, int bpp);
+// Signature, IHDR and acTL(num_frames, num_plays) into out[0 .. 53); returns 53.
+size_t apng_header(int width, int height, int bpp, uint32_t num_frames, uint32_t num_plays, uint8_t* out);
+// Enqueue the PNG kernels and the reframe (and, for index >= 1, the two CRC kernels): frame -> block at `block` (capacity >=
+// apng_frame_bound), its length in *(uint64*)size_out.  0 <= index <= 2^30 - 1, delays 0 .. 65535.
+int launch_apng_frame(const void* rgba, int width, int height, int bpp, int index, int delay_num, int delay_den, void* work, void* block,
+                      void* size_out, cudaStream_t s);
+
 // GIF frame blocks on the device (pe_gif.cu; the encoding is tests/host_harness/gif_spec.cpp, DESIGN.md section 5.6): the index
 // stream is LZW-coded in segments of kGifSegment indices, each with a fresh dictionary.
 constexpr size_t kGifSegment = 16384;

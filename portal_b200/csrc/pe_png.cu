@@ -13,8 +13,15 @@
 //                      checksum, IEND and the file's length
 //   pe_k_png_gather    one CTA per segment: its bytes to their place in the file, around the IDAT chunk headers
 //   pe_k_png_chunks    one thread per IDAT chunk: length, type and CRC-32
+//
+// An APNG frame block (pe_encode_apng_frame, DESIGN.md section 5.8) is the still file of these kernels reframed:
+//   pe_k_apng_reframe    one CTA per IDAT chunk: frame 0 copies the chunk, a later frame gathers its payload into one fdAT
+//   pe_k_apng_piece_crc  one thread per IDAT chunk: the CRC-32 of its payload
+//   pe_k_apng_crc        one CTA: the fdAT chunk's CRC-32 from the pieces' by a tree of CRC combines, its framing, the length
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <algorithm>
 
 #include "pe_kernels.h"
 
@@ -341,6 +348,105 @@ __global__ void __launch_bounds__(128) pe_k_png_chunks(const uint32_t* __restric
     put_be32(q + 8 + len, ~c);
 }
 
+// ---- APNG frame blocks (pe_encode_apng_frame; DESIGN.md section 5.8): the still file S of the kernels above, reframed.
+struct FcTL { uint8_t b[38]; };
+constexpr int kCombineThreads = 1024;
+
+// One CTA per IDAT chunk of S (grid from the bound; CTAs past the stream exit), and the fcTL chunk from CTA 0.  `fdat` 0 (frame
+// 0): the chunk as it is, so that the block is fcTL || S[33 : |S| - 12], and its length.  `fdat` 1: the chunk's payload to its
+// place in the one fdAT chunk's data, after the 12 bytes of fdAT length, type and sequence number (pe_k_apng_crc writes those).
+__global__ void __launch_bounds__(256) pe_k_apng_reframe(const uint8_t* __restrict__ png, const uint32_t* __restrict__ zlen, FcTL fc, int fdat,
+                                                         uint8_t* __restrict__ out, unsigned long long* __restrict__ size_out) {
+    const size_t z = *zlen, c = blockIdx.x;
+    if (c == 0 && threadIdx.x < 38) out[threadIdx.x] = fc.b[threadIdx.x];
+    if (c * kPngChunk >= z) return;
+    const uint32_t len = uint32_t(min(size_t(kPngChunk), z - c * kPngChunk));
+    const uint8_t* src = png + 33 + c * (kPngChunk + 12);
+    if (fdat) {
+        uint8_t* dst = out + 38 + 12 + c * kPngChunk;
+        for (uint32_t i = threadIdx.x; i < len; i += blockDim.x) dst[i] = src[8 + i];
+    } else {
+        uint8_t* dst = out + 38 + c * (kPngChunk + 12);
+        for (uint32_t i = threadIdx.x; i < len + 12; i += blockDim.x) dst[i] = src[i];
+        if (c == 0 && threadIdx.x == 0) *size_out = 38 + 12 * ((z + kPngChunk - 1) / kPngChunk) + z;
+    }
+}
+
+// One thread per kPngChunk piece of the zlib stream Z (the payload of one IDAT chunk of S): its standard CRC-32.
+__global__ void __launch_bounds__(128) pe_k_apng_piece_crc(const uint8_t* __restrict__ png, const uint32_t* __restrict__ zlen,
+                                                           uint32_t* __restrict__ piece) {
+    __shared__ uint32_t table[256];
+    for (int i = int(threadIdx.x); i < 256; i += blockDim.x) {
+        uint32_t c = uint32_t(i);
+        for (int k = 0; k < 8; k++) c = (c & 1u) ? 0xEDB88320u ^ (c >> 1) : c >> 1;
+        table[i] = c;
+    }
+    __syncthreads();
+    const size_t z = *zlen, k = size_t(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (k * kPngChunk >= z) return;
+    const uint32_t len = uint32_t(min(size_t(kPngChunk), z - k * kPngChunk));
+    const uint8_t* q = png + 33 + k * (kPngChunk + 12) + 8;
+    uint32_t c = 0xFFFFFFFFu;
+    for (uint32_t i = 0; i < len; i++) c = table[(c ^ q[i]) & 0xFFu] ^ (c >> 8);
+    piece[k] = ~c;
+}
+
+// a * b mod P in the reflected domain of CRC-32 (bit 31 is the coefficient of x^0)
+__device__ __forceinline__ uint32_t gf2_mul(uint32_t a, uint32_t b) {
+    uint32_t p = 0;
+    for (int i = 31; i >= 0; i--) {
+        if ((a >> i) & 1u) p ^= b;
+        b = (b & 1u) ? 0xEDB88320u ^ (b >> 1) : b >> 1;
+    }
+    return p;
+}
+
+// x^(8 n) mod P from sq[k] = x^(2^k) mod P: one product per set bit of n
+__device__ __forceinline__ uint32_t x8n(const uint32_t* sq, size_t n) {
+    uint32_t p = 1u << 31;
+    for (int k = 3; n; n >>= 1, k++)
+        if (n & 1) p = gf2_mul(sq[k], p);
+    return p;
+}
+
+// One CTA: the CRC of "fdAT" || sequence number || Z from `prefix` (the CRC of the first 8 bytes) and the pieces', by zlib's
+// combine crc(A || B) = crc(A) x^(8 |B|) mod P xor crc(B).  Each pass takes kCombineThreads pieces through a log-depth tree
+// and folds the result into the running CRC.  Then the fdAT chunk's length, type, sequence number and CRC, and the length last.
+__global__ void __launch_bounds__(kCombineThreads) pe_k_apng_crc(const uint32_t* __restrict__ zlen, const uint32_t* __restrict__ piece, uint32_t prefix,
+                                                                 uint32_t seq, uint8_t* __restrict__ out, unsigned long long* __restrict__ size_out) {
+    __shared__ uint32_t sq[64], crc[kCombineThreads], carry;
+    const int tid = int(threadIdx.x);
+    if (tid == 0) {
+        uint32_t v = 1u << 30;                                    // x^1
+        for (int k = 0; k < 64; k++) { sq[k] = v; v = gf2_mul(v, v); }
+        carry = prefix;
+    }
+    const size_t z = *zlen, n = (z + kPngChunk - 1) / kPngChunk;
+    for (size_t base = 0; base < n; base += kCombineThreads) {
+        crc[tid] = base + tid < n ? piece[base + tid] : 0u;
+        __syncthreads();
+        // stride s: entry t (a multiple of 2 s) covers pieces [t, t + s) of the pass and takes in [t + s, t + 2 s)
+        for (int s = 1; s < kCombineThreads; s <<= 1) {
+            const size_t right = base + size_t(tid) + size_t(s);
+            if ((tid & (2 * s - 1)) == 0 && right < n) {
+                const size_t len = min(z, (right + size_t(s)) * kPngChunk) - right * kPngChunk;
+                crc[tid] = gf2_mul(x8n(sq, len), crc[tid]) ^ crc[tid + s];
+            }
+            __syncthreads();
+        }
+        if (tid == 0) carry = gf2_mul(x8n(sq, min(z, (base + kCombineThreads) * kPngChunk) - base * kPngChunk), carry) ^ crc[0];
+        __syncthreads();
+    }
+    if (tid == 0) {
+        uint8_t* q = out + 38;
+        put_be32(q, uint32_t(z + 4));
+        q[4] = 'f'; q[5] = 'd'; q[6] = 'A'; q[7] = 'T';
+        put_be32(q + 8, seq);
+        put_be32(q + 12 + z, carry);
+        *size_out = 38 + 12 + z + 4;
+    }
+}
+
 uint32_t host_crc32(const uint8_t* d, size_t n) {
     uint32_t c = 0xFFFFFFFFu;
     for (size_t i = 0; i < n; i++) {
@@ -348,6 +454,35 @@ uint32_t host_crc32(const uint8_t* d, size_t n) {
         for (int k = 0; k < 8; k++) c = (c & 1u) ? 0xEDB88320u ^ (c >> 1) : c >> 1;
     }
     return ~c;
+}
+
+// A chunk of `n` data bytes at p: length, type, the data (already at p + 8) and the CRC of type and data
+void host_chunk(uint8_t* p, const char* type, uint32_t n) {
+    for (int k = 0; k < 4; k++) {
+        p[k] = uint8_t(n >> (24 - 8 * k));
+        p[4 + k] = uint8_t(type[k]);
+    }
+    const uint32_t crc = host_crc32(p + 4, size_t(n) + 4);
+    for (int k = 0; k < 4; k++) p[8 + n + k] = uint8_t(crc >> (24 - 8 * k));
+}
+
+void host_be32(uint8_t* p, uint32_t v) {
+    for (int k = 0; k < 4; k++) p[k] = uint8_t(v >> (24 - 8 * k));
+}
+
+// The PNG signature and IHDR of a width x height RGBA file at 2 bpp bits per sample: the first 33 bytes of every file
+PngHeader png_header(int width, int height, int bpp) {
+    PngHeader hdr;
+    const uint8_t sig[8] = {0x89, 'P', 'N', 'G', '\r', '\n', 0x1A, '\n'};
+    for (int k = 0; k < 8; k++) hdr.b[k] = sig[k];
+    uint8_t* ihdr = hdr.b + 8;                                     // length, type, 13 bytes of data, CRC
+    host_be32(ihdr + 8, uint32_t(width));
+    host_be32(ihdr + 12, uint32_t(height));
+    ihdr[16] = uint8_t(2 * bpp);                                   // bit depth: 8 or 16
+    ihdr[17] = 6;                                                  // RGBA
+    ihdr[18] = ihdr[19] = ihdr[20] = 0;
+    host_chunk(ihdr, "IHDR", 13);
+    return hdr;
 }
 
 struct Layout {
@@ -391,21 +526,7 @@ int launch_png_encode(const void* rgba, int width, int height, int bpp, void* wo
     uint32_t* meta = reinterpret_cast<uint32_t*>(w + L.meta);
     uint32_t* offs = reinterpret_cast<uint32_t*>(w + L.offs);
     uint32_t* zlen = reinterpret_cast<uint32_t*>(w + L.zlen);
-    PngHeader hdr;
-    const uint8_t sig[8] = {0x89, 'P', 'N', 'G', '\r', '\n', 0x1A, '\n'};
-    for (int k = 0; k < 8; k++) hdr.b[k] = sig[k];
-    uint8_t* ihdr = hdr.b + 8;                                     // length, type, 13 bytes of data, CRC
-    const uint8_t fixed[8] = {0, 0, 0, 13, 'I', 'H', 'D', 'R'};
-    for (int k = 0; k < 8; k++) ihdr[k] = fixed[k];
-    for (int k = 0; k < 4; k++) {
-        ihdr[8 + k] = uint8_t(uint32_t(width) >> (24 - 8 * k));
-        ihdr[12 + k] = uint8_t(uint32_t(height) >> (24 - 8 * k));
-    }
-    ihdr[16] = uint8_t(2 * bpp);                                   // bit depth: 8 or 16
-    ihdr[17] = 6;                                                  // RGBA
-    ihdr[18] = ihdr[19] = ihdr[20] = 0;
-    const uint32_t crc = host_crc32(ihdr + 4, 17);
-    for (int k = 0; k < 4; k++) ihdr[21 + k] = uint8_t(crc >> (24 - 8 * k));
+    const PngHeader hdr = png_header(width, height, bpp);
 
     cudaError_t e = cudaFuncSetAttribute(pe_k_png_deflate, cudaFuncAttributeMaxDynamicSharedMemorySize, int(kDeflateSmem));
     if (e != cudaSuccess) return int(e);
@@ -416,6 +537,64 @@ int launch_png_encode(const void* rgba, int width, int height, int bpp, void* wo
     pe_k_png_gather<<<unsigned(L.n_seg), 256, 0, s>>>(staging, meta, offs, static_cast<uint8_t*>(png));
     const size_t max_chunks = (png_bound(width, height, bpp) + kPngChunk - 1) / kPngChunk;
     pe_k_png_chunks<<<unsigned((max_chunks + 127) / 128), 128, 0, s>>>(zlen, static_cast<uint8_t*>(png));
+    return int(cudaGetLastError());
+}
+
+size_t apng_frame_bound(int width, int height, int bpp) {
+    const size_t bound = png_bound(width, height, bpp);
+    if (!bound) return 0;
+    const size_t z = bound - 45 - 12 * ((bound - 45 + kPngChunk + 11) / (kPngChunk + 12));   // the longest zlib stream
+    return std::max(38 + bound - 45, 38 + 12 + z + 4);
+}
+
+// [PNG work space | the still file | its length | one CRC per IDAT chunk]
+static size_t apng_file_offset(int width, int height, int bpp) { return (png_workspace_bytes(width, height, bpp) + 255) & ~size_t(255); }
+static size_t apng_size_offset(int width, int height, int bpp) { return apng_file_offset(width, height, bpp) + ((png_bound(width, height, bpp) + 255) & ~size_t(255)); }
+
+size_t apng_workspace_bytes(int width, int height, int bpp) {
+    return apng_size_offset(width, height, bpp) + 256 + 4 * ((png_bound(width, height, bpp) + kPngChunk - 1) / kPngChunk);
+}
+
+size_t apng_header(int width, int height, int bpp, uint32_t num_frames, uint32_t num_plays, uint8_t* out) {
+    const PngHeader hdr = png_header(width, height, bpp);
+    for (int k = 0; k < 33; k++) out[k] = hdr.b[k];
+    host_be32(out + 33 + 8, num_frames);
+    host_be32(out + 33 + 12, num_plays);
+    host_chunk(out + 33, "acTL", 8);
+    return 53;
+}
+
+int launch_apng_frame(const void* rgba, int width, int height, int bpp, int index, int delay_num, int delay_den, void* work, void* block,
+                      void* size_out, cudaStream_t s) {
+    const Layout L = layout(width, height, bpp);
+    uint8_t* w = static_cast<uint8_t*>(work);
+    uint8_t* png = w + apng_file_offset(width, height, bpp);
+    void* png_size = w + apng_size_offset(width, height, bpp);
+    uint32_t* piece = reinterpret_cast<uint32_t*>(w + apng_size_offset(width, height, bpp) + 256);
+    const uint32_t* zlen = reinterpret_cast<const uint32_t*>(w + L.zlen);
+    const int rc = launch_png_encode(rgba, width, height, bpp, work, png, png_size, s);
+    if (rc) return rc;
+    FcTL fc;                                                       // sequence number 2k - 1 (0 for frame 0), full frame at 0, 0
+    host_be32(fc.b + 8, index ? uint32_t(2 * index - 1) : 0u);
+    host_be32(fc.b + 12, uint32_t(width));
+    host_be32(fc.b + 16, uint32_t(height));
+    host_be32(fc.b + 20, 0);
+    host_be32(fc.b + 24, 0);
+    fc.b[28] = uint8_t(delay_num >> 8); fc.b[29] = uint8_t(delay_num);
+    fc.b[30] = uint8_t(delay_den >> 8); fc.b[31] = uint8_t(delay_den);
+    fc.b[32] = 0;                                                  // dispose_op NONE
+    fc.b[33] = 0;                                                  // blend_op SOURCE
+    host_chunk(fc.b, "fcTL", 26);
+    uint8_t* out = static_cast<uint8_t*>(block);
+    auto* size = static_cast<unsigned long long*>(size_out);
+    const size_t max_chunks = (png_bound(width, height, bpp) + kPngChunk - 1) / kPngChunk;
+    pe_k_apng_reframe<<<unsigned(max_chunks), 256, 0, s>>>(png, zlen, fc, index ? 1 : 0, out, size);
+    if (index) {
+        uint8_t prefix[8] = {'f', 'd', 'A', 'T'};
+        host_be32(prefix + 4, uint32_t(2 * index));
+        pe_k_apng_piece_crc<<<unsigned((max_chunks + 127) / 128), 128, 0, s>>>(png, zlen, piece);
+        pe_k_apng_crc<<<1, kCombineThreads, 0, s>>>(zlen, piece, host_crc32(prefix, 8), uint32_t(2 * index), out, size);
+    }
     return int(cudaGetLastError());
 }
 

@@ -308,6 +308,10 @@ class HostPlayer:
         mb = (frame_index, frame_count, motion_blur_frames, float(duration_seconds))
         return self._render(capi.PH_OUT_GIF, 8, width, height, depth, aa_count, motion_blur=mb).tobytes()
 
+    def set_apng_frame(self, index: int, delay_num: int, delay_den: int):
+        """The frame index and the fcTL delay (delay_num / delay_den seconds) of the next APNG frame blocks."""
+        self._check(self._lib.ph_player_set_apng_frame(self._p, int(index), int(delay_num), int(delay_den)))
+
     def set_jpeg_quality(self, quality: int):
         """The quality (1 .. 100; 90 by default) of the next JPEG frames."""
         self._check(self._lib.ph_player_set_jpeg_quality(self._p, int(quality)))
