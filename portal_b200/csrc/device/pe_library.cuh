@@ -98,10 +98,10 @@ PE_FI vec3 get_normal(const M& matrix) {
 
 PE_FI Ray normalize_ray(Ray r) {  // library.glsl:108-113
     float len = length(r.d);
-    // `r.d /= len` = r.d * (1 / len) component by component (pe_glsl.cuh); a direction's w stays the exact zero it is
-    // (0 * (1 / len) is a zero for every len but 0 and NaN, and then x, y, z are NaN already)
-    const float inv = 1.0f / len;
-    r.d = vec4(r.d.x * inv, r.d.y * inv, r.d.z * inv, (r.d.w == 0.0f) ? 0.0f : r.d.w * inv);
+    // `r.d /= len` = r.d * (1 / len) component by component (pe_glsl.cuh), w included: a w of -0 stays -0, and when the
+    // squared length underflows to 0 (or is NaN) w becomes 0 * inf = NaN, as in GLSL.  A scene's own code may read r.d.w.
+    // The ray loop does not need w kept at +0: bounce_once tests `w == 0` again at the next bounce (pe_kernel.cuh).
+    r.d = r.d * (1.0f / len);
     r.tmul /= len;
     return r;
 }

@@ -29,9 +29,10 @@ def nvrtc_library():
     return os.path.join(cuda, "lib64", "libnvrtc.so.12")
 
 
-def compile_probe(options=None, include_dir=None, source=PROBE_SRC, extra=()):
+def compile_probe(options=None, include_dir=None, source=PROBE_SRC, extra=(), want_log=False):
     """A probe source (glsl_probe.cu by default) -> sm_90a cubin bytes (options: OPTIONS; include_dir: the product's device
-    headers; extra: further options of this probe, such as its own include directory or a -D)."""
+    headers; extra: further options of this probe, such as its own include directory or a -D).  want_log: return
+    (cubin, NVRTC's log) instead."""
     nv = C.CDLL(nvrtc_library())
     with open(source, "rb") as f:
         src = f.read()
@@ -50,7 +51,7 @@ def compile_probe(options=None, include_dir=None, source=PROBE_SRC, extra=()):
         nv.nvrtcGetCUBINSize(prog, C.byref(size))
         cubin = C.create_string_buffer(size.value)
         assert nv.nvrtcGetCUBIN(prog, cubin) == 0
-        return cubin.raw
+        return (cubin.raw, log.value.decode(errors="replace")) if want_log else cubin.raw
     finally:
         nv.nvrtcDestroyProgram(C.byref(prog))
 

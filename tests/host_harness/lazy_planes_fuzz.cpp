@@ -7,7 +7,9 @@
 // both signs, denormals, huge values, Inf, NaN, candidates within a few ulp of the current best hit), with the
 // full-chain matrix type (cmat4) and with structure-specialised ones (smat4<Z,O>).  x86-64 float arithmetic is
 // IEEE like the GPU's (-ffp-contract=off, no fast-math), so the comparison is meaningful bit for bit.
-// Built and run by tests/test_lazy_planes_host.py; prints "cases N mismatches M".
+// Built and run by tests/test_lazy_planes_host.py; prints "cases N mismatches M".  `lazy_planes_fuzz N cases.bin` also writes
+// every case it checks as a record of tests/gpu_probe/library_probe.cu (tests/test_library_probe.py replays them there, on
+// the host and through NVRTC on the device).
 #include <math.h>
 
 #include <cmath>
@@ -61,8 +63,28 @@ static bool same_bits(float a, float b) { return __float_as_int(a) == __float_as
 
 static long long cases = 0, mismatches = 0, accepted = 0, early = 0;
 
+// library_probe.cu's record: function id (its lazy-plane entry for the matrix type), then 40 floats of arguments
+static FILE* dump = nullptr;
+template <class M> struct probe_fn;
+template <> struct probe_fn<cmat4> { static constexpr int id = 8; };
+template <> struct probe_fn<smat4<0x0888u, 0x8000u>> { static constexpr int id = 29; };
+template <> struct probe_fn<smat4<0x0BDEu, 0x8421u>> { static constexpr int id = 30; };
+static const cmat4& matrix_of(const cmat4& m) { return m; }
+template <unsigned Z, unsigned O, unsigned F> static const cmat4& matrix_of(const smat4<Z, O, F>& m) { return m.m; }
+template <class M>
+static void dump_case(const SurfaceIntersection& best, const Ray& r, const M& m, vec3 n) {
+    float rec[40] = {r.o.x, r.o.y, r.o.z, r.o.w, r.d.x, r.d.y, r.d.z, r.d.w, r.tmul, r.in_subspace ? 1.0f : 0.0f, n.x, n.y, n.z};
+    std::memcpy(rec + 20, matrix_of(m).e, sizeof(float) * 16);
+    rec[36] = best.hit ? 1.0f : 0.0f;
+    rec[37] = best.t;
+    const int id = probe_fn<M>::id;
+    std::fwrite(&id, 4, 1, dump);
+    std::fwrite(rec, 4, 40, dump);
+}
+
 template <class M>
 static void check(const SurfaceIntersection& best, const Ray& r, const M& m, vec3 n) {
+    if (dump) dump_case(best, r, m, n);
     bool f1 = false, f2 = false;
     const SurfaceIntersection a = plane_intersect_pre(r, m, n, f1);
     const SurfaceIntersection b = plane_intersect_lazy(best, r, m, n, f2);
@@ -85,6 +107,7 @@ static void check(const SurfaceIntersection& best, const Ray& r, const M& m, vec
 
 int main(int argc, char** argv) {
     const long long n = argc > 1 ? std::atoll(argv[1]) : 2000000;
+    if (argc > 2 && !(dump = std::fopen(argv[2], "wb"))) return 2;
     cmat4 M;
     for (long long it = 0; it < n; it++) {
         const unsigned mode = unsigned(rnd() % 8);
@@ -130,5 +153,6 @@ int main(int argc, char** argv) {
         }
     }
     std::printf("cases %lld mismatches %lld accepted %lld early_exits %lld\n", cases, mismatches, accepted, early);
+    if (dump) std::fclose(dump);
     return mismatches ? 1 : 0;
 }
